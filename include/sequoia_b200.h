@@ -103,6 +103,11 @@ int sq_attn_plan_create(sq_attn_plan** plan, const sq_half* q, int ld, int n_max
 int sq_attn_plan_destroy(sq_attn_plan* plan);
 /* Synchronous: returns the watchdog word of the plan (0 = no tensor-core / TMA wait ever timed out). */
 int sq_attn_plan_error(sq_attn_plan* plan);
+/* Launch shape of the plan: gp = query heads packed into one 128-row tile; splits = KV splits per cluster (Z) of the last
+ * tensor-core launch (0 before the first).  Z comes from the SM count, or from the environment variable SQ_ATTN_SPLITS
+ * read at plan creation (tuning / tests); either way it is clamped to 8, to the cache's KV tiles and, for calls without
+ * a state array, to the tiles of kv_end. */
+int sq_attn_plan_info(sq_attn_plan* plan, int* gp, int* splits);
 /* Debug: with SQ_ATTN_TIMING=1 the kernel records clock64() phase stamps of CTA (head 0, q tile 0, split s) at
  * host_out[s*16 + k] (128 values); SQ_ERR_UNSUPPORTED otherwise. */
 int sq_attn_plan_debug_times(sq_attn_plan* plan, long long* host_out);
@@ -278,7 +283,8 @@ int sq_tp_ll_consume(const void* mbox_local, int cap_words, uint32_t* epoch, uin
 
 /* ---- fused draft forward (csrc/sq_draft.cu): one persistent cooperative kernel per tree level for small draft models
  * (Engine/Engine.py:158-164 replays a ~25-kernel graph per level; Tree/SpecTree.py:245-259).  Supported: head_dim 64,
- * n_heads * 64 == hidden, no GQA, intermediate %% hidden == 0, <= 16 layers, max_length <= 512 (see sq_draft_supported).
+ * n_heads * 64 == hidden, no GQA, intermediate %% hidden == 0, <= 16 layers, max_length <= 640 (the attention phase keeps
+ * a head's K and V in shared memory; see sq_draft_supported).
  * layer_weights: 6 pointers per layer {wqkv (3h,h), wo (h,h), wgu (2I,h), wd (h,I), input_layernorm, post_attention_layernorm}.
  * workspace: sq_draft_workspace_bytes(hidden, intermediate) bytes of device memory owned by the caller. ---- */
 typedef struct sq_draft_plan sq_draft_plan;

@@ -35,6 +35,7 @@ _SIGNATURES = {
     "sq_attn_plan_create": (i32, [C.POINTER(vp), vp, i32, i32, i32, i32, i32, vp, vp, i32, i32, vp, vp, i64]),
     "sq_attn_plan_destroy": (i32, [vp]),
     "sq_attn_plan_error": (i32, [vp]),
+    "sq_attn_plan_info": (i32, [vp, C.POINTER(i32), C.POINTER(i32)]),
     "sq_attn_plan_debug_times": (i32, [vp, vp]),
     "sq_tree_attn": (i32, [vp, i32, i32, vp, i32, i32, i32, vp, i64, vp, i32, i32, i32, vp]),
     "sq_softmax_T": (i32, [vp, i64, vp, i64, i32, i32, f32, vp]),

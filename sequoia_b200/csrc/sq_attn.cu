@@ -27,6 +27,8 @@ struct sq_attn_plan {
   const __half* v_cache;
   __half* out;
   int splits_max;
+  int splits_force;   // SQ_ATTN_SPLITS (tuning / tests): KV splits per cluster instead of the SM-count heuristic; 0 = off
+  int last_splits;    // KV splits (Z) of the last tensor-core launch
   int GP;         // query heads packed into one MMA tile (H/Hkv when that divides 128, else 1)
   int pdl;        // launch with programmatic stream serialization (SQ_PDL=1)
   int debug_flags;
@@ -565,6 +567,11 @@ extern "C" int sq_attn_plan_create(sq_attn_plan** plan, const sq_half* q, int ld
   }
   const char* dbg = getenv("SQ_ATTN_DEBUG");
   p->debug_flags = dbg ? atoi(dbg) : 0;
+  {
+    // "Z": replaces only the SM-count heuristic, the clamps below still apply (the GEMM's counterpart: SQ_GEMM_FORCE)
+    const char* zs = getenv("SQ_ATTN_SPLITS");
+    p->splits_force = zs ? atoi(zs) : 0;
+  }
   cudaMemset(workspace, 0, 256 + 8 * 16 * 8);
   {
     // Q as (D, H, rows): a (64, GP, 128/GP) box lands in shared memory as the packed 128-row tile
@@ -594,6 +601,13 @@ extern "C" int sq_attn_plan_destroy(sq_attn_plan* plan) {
 extern "C" int sq_attn_plan_debug_times(sq_attn_plan* plan, long long* host_out) {
   if (!plan->dbg) return SQ_ERR_UNSUPPORTED;
   cudaMemcpy(host_out, plan->dbg, 8 * 16 * sizeof(long long), cudaMemcpyDeviceToHost);
+  return SQ_OK;
+}
+
+extern "C" int sq_attn_plan_info(sq_attn_plan* plan, int* gp, int* splits) {
+  SQ_CHECK_ARG(plan != nullptr && gp != nullptr && splits != nullptr, "sq_attn_plan_info: null argument");
+  *gp = plan->GP;
+  *splits = plan->last_splits;
   return SQ_OK;
 }
 
@@ -629,9 +643,11 @@ static int launch_attn(sq_attn_plan* p, AttnArgs& a, int impl, cudaStream_t st) 
     cudaGetDevice(&dev);
     if (cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n_sm <= 0) n_sm = 132;
   }
-  int Z = std::max(1, std::min(8, n_sm / std::max(1, groups * q_tiles)));
+  int Z = p->splits_force > 0 ? p->splits_force : n_sm / std::max(1, groups * q_tiles);
+  Z = std::max(1, std::min(8, Z));
   Z = std::min(Z, p->splits_max);
   if (a.state == nullptr) Z = std::max(1, std::min(Z, (a.kv_end + TILE_KV - 1) / TILE_KV));
+  p->last_splits = Z;
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(groups, q_tiles, Z);
   cfg.blockDim = dim3(256);

@@ -312,7 +312,9 @@ static void pick_tiles(sq_gemm_plan* p) {
   const int kb = p->K / 64;
   const bool allow_split = p->epi == 0;                 // a fused epilogue needs the whole K sum in one CTA
   choose_tiles(p, allow_split);
-  const char* force = getenv("SQ_GEMM_FORCE");          // tuning / debugging: "bn,split,mc"
+  // tuning / tests: "bn,split,mc" (an illegal triple is ignored: check sq_gemm_plan_info).  The attention kernel's
+  // counterpart is SQ_ATTN_SPLITS (sq_attn.cu).
+  const char* force = getenv("SQ_GEMM_FORCE");
   if (force) {
     int fb = 0, fs = 0, fm = 1;
     const int nf = sscanf(force, "%d,%d,%d", &fb, &fs, &fm);

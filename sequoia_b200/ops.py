@@ -87,6 +87,12 @@ class AttnPlan:
     def error(self) -> int:
         return _lib.load().sq_attn_plan_error(self.handle)
 
+    def info(self):
+        """(query heads per 128-row tile, KV splits of the last tensor-core launch)"""
+        gp, z = C.c_int(), C.c_int()
+        check(_lib.load().sq_attn_plan_info(self.handle, C.byref(gp), C.byref(z)), "sq_attn_plan_info")
+        return gp.value, z.value
+
     def __del__(self):
         try:
             if self.handle:

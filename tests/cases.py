@@ -117,7 +117,16 @@ SWEEP_CASES = {
     "sweep_greedys_5x8": ("L40_growmaps/5x8-tree.pt", "greedys", "draft", "draft", 256, 57, 64, 3, 17),
 }
 
-_MODELS = {"draft": (CFG_DRAFT, DRAFT_SEED), "target": (CFG_TARGET, TARGET_SEED),
+# Every instantiation of gemm_tn_kernel<BN, STAGES, SPLIT, MC> that sq_gemm.cu's run_tile can launch, in table order.
+# test_gpu_kernels.py forces each one through SQ_GEMM_FORCE; test_cabi.py checks this list against the SQ_G(...) lines.
+GEMM_VARIANTS = [
+    (256, 4, 1, 1), (256, 4, 1, 2),
+    (192, 5, 1, 1), (192, 5, 1, 2),
+    (128, 6, 1, 1), (128, 6, 1, 2), (128, 4, 2, 1), (128, 4, 4, 1), (128, 4, 2, 2), (128, 4, 4, 2),
+    (64, 8, 1, 1), (64, 8, 1, 2), (64, 4, 2, 1), (64, 4, 4, 1), (64, 4, 2, 2), (64, 4, 4, 2),
+]
+
+_MODELS = {"draft":(CFG_DRAFT, DRAFT_SEED), "target": (CFG_TARGET, TARGET_SEED),
            "target_gqa": (CFG_TARGET_GQA, GQA_SEED)}
 _wcache = {}
 

@@ -64,6 +64,27 @@ def test_reference_module_paths_and_signatures():
         assert hasattr(KV_Cache, m)
 
 
+def test_gemm_dispatch_table_is_swept():
+    """Every gemm_tn_kernel instantiation run_tile can launch is in the GPU variant sweep (cases.GEMM_VARIANTS), so a
+    variant added to the table cannot go untested.  (The sweep also checks that each forced plan records the table's
+    stage count.)"""
+    import cases
+    src = open(os.path.join(ROOT, "sequoia_b200", "csrc", "sq_gemm.cu")).read()
+    body = src[src.index("static int run_tile("):]
+    body = body[:body.index("#undef SQ_G")]
+    table = [tuple(int(x) for x in m) for m in re.findall(r"\bSQ_G\(\s*(\d+),\s*(\d+),\s*(\d+),\s*(\d+)\s*\)", body)]
+    assert len(table) == 16, table
+    assert table == cases.GEMM_VARIANTS
+
+
+def test_draft_attention_max_length_limit():
+    """The draft kernel keeps the whole K/V of a head in shared memory: for the 68m draft shape (h = 768, 12 heads of 64,
+    2 layers) 640 is the longest max_length that fits, and 672 (the next multiple of 32) must be refused."""
+    from sequoia_b200 import ops
+    assert ops.draft_supported(768, 3072, 2, 12, 12, 64, 32000, 640)
+    assert not ops.draft_supported(768, 3072, 2, 12, 12, 64, 32000, 672)
+
+
 def test_product_never_imports_oracle():
     for dirpath, _, files in os.walk(os.path.join(ROOT, "sequoia_b200")):
         for f in files:

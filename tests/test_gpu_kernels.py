@@ -1,6 +1,7 @@
 """GPU parity tests: every kernel of libsequoia_b200.so (called through the C ABI via sequoia_b200.ops) against
 the CPU oracle / golden vectors on the same seeded inputs.  Integer / index / byte results must be bit-exact;
 floating-point results within the tolerance written next to each assert."""
+import contextlib
 import math
 import os
 
@@ -294,16 +295,45 @@ def test_top_p_filter_ties_rank_by_index():
 
 # ------------------------------------------------------------------------------------------------ attention
 def _attn_reference(q, kc, vc, vis, H, Hkv, D):
-    """fp32 reference: q (n,H,D), kc/vc (Hkv,kv,D), vis (n,kv) bool."""
-    n = q.shape[0]
-    out = torch.zeros(n, H, D)
+    """float64 reference on the device: q (n,H,D), kc/vc (Hkv,kv,D), vis (n,kv) bool.  Returns (out, tol, p): the exact
+    output (n,H,D), the per-element error bound of an fp16 kernel (`_attn_tol`) and the probabilities (H,n,kv)."""
+    q, kc, vc, vis = (t.to(DEV) for t in (q, kc, vc, vis))
     rep = H // Hkv
-    for h in range(H):
-        s = (q[:, h].float() @ kc[h // rep].float().t()) / math.sqrt(D)
-        s = s.masked_fill(~vis, float("-inf"))
-        p = torch.softmax(s, dim=-1)
-        out[:, h] = p @ vc[h // rep].float()
-    return out
+    q64 = q.double()
+    k64 = kc.double().repeat_interleave(rep, 0)                         # (H, kv, D): head h reads kv head h // rep
+    v64 = vc.double().repeat_interleave(rep, 0)
+    s = torch.einsum("nhd,hkd->hnk", q64, k64) / math.sqrt(D)
+    p = torch.softmax(s.masked_fill(~vis[None], float("-inf")), dim=-1)
+    out = torch.einsum("hnk,hkd->nhd", p, v64)
+    wabs = torch.einsum("hnk,hkd->nhd", p, v64.abs())                   # sum_i p_i |v_i|
+    # fp32 score error of an fp16 x fp16 -> fp32 dot product of D terms: <= D 2^-24 sum_d |q_d k_d| (scaled like s)
+    sabs = torch.einsum("nhd,hkd->hnk", q64.abs(), k64.abs()) / math.sqrt(D)
+    eps_s = D * 2.0 ** -24 * sabs.masked_fill(~vis[None], 0).amax(-1)   # (H, n)
+    vmax = vc.double().abs().max()
+    return out, _attn_tol(wabs, eps_s.permute(1, 0).unsqueeze(-1), vis.shape[1], vmax), p
+
+
+def _attn_tol(wabs, eps_s, kv_len, vmax):
+    """|kernel - exact| bound per output element, in units of wabs = sum_i p_i |v_i| (p normalised):
+      3 x 2^-11 wabs   three fp16 roundings of a weighted sum of the v_i: P (relative 2^-11 per term), the split's
+                       normalised partial row O_s / l_s (its split-weighted sum is again wabs) and the output (|out| <= wabs);
+      2^-16 wabs       fp32 exp2 / max-subtraction rounding of each p_i;
+      2 eps_s wabs     an fp32 score error eps_s moves p_i by a factor exp(+-eps_s); normalised, the output moves by at most
+                       2 eps_s wabs;
+      kv 2^-25 vmax    P entries below 2^-14 of the reference maximum are fp16 subnormals (absolute error 2^-25 each), and
+                       the row sum they are divided by is >= 1."""
+    return (3 * 2.0 ** -11 + 2.0 ** -16 + 2 * eps_s) * wabs + kv_len * 2.0 ** -25 * vmax
+
+
+def _tree_vis(slots, kv_len, P, tmask):
+    """The structured mask of include/sequoia_b200.h on the device: key c is visible from row slot s iff c <= min(s, P-1)
+    or (s >= P and c >= P-1 and tree bit (s-(P-1), c-(P-1)) of the (S,S) ancestor-or-self matrix `tmask`)."""
+    S = tmask.shape[0]
+    s = slots.to(DEV).view(-1, 1)
+    c = torch.arange(kv_len, device=DEV).view(1, -1)
+    node, col = s - (P - 1), c - (P - 1)
+    inside = (s >= P) & (col >= 0) & (node < S) & (col < S)
+    return (c <= s.clamp(max=P - 1)) | (inside & tmask[node.clamp(0, S - 1), col.clamp(0, S - 1)])
 
 
 @pytest.mark.parametrize("D,H,Hkv,M,P,gm,mode", [
@@ -352,7 +382,8 @@ def test_tree_attention(D, H, Hkv, M, P, gm, mode, impl):
     bits = pack_tree_mask(grow["mask"]).to(DEV)
     state = torch.zeros(16, dtype=torch.int32, device=DEV)
     state[0] = P
-    ref = _attn_reference(qkv[:n, :H * D].view(n, H, D), kc[layer, 0, :, :kv_len], vc[layer, 0, :, :kv_len], vis, H, Hkv, D)
+    ref = _attn_reference(qkv[:n, :H * D].view(n, H, D), kc[layer, 0, :, :kv_len], vc[layer, 0, :, :kv_len], vis, H, Hkv,
+                          D)[0].float().cpu()
     # structured mask
     sops.tree_attn(plan, layer, n, state=state if use_state else None, n0=n0, kv_end=kv_end, prefix_len=P,
                    tree_bits=bits, tree_words=bits.shape[1], tree_size=S, impl=impl)
@@ -406,7 +437,8 @@ def test_tree_attention_long_kv_and_lazy_rescale(D, H, Hkv, M, P, boost):
     bits = pack_tree_mask(grow["mask"]).to(DEV)
     state = torch.zeros(16, dtype=torch.int32, device=DEV)
     state[0] = P
-    ref = _attn_reference(qkv[:S, :H * D].view(S, H, D), kc[layer, 0, :, :kv_len], vc[layer, 0, :, :kv_len], vis, H, Hkv, D)
+    ref = _attn_reference(qkv[:S, :H * D].view(S, H, D), kc[layer, 0, :, :kv_len], vc[layer, 0, :, :kv_len], vis, H, Hkv,
+                          D)[0].float().cpu()
     for impl in (1, 0):
         out.zero_()
         sops.tree_attn(plan, layer, S, state=state, n0=0, kv_end=S, prefix_len=P, tree_bits=bits, tree_words=bits.shape[1],
@@ -415,6 +447,173 @@ def test_tree_attention_long_kv_and_lazy_rescale(D, H, Hkv, M, P, boost):
         assert plan.error() == 0
         err = (out[:S].float().cpu().view(S, H, D) - ref).abs().max().item()
         assert err < 6e-3, f"impl {impl}: max abs err {err}"          # fp16 P (up to 2^8 under a stale maximum) and output
+
+
+SENT = -1000.0                 # canary: no attention output (|out| <= max |v|) or test GEMM output comes near it
+
+
+@contextlib.contextmanager
+def _env(**kv):
+    """Set environment variables (read by the C library at plan creation) for the duration of the block."""
+    old = {k: os.environ.get(k) for k in kv}
+    os.environ.update({k: str(v) for k, v in kv.items()})
+    try:
+        yield
+    finally:
+        for k, v in old.items():
+            if v is None:
+                os.environ.pop(k, None)
+            else:
+                os.environ[k] = v
+
+
+def _assert_within(got, ref, tol, what):
+    """every element finite and |got - ref| <= tol; returns the worst |got - ref| / tol"""
+    g = got.double()
+    assert bool(torch.isfinite(g).all()), f"{what}: non-finite outputs"
+    ratio = ((g - ref).abs() / tol).max().item()
+    nbad = int(((g - ref).abs() > tol).sum())
+    assert nbad == 0, f"{what}: {nbad}/{g.numel()} elements outside the bound (worst {ratio:.2f} x tol)"
+    return ratio
+
+
+def _negative_controls(got, q, kc, vc, vis, H, Hkv, D, tol, p, what):
+    """The tolerance `tol` must be able to see a real attention error (one case per sweep):
+      * drop the second 128-key tile (keys 128..255, visible to every row here) from the reference: at least half of the
+        (row, head) outputs must fall outside tol of it;
+      * hide from its row the one key with the largest softmax mass (asserted >= 1%): that row and head must fall outside."""
+    assert bool(vis[:, 128:256].all()), "the dropped tile must be visible to every row"
+    drop = vis.clone()
+    drop[:, 128:256] = False
+    wrong = _attn_reference(q, kc, vc, drop, H, Hkv, D)[0]
+    outside = ((got.double() - wrong).abs() > tol).any(-1)            # (n, H)
+    assert outside.float().mean().item() >= 0.5, f"{what}: a dropped 128-key tile is within tolerance for most rows"
+    h, r, c = (int(x) for x in torch.unravel_index(p.argmax(), p.shape))
+    assert p[h, r, c].item() >= 0.01, f"{what}: no key holds 1% of a row's mass ({p[h, r, c].item():.4f})"
+    hide = vis.clone()
+    hide[r, c] = False
+    wrong = _attn_reference(q, kc, vc, hide, H, Hkv, D)[0]
+    assert bool(((got[r, h].double() - wrong[r, h]).abs() > tol[r, h]).any()), \
+        f"{what}: hiding a key with {p[h, r, c].item():.3f} of row {r}'s mass stays within tolerance"
+
+
+_GM768 = "L40_growmaps/L40-CNN-7b-70b-stochastic.pt"   # 768-node tree: room for 129 tree rows in tree-relative addressing
+ATTN_LAYOUTS = [(4, 4), (8, 4), (8, 2), (8, 1), (16, 1), (12, 4)]   # (H, Hkv): GP = 1, 2, 4, 8, 16, and 1 with G = 3
+
+
+class _AttnRig:
+    """Caches, q rows and a plan with SQ_ATTN_SPLITS = Z for one head layout; runs one launch per call and checks it."""
+    M, L, LAYER, N_MAX = 1152, 2, 1, 160          # 9 KV tiles: Z = 8 is reachable with kv_end up to 1025 and beyond
+
+    def __init__(self, H, Hkv, D, Z, seed):
+        from sequoia_b200.tree import pack_tree_mask
+        g = torch.Generator(device=DEV).manual_seed(seed)
+        self.H, self.Hkv, self.D, self.Z = H, Hkv, D, Z
+        grow = cases.load_growmap(_GM768)
+        self.S = grow["size"]
+        self.tmask = grow["mask"].bool().to(DEV)
+        self.bits = pack_tree_mask(grow["mask"]).to(DEV)
+        self.kc = torch.randn(self.L, 1, Hkv, self.M, D, generator=g, device=DEV).to(F16)
+        self.vc = torch.randn(self.L, 1, Hkv, self.M, D, generator=g, device=DEV).to(F16)
+        self.qkv = torch.randn(self.N_MAX, (H + 2 * Hkv) * D, generator=g, device=DEV).to(F16)
+        self.out = torch.full((self.N_MAX, H * D), SENT, dtype=F16, device=DEV)
+        self.dense = torch.full((self.N_MAX, self.M + 64), O.FP16_MIN, dtype=F16, device=DEV)   # row pitch != kv_len
+        self.state = torch.zeros(16, dtype=torch.int32, device=DEV)
+        with _env(SQ_ATTN_SPLITS=Z):
+            self.plan = ops().AttnPlan(self.qkv, self.N_MAX, H, Hkv, D, self.kc, self.vc, self.out)
+        self.worst = 0.0
+
+    def rows(self, n, kv_len, mode, tree_rows=None):
+        """(slots of the n rows, P, n0, kv_end, state) of one call.  rel: tree nodes 0..n-1 (state-driven, tree-relative);
+        abs: the last n slots below kv_len, about half of them prefix rows (host-known P)."""
+        if mode == "rel":
+            tn = tree_rows or min(kv_len, max(n, 150))
+            P = kv_len - tn + 1
+            self.state[0] = P
+            return torch.arange(P - 1, P - 1 + n), P, 0, tn, self.state
+        tn = tree_rows or max(1, n // 2)
+        P = kv_len - tn + 1
+        return torch.arange(kv_len - n, kv_len), P, kv_len - n, kv_len, None
+
+    def check(self, n, kv_len, vis, want_z, what):
+        torch.cuda.synchronize()
+        assert self.plan.error() == 0, f"{what}: watchdog fired (code {self.plan.error()})"
+        gp, z = self.plan.info()
+        assert z == want_z, f"{what}: launched with Z = {z}, expected {want_z}"
+        H, Hkv, D, ly = self.H, self.Hkv, self.D, self.LAYER
+        ref, tol, p = _attn_reference(self.qkv[:n, :H * D].view(n, H, D), self.kc[ly, 0, :, :kv_len], self.vc[ly, 0, :, :kv_len],
+                                      vis, H, Hkv, D)
+        got = self.out[:n].view(n, H, D)
+        self.worst = max(self.worst, _assert_within(got, ref, tol, what))
+        assert bool((self.out[n:] == SENT).all()), f"{what}: output rows >= n were written"
+        return got, ref, tol, p
+
+    def run(self, n, kv_len, mode, tree_rows=None, masks=("tree", "dense")):
+        """Both masks on the same rows; returns the last (got, ref, tol, p, vis)."""
+        slots, P, n0, kv_end, state = self.rows(n, kv_len, mode, tree_rows)
+        vis = _tree_vis(slots, kv_len, P, self.tmask)
+        res = None
+        for mask in masks:
+            self.out.fill_(SENT)
+            what = f"Z={self.Z} H={self.H} Hkv={self.Hkv} D={self.D} {mask}/{mode} n={n} kv_len={kv_len}"
+            if mask == "tree":
+                ops().tree_attn(self.plan, self.LAYER, n, state=state, n0=n0, kv_end=kv_end, prefix_len=P, tree_bits=self.bits,
+                                tree_words=self.bits.shape[1], tree_size=self.S)
+                # host-known kv_end caps Z at its KV tiles; the state-driven launch is capped only by the cache's 9 tiles
+                want_z = self.Z if state is not None else min(self.Z, -(-kv_len // 128))
+            else:
+                self.dense.fill_(O.FP16_MIN)
+                self.dense[:n, :kv_len].masked_fill_(vis, 0.0)
+                ops().tree_attn(self.plan, self.LAYER, n, state=None, n0=0, kv_end=kv_len, prefix_len=0, dense_mask=self.dense,
+                                mask_ld=self.dense.stride(0))
+                want_z = min(self.Z, -(-kv_len // 128))
+            res = self.check(n, kv_len, vis, want_z, what) + (vis,)
+        return res
+
+
+@pytest.mark.parametrize("Z", range(1, 9))
+@pytest.mark.parametrize("H,Hkv", ATTN_LAYOUTS, ids=lambda v: str(v))
+def test_tree_attention_split_sweep(H, Hkv, Z):
+    """tree_attn_tc_kernel at every KV split count Z = 1..8 (forced through SQ_ATTN_SPLITS) against every head packing,
+    float64 reference.  Covering design: both masks in every case; D and the addressing mode alternate over (Z, layout) so
+    that every Z meets both head dims, both masks and both addressings, and every GP meets every Z.  Rows at the
+    warpgroup / tile boundaries (64, 65, 128, 129, RPT +- 1), kv_len = 128 Z - 1, 128 Z, 128 Z + 1, a launch whose splits
+    outnumber the active KV tiles, and keys boosted in the second tile of split 1 so that the lazy rescale fires there."""
+    i = ATTN_LAYOUTS.index((H, Hkv))
+    D = (64, 128)[(Z + i) % 2]
+    mode = ("rel", "abs")[(Z // 2 + i) % 2]
+    G = H // Hkv
+    GP = G if 128 % G == 0 else 1
+    RPT = 128 // GP
+    rig = _AttnRig(H, Hkv, D, Z, seed=1000 * Z + i)
+    assert rig.plan.info()[0] == GP
+    ns = sorted({1, 64, 65, 128, 129} | ({RPT - 1, RPT + 1} if GP > 1 else set()))
+    kvs = []
+    for j, n in enumerate(ns):
+        kv_len = max(128 * Z + j % 3 - 1, n)
+        kvs.append(kv_len)
+        rig.run(n, kv_len, mode)
+    if Z > 1:
+        # Z - 1 active KV tiles (state-driven: Z is not capped by kv_end): the last split has no tile
+        rig.run(64, 128 * (Z - 1) - 1, "rel", tree_rows=64, masks=("tree",))
+    # lazy rescale in a split other than the first: 9 active tiles, tps = ceil(9 / Z) per split; the keys of the second tile
+    # of split 1 (prefix keys, visible to every row) get 8x the magnitude, so that tile's row maximum jumps by ~2^20
+    tps = -(-9 // Z)
+    b = tps + 1 if Z > 1 else 5
+    rig.kc[rig.LAYER, 0, :, 128 * b:128 * b + 64] *= 8
+    rig.run(64, rig.M, "abs", tree_rows=32)
+    cases.log_line("variant_sweep.log", f"attention Z={Z} GP={GP} H={H} Hkv={Hkv} D={D} masks=tree,dense addressing={mode} "
+                   f"n={ns} kv_len={kvs} boosted_tile={b}: worst err/bound {rig.worst:.3f}")
+
+
+def test_tree_attention_sweep_tolerance_sees_errors():
+    """Negative controls for the split sweep's bound, on one of its cases (Z = 3, GP = 4, D = 128, absolute addressing)."""
+    rig = _AttnRig(8, 2, 128, 3, seed=77)
+    n, kv_len = 64, 3 * 128 + 1
+    got, ref, tol, p, vis = rig.run(n, kv_len, "abs", masks=("tree",))
+    ly = rig.LAYER
+    _negative_controls(got, rig.qkv[:n, :8 * 128].view(n, 8, 128), rig.kc[ly, 0, :, :kv_len], rig.vc[ly, 0, :, :kv_len], vis,
+                       8, 2, 128, tol, p, "tree attention Z=3")
 
 
 # ------------------------------------------------------------------------------------------------ accept walk
@@ -781,6 +980,138 @@ def test_gemm_fused_swiglu_epilogue_bit_exact(I, K, n, tiled):
     assert torch.equal(act2, want2), "interleaved silu_mul must equal the plain one on de-interleaved columns"
 
 
+def _fp16_ulp(x):
+    """spacing of fp16 at |x| (subnormal spacing 2^-24 below 2^-14), float64"""
+    return torch.pow(2.0, torch.floor(torch.log2(x.abs().clamp(min=2.0 ** -14))) - 10)
+
+
+def _gemm_reference(a, w):
+    """float64 A W^T on the device and the bound of an fp16-out GEMM with fp32 accumulation over K: 1 fp16 ulp of the
+    exact value (the final rounding, with the accumulated error allowed to move it across a rounding boundary) plus
+    K 2^-24 (|A| |W|^T) (fp32 accumulation of K products, any order or K split)."""
+    a64, w64 = a.double(), w.double()
+    ref = a64 @ w64.t()
+    return ref, _fp16_ulp(ref) + a.shape[1] * 2.0 ** -24 * (a64.abs() @ w64.abs().t())
+
+
+def _gemm_case(variant, tiled, N, K, seed):
+    """Forced plans of one variant for (N, K): a 128-row plan with its output at ldc = N + 64 in a 136-row buffer, and a
+    320-row plan run at an activation-row offset into an output override (more than 128 rows: two row tiles)."""
+    bn, stages, split, mc = variant
+    g = torch.Generator(device=DEV).manual_seed(seed)
+    a = (torch.randn(320, K, generator=g, device=DEV) * 0.5).to(F16)
+    w = (torch.randn(N, K, generator=g, device=DEV) * 0.05).to(F16)
+    err = torch.zeros(4, dtype=torch.int32, device=DEV)
+    c = torch.full((136, N + 64), SENT, dtype=F16, device=DEV)
+    c_big = torch.full((328, N + 64), SENT, dtype=F16, device=DEV)
+    with _env(SQ_GEMM_FORCE=f"{bn},{split},{mc}"):
+        plan = ops().GemmPlan(a[:128], w, c, err, tiled=tiled)
+        big = ops().GemmPlan(a, w, c_big, err, tiled=tiled)
+    # SQ_GEMM_FORCE ignores an illegal triple: the plan must report exactly the forced variant (info: stages + 100 * mc)
+    assert plan.info() == big.info() == (bn, split, stages + 100 * mc), f"forced {variant}, plan {plan.info()}"
+    return a, w, err, c, c_big, plan, big
+
+
+def _assert_canary(buf, n, N, what):
+    keep = torch.ones(buf.shape, dtype=torch.bool, device=buf.device)
+    keep[:n, :N] = False
+    assert bool((buf[keep] == SENT).all()), f"{what}: wrote outside rows [0, {n}) x columns [0, {N})"
+
+
+@pytest.mark.parametrize("tiled", [False, True], ids=["rowmajor", "tiled"])
+@pytest.mark.parametrize("variant", cases.GEMM_VARIANTS, ids=lambda v: "bn%d_st%d_sp%d_mc%d" % v)
+def test_gemm_variant_sweep(variant, tiled):
+    """Every gemm_tn_kernel instantiation of run_tile's table, forced through SQ_GEMM_FORCE, against a float64 reference:
+    N = 4 BN (even tile count, legal for every split / multicast) and, for split 1, a ragged N = 3 BN + 32; K with fewer
+    64-wide K blocks per split than ring stages (the ring never fills) and 2 STAGES + 1 (it wraps twice); n = 1, 63, 64,
+    65, 128 and 200 rows at activation row 37 into an output override.  Outputs sit in buffers wider (ldc = N + 64) and
+    taller than the written region, filled with a sentinel that must survive outside [:n, :N]."""
+    bn, stages, split, mc = variant
+    Ns = [4 * bn] + ([3 * bn + 32] if split == 1 else [])
+    Ks = [64 * split * (stages - 1), 64 * split * (2 * stages + 1)]
+    worst = 0.0
+    for N in Ns:
+        for K in Ks:
+            a, w, err, c, c_big, plan, big = _gemm_case(variant, tiled, N, K, seed=N + K)
+            ref, tol = _gemm_reference(a[:128], w)
+            for n in (1, 63, 64, 65, 128):
+                what = f"gemm {variant} {'tiled' if tiled else 'row-major'} N={N} K={K} n={n}"
+                c.fill_(SENT)
+                plan.run(n)
+                torch.cuda.synchronize()
+                assert err.tolist() == [0, 0, 0, 0], f"{what}: pipeline watchdog fired"
+                worst = max(worst, _assert_within(c[:n, :N], ref[:n], tol[:n], what))
+                _assert_canary(c, n, N, what)
+            n, row0 = 200, 37
+            out = torch.full((216, N + 64), SENT, dtype=F16, device=DEV)
+            big.run(n, a_row0=row0, out=out)
+            torch.cuda.synchronize()
+            what = f"gemm {variant} {'tiled' if tiled else 'row-major'} N={N} K={K} n={n} a_row0={row0}"
+            assert err.tolist() == [0, 0, 0, 0], f"{what}: pipeline watchdog fired"
+            ref, tol = _gemm_reference(a[row0:row0 + n], w)
+            worst = max(worst, _assert_within(out[:n, :N], ref, tol, what))
+            _assert_canary(out, n, N, what)
+            assert bool((c_big == SENT).all()), f"{what}: the plan's own buffer was written despite the output override"
+    cases.log_line("variant_sweep.log", f"gemm (BN,STAGES,SPLIT,MC)={variant} {'tiled' if tiled else 'row-major'} N={Ns} K={Ks} "
+                   f"n=[1,63,64,65,128,200@37]: worst err/bound {worst:.3f}")
+
+
+def test_gemm_sweep_tolerance_sees_a_dropped_k_block():
+    """Negative control for the sweep's bound, on one of its cases ((64, 4, 4, 2), N = 256, K = 2304, 128 rows): a
+    reference without the last 64-wide K block must be outside the bound for most outputs (that block adds a term of
+    standard deviation ~0.2 against a bound of ~6e-3)."""
+    variant = (64, 4, 4, 2)
+    N, K = 256, 64 * 4 * 9
+    a, w, err, c, _, plan, _ = _gemm_case(variant, False, N, K, seed=N + K)
+    plan.run(128)
+    torch.cuda.synchronize()
+    ref, tol = _gemm_reference(a[:128], w)
+    _assert_within(c[:128, :N], ref, tol, "gemm negative control (exact reference)")
+    wrong = ref - _gemm_reference(a[:128, K - 64:], w[:, K - 64:])[0]
+    frac = ((c[:128, :N].double() - wrong).abs() > tol).float().mean().item()
+    assert frac >= 0.9, f"only {frac:.2%} of the outputs see a dropped K block"
+
+
+@pytest.mark.parametrize("tiled", [False, True], ids=["rowmajor", "tiled"])
+@pytest.mark.parametrize("bn,stages,mc", [(v[0], v[1], v[3]) for v in cases.GEMM_VARIANTS if v[2] == 1],
+                         ids=lambda v: str(v))
+def test_gemm_swiglu_variant_sweep(bn, stages, mc, tiled):
+    """Fused SwiGLU epilogue at every split-1 (BN, MC), forced for both plans: with the same tile the fused output must be
+    bit-identical to the plain GEMM on [gate; up] followed by sq_silu_mul (same accumulators, same rounding points), and
+    that plain GEMM is within the float64 bound.  2I = 4 BN and the ragged 2I = 3 BN + 32; K as in the GEMM sweep."""
+    worst = 0.0
+    for two_i in (4 * bn, 3 * bn + 32):
+        I = two_i // 2
+        for K in (64 * (stages - 1), 64 * (2 * stages + 1)):
+            g = torch.Generator(device=DEV).manual_seed(two_i + K)
+            a = (torch.randn(128, K, generator=g, device=DEV) * 0.5).to(F16)
+            wg = (torch.randn(I, K, generator=g, device=DEV) * 0.05).to(F16)
+            wu = (torch.randn(I, K, generator=g, device=DEV) * 0.05).to(F16)
+            wcat = torch.cat([wg, wu], 0).contiguous()
+            err = torch.zeros(4, dtype=torch.int32, device=DEV)
+            act = torch.full((136, I + 64), SENT, dtype=F16, device=DEV)
+            gu = torch.zeros(128, 2 * I, dtype=F16, device=DEV)
+            want = torch.zeros(128, I, dtype=F16, device=DEV)
+            with _env(SQ_GEMM_FORCE=f"{bn},1,{mc}"):
+                fused = ops().GemmPlan(a, ops().interleave_gate_up(wg, wu), act, err, tiled=tiled, swiglu=True)
+                plain = ops().GemmPlan(a, wcat, gu, err)
+            assert fused.info() == plain.info() == (bn, 1, stages + 100 * mc), f"forced ({bn}, 1, {mc}): {fused.info()}"
+            ref, tol = _gemm_reference(a, wcat)
+            for n in (1, 64, 65, 128):
+                what = f"swiglu bn={bn} mc={mc} {'tiled' if tiled else 'row-major'} 2I={two_i} K={K} n={n}"
+                act.fill_(SENT)
+                fused.run(n)
+                plain.run(n)
+                ops().silu_mul(gu, want, n)
+                torch.cuda.synchronize()
+                assert err.tolist() == [0, 0, 0, 0], f"{what}: pipeline watchdog fired"
+                worst = max(worst, _assert_within(gu[:n], ref[:n], tol[:n], what + " (plain gate_up)"))
+                assert torch.equal(act[:n, :I], want[:n]), f"{what}: fused epilogue differs from GEMM + sq_silu_mul"
+                _assert_canary(act, n, I, what)
+    cases.log_line("variant_sweep.log", f"swiglu (BN,1,MC)=({bn},1,{mc}) {'tiled' if tiled else 'row-major'} "
+                   f"2I=[{4 * bn},{3 * bn + 32}] n=[1,64,65,128]: bit-identical, plain GEMM worst err/bound {worst:.3f}")
+
+
 # ------------------------------------------------------------------------------------------------ fused draft forward
 @pytest.mark.parametrize("mode", ["attn", "chain", "coop"])
 @pytest.mark.parametrize("hidden,inter,heads,layers,M", [(768, 3072, 12, 2, 384), (512, 1024, 8, 3, 256)])
@@ -867,3 +1198,96 @@ def test_fused_draft_forward_matches_multi_kernel_path(hidden, inter, heads, lay
         kerr = ((ka - kb).abs().amax(dim=-1) / ka.abs().amax(dim=-1).clamp(min=1e-3)).max().item()
         assert kerr < 4e-3, f"level n0={n0}: appended K rows differ by {kerr:.3e} of the row's max"
     _log(f"fused draft forward [{mode}] (h={hidden} I={inter} L={layers}): max rel logit diff vs the multi-kernel path {worst:.3e}")
+
+
+# ------------------------------------------------------------------------------------------------ draft attention phase
+@pytest.fixture(scope="module")
+def draft68m():
+    """LlamaRunner of the 68m draft shape (h = 768, 12 heads of 64, 2 layers) at the longest max_length the draft
+    attention phase supports (its K/V of a head live in shared memory)."""
+    from sequoia_b200.model import LlamaRunner
+    cfg = O.LlamaCfg(hidden_size=768, intermediate_size=3072, num_hidden_layers=2, num_attention_heads=12,
+                     num_key_value_heads=12, vocab_size=cases.V)
+    with _env(SQ_DRAFT_FUSED="0", SQ_DRAFT_ATTN="1"):
+        runner = LlamaRunner({"config": cfg, "state_dict": O.init_llama_weights(cfg, 68)}, 640, device=DEV)
+    assert runner.draft_plan is not None, "the draft attention phase must engage for the 68m shape at max_length 640"
+    g = torch.Generator(device=DEV).manual_seed(680)
+    runner.k_cache.copy_(torch.randn(runner.k_cache.shape, generator=g, device=DEV).to(F16))
+    runner.v_cache.copy_(torch.randn(runner.v_cache.shape, generator=g, device=DEV).to(F16))
+    return runner
+
+
+def _draft_attn_rows():
+    """(n0, n) of every level of the config-2 tree, the bonus-token row, and n = 1, 15, 16, 17, 33, 64 ending at node 127"""
+    gm = cases.load_growmap("A100_growmaps/68m_7b/growmaps/A100-CNN-68m-7b-stochastic.pt")
+    rows, first = [(0, 1)], 1
+    for br in gm["branches"][:-1]:
+        tb = int(sum(br))
+        rows.append((first, tb))
+        first += tb
+    return gm, rows + [(128 - n, n) for n in (1, 15, 16, 17, 33, 64)]
+
+
+def _draft_attn_run(runner, gm, bits, layer, n0, n, P, qkv, out, state):
+    H, D = 12, 64
+    kv_end = n0 + n
+    kv_len = P - 1 + kv_end
+    out.fill_(SENT)
+    state[0] = P
+    runner.draft_plan.attention(layer, n, qkv, out, state, n0, kv_end, bits, bits.shape[1], gm["size"])
+    torch.cuda.synchronize()
+    vis = _tree_vis(torch.arange(P - 1 + n0, P - 1 + n0 + n), kv_len, P, gm["mask"].bool().to(DEV))
+    ref, tol, p = _attn_reference(qkv[:n, :H * D].view(n, H, D), runner.k_cache[layer, 0, :, :kv_len],
+                                  runner.v_cache[layer, 0, :, :kv_len], vis, H, H, D)
+    return out[:n].view(n, H, D), ref, tol, p, vis, kv_len
+
+
+@pytest.mark.parametrize("P", [40, 200, 513])
+def test_draft_attention_phase_vs_float64(draft68m, P):
+    """sq_draft_attention (the default attention of every draft forward of <= 64 rows) against the float64 reference:
+    every level of the config-2 tree and n = 1, 15, 16, 17, 33, 64, in layers 0 and 1.  P = 40 keeps kv_len below 256
+    (one 32-key block per warp), 200 crosses it (the 8-warp round-robin wraps), 513 reaches kv_len = 640 = max_length;
+    most kv_len are not multiples of 32 (zero-padded last block).  In layer 1 the late prefix keys [P-65, P-33) are
+    boosted 8x: the running maximum jumps there and every earlier block of that warp is rescaled.  Rows n..63 of the
+    output buffer keep their sentinel.  Bound: _attn_tol (two fp16 roundings here -- P and the output -- within its three)."""
+    runner = draft68m
+    gm, rows = _draft_attn_rows()
+    from sequoia_b200.tree import pack_tree_mask
+    bits = pack_tree_mask(gm["mask"]).to(DEV)
+    g = torch.Generator(device=DEV).manual_seed(P)
+    qkv = torch.randn(64, 3 * 768, generator=g, device=DEV).to(F16)
+    out = torch.full((64, 768), SENT, dtype=F16, device=DEV)
+    state = torch.zeros(16, dtype=torch.int32, device=DEV)
+    saved = runner.k_cache[1].clone()
+    if P > 65:
+        runner.k_cache[1, 0, :, P - 65:P - 33] *= 8
+    worst, kvs = 0.0, set()
+    try:
+        for layer in (0, 1):
+            for n0, n in rows:
+                got, ref, tol, _, _, kv_len = _draft_attn_run(runner, gm, bits, layer, n0, n, P, qkv, out, state)
+                what = f"draft attention P={P} layer={layer} n0={n0} n={n} kv_len={kv_len}"
+                worst = max(worst, _assert_within(got, ref, tol, what))
+                assert bool((out[n:] == SENT).all()), f"{what}: rows >= n were written"
+                kvs.add(kv_len)
+    finally:
+        runner.k_cache[1].copy_(saved)
+    cases.log_line("variant_sweep.log", f"draft attention P={P} layers=0,1 (n0,n)={rows} kv_len={min(kvs)}..{max(kvs)} "
+                   f"boosted={'layer 1' if P > 65 else 'none'}: worst err/bound {worst:.3f}")
+
+
+def test_draft_attention_tolerance_sees_errors(draft68m):
+    """Negative controls for the draft attention bound on one of its cases (layer 1, P = 513, the last 64 tree rows)."""
+    runner = draft68m
+    gm, _ = _draft_attn_rows()
+    from sequoia_b200.tree import pack_tree_mask
+    bits = pack_tree_mask(gm["mask"]).to(DEV)
+    g = torch.Generator(device=DEV).manual_seed(513)
+    qkv = torch.randn(64, 3 * 768, generator=g, device=DEV).to(F16)
+    out = torch.full((64, 768), SENT, dtype=F16, device=DEV)
+    state = torch.zeros(16, dtype=torch.int32, device=DEV)
+    n0, n, P = 64, 64, 513
+    got, ref, tol, p, vis, kv_len = _draft_attn_run(runner, gm, bits, 1, n0, n, P, qkv, out, state)
+    _assert_within(got, ref, tol, "draft attention negative control (exact reference)")
+    _negative_controls(got, qkv[:n, :768].view(n, 12, 64), runner.k_cache[1, 0, :, :kv_len], runner.v_cache[1, 0, :, :kv_len],
+                       vis, 12, 12, 64, tol, p, "draft attention")
