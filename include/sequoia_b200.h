@@ -39,6 +39,7 @@ extern "C" {
 #define SQ_ST_NAN 6
 #define SQ_ST_SKIPPED 7
 #define SQ_ST_M 8 /* host-written: length of tokens / position_ids (max_length); bounds the walk's epilogue writes */
+#define SQ_ST_FROZEN 9 /* host-written, batched calls only: nonzero = finished sequence, nothing of it is written */
 #define SQ_ST_WORDS 16
 
 typedef uint16_t sq_half;
@@ -305,6 +306,56 @@ int sq_draft_forward(sq_draft_plan* plan, int n, const int64_t* tokens, const in
  * plan's caches (rows already appended), output (n, hidden).  Small-shape alternative to sq_tree_attn for draft forwards. */
 int sq_draft_attention(sq_draft_plan* plan, int layer, int n, const sq_half* qkv, sq_half* attn_out, const int32_t* state,
                        int n0, int kv_end, const uint32_t* tree_bits, int tree_words, int tree_size, void* stream);
+
+/* ---- batches: B <= SQ_MAX_BATCH sequences that share one growmap, one launch per op for all of them ----
+ * Sequence b is a batch index of the grid.  Per-sequence data:
+ *   state:            B rows of SQ_ST_WORDS words (sequence b at state + b*SQ_ST_WORDS); tree-relative addressing uses
+ *                     that row's P.  A sequence whose SQ_ST_FROZEN word is nonzero writes nothing except its own
+ *                     activation / attention-output rows, and embed and the walks skip it entirely.
+ *   tokens, position_ids, storage_ids, r: B rows of ld_seq elements;
+ *   activation rows:  sequence-major, sequence b's n rows start at row b*n;
+ *   KV cache:         (L, B, Hkv, M, D), sequence b of layer l at planes (l*B + b)*Hkv + h;
+ *   target logits:    (B*S, V), node k of sequence b at row b*S + k;
+ *   draft logits:     node k of sequence b at row row_base[k] + b*row_step[k] (static int32 tables of S entries), so that
+ *                     one GEMM can write a whole tree level of all sequences: level rows n0..n0+tb-1 as one block of B*tb
+ *                     rows at row B*n0 gives row_base[k] = B*n0 + (k - n0), row_step[k] = tb;
+ *   accept_idx:       B rows of ld_acc (>= S) words; bonus-token noise: B rows of ld_noise (>= V) halfs.
+ * With B = 1 every call computes bit for bit what its single-sequence counterpart computes. */
+#define SQ_MAX_BATCH 8
+int sq_embed_rows_batch(const sq_half* table, const int64_t* tokens, int64_t ld_seq, const int32_t* state, int n0, int n,
+                        int B, int hidden, sq_half* out, void* stream);
+/* k_layer / v_layer: (B, Hkv, M, D) of this layer */
+int sq_rope_kv_append_batch(sq_half* qkv, int ld, int H, int Hkv, int D, const sq_half* cos, const sq_half* sin,
+                            const int64_t* position_ids, const int64_t* storage_ids, int64_t ld_seq, const int32_t* state,
+                            int n0, int n, int B, sq_half* k_layer, sq_half* v_layer, int M, void* stream);
+/* device-driven compaction of every sequence (n = state[N_NEW], offset = state[P_OLD] of its own row, indices from its
+ * accept_idx row); tail rows are left stale as in sq_kv_gather with state */
+int sq_kv_gather_batch(sq_half* k_cache, sq_half* v_cache, int L, int B, int Hkv, int M, int D, const int32_t* accept_idx,
+                       int ld_idx, const int32_t* state, int max_n, void* stream);
+/* attention plan over a (L, B, Hkv, M, D) cache; q / out hold B*n rows (n_max counts all of them) */
+int sq_attn_plan_create_batch(sq_attn_plan** plan, const sq_half* q, int ld, int n_max, int H, int Hkv, int D,
+                              const sq_half* k_cache, const sq_half* v_cache, int L, int B, int M, sq_half* out,
+                              void* workspace, int64_t workspace_bytes);
+/* n query rows per sequence under the structured tree mask (state required, B == the plan's B); the KV split count is
+ * chosen once for the whole launch */
+int sq_tree_attn_batch(sq_attn_plan* plan, int layer, int n, int B, const int32_t* state, int n0, int kv_end,
+                       const uint32_t* tree_bits, int tree_words, int tree_size, void* stream);
+/* sq_sample_level for every sequence: parent node parent_rows[j]'s logits from the draft-row table, its rand row at
+ * rand + b*ld_rand_seq + node*ld_rand (mode 0); children to tokens + b*ld_seq */
+int sq_sample_level_batch(const sq_half* logits, int64_t ld_logits, const int32_t* row_base, const int32_t* row_step,
+                          const sq_half* rand, int64_t ld_rand, int64_t ld_rand_seq, const int32_t* parent_rows,
+                          const int32_t* child_first, const int32_t* n_branch, int n_parents, int k_max, int V, float T,
+                          int mode, int64_t* tokens, int64_t ld_seq, const int32_t* state, int B, void* stream);
+/* one walk (one 8-CTA cluster) per sequence; target_logits (B*S, V) */
+int sq_accept_stochastic_batch(const sq_half* target_logits, int64_t ld_t, const sq_half* draft_logits, int64_t ld_d,
+                               const int32_t* row_base, const int32_t* row_step, const sq_half* r, const sq_half* noise,
+                               int64_t ld_noise, const int32_t* succ_off, const int32_t* succ, const int32_t* depth, int S,
+                               int V, float T, int64_t* tokens, int64_t* position_ids, int64_t ld_seq, int32_t* accept_idx,
+                               int64_t ld_acc, int32_t* state, int B, int max_target_seq, int policy, void* stream);
+/* target_token (B*S) int64 */
+int sq_accept_greedy_batch(const int64_t* target_token, const int32_t* succ_off, const int32_t* succ, const int32_t* depth,
+                           int S, int64_t* tokens, int64_t* position_ids, int64_t ld_seq, int32_t* accept_idx,
+                           int64_t ld_acc, int32_t* state, int B, int max_target_seq, void* stream);
 
 #ifdef __cplusplus
 }

@@ -1,0 +1,287 @@
+"""Several prompts per decode step: B sequences that share the engines, the growmap, T and top_p (DESIGN.md §3a).
+
+A steady step is the same two graph replays and one host sync as a single-sequence tree (sequoia_b200.tree), for all B
+sequences together: every per-sequence kernel is one launch for the batch, the row-wise kernels and the GEMMs see B*n
+rows.  Sequence b's device data: row b of state (B, 16), tokens / position_ids / storage_ids / r (B, M), rand (B, S, V),
+noise (B, V), accept_idx (B, S); rows b*S .. b*S+S-1 of the target logits (B*S, V); the draft logits of node k at
+row_base[k] + b*row_step[k] (each tree level of all sequences is one block, written by one lm_head GEMM).
+
+A sequence that is terminal, or has no room for another tree in max_length, is frozen: its state word SQ_ST_FROZEN is
+set and every batched kernel leaves its tokens, state and KV rows alone until the batch ends.
+"""
+from __future__ import annotations
+
+from typing import Dict, List, Optional, Sequence
+
+import torch
+
+from . import _lib, ops
+from .tree import _Static
+
+F16 = torch.float16
+ST_P, ST_M, ST_FROZEN = 0, 8, 9
+POLICIES = ("spec", "greedy")
+
+
+def draw_random(prompts: Sequence[torch.Tensor], M: int, S: int, V: int):
+    """The CPU draws of each sequence, in prompt order, exactly as a lone SpecTree for that prompt makes them: r (M) in
+    its constructor (Tree/SpecTree.py:60), then rand (S, V) after the draft prefill (:84).  -> (r (B, M), rand (B, S, V))"""
+    rs, rands = [], []
+    for _ in prompts:
+        rs.append(torch.rand(M, dtype=F16))
+        rands.append(torch.empty((S, V), dtype=F16).uniform_())
+    return torch.stack(rs), torch.stack(rands)
+
+
+class BatchTree:
+    """Batched SpecTree ("spec") / GreedyTree ("greedy") over `len(prompts)` sequences.  The engines must have been built
+    with batch_size == len(prompts).  verify() returns one (valid_tokens, accept_length, terminal) per sequence."""
+
+    def __init__(self, draft, target, prompts: Sequence[torch.Tensor], grow_map: dict, policy: str = "spec",
+                 temperature: float = 0.6, top_p: float = 1.0, max_length: int = 256,
+                 max_target_seq: Optional[int] = None):
+        if policy not in POLICIES:
+            raise ValueError(f"BatchTree policy {policy!r} is not supported (only {POLICIES}); greedys, specinfer and the "
+                             "*TreeTest policies run one sequence at a time")
+        B = len(prompts)
+        for name, eng in (("draft", draft), ("target", target)):
+            if eng.engine.batch_size != B:
+                raise ValueError(f"{name} engine holds {eng.engine.batch_size} sequences, got {B} prompts")
+            if eng.engine.max_length != max_length:
+                raise ValueError(f"{name} engine max_length {eng.engine.max_length} != {max_length}")
+        dev = torch.device(draft.device)
+        if dev.type != "cuda":
+            raise RuntimeError("sequoia_b200 trees run on a CUDA device only (there is no CPU path)")
+        self.draft, self.target = draft, target
+        self.policy, self.greedy = policy, policy == "greedy"
+        self.T, self.top_p = float(temperature), float(top_p)
+        self.B, self.M = B, max_length
+        self.max_target_seq = max_target_seq or max_length
+        self.st = st = _Static(grow_map, dev)
+        S = self.S = st.S
+        V = self.V = draft.engine.model_config.vocab_size
+        M = max_length
+        for p in prompts:
+            if len(p) + S - 1 > M:
+                raise ValueError(f"max_length={M} must hold the prompt ({len(p)}) + tree ({S}) - 1")
+        self.device = dev
+        i64 = dict(dtype=torch.int64, device=dev)
+        self.tokens = torch.zeros(B, M, **i64)
+        self.position_ids = torch.zeros(B, M, **i64)
+        self.storage_ids = torch.arange(M, **i64).repeat(B, 1)
+        self.state = torch.zeros(B, 16, dtype=torch.int32, device=dev)
+        self.host_state = torch.zeros(B, 16, dtype=torch.int32).pin_memory()
+        self.accept_idx = torch.zeros(B, max(S, 8), dtype=torch.int32, device=dev)
+        self.draft_logits = torch.zeros(B * S, V, dtype=F16, device=dev)
+        self.target_logits = torch.zeros(B * S, V, dtype=F16, device=dev)
+        self.row_base, self.row_step = ops.draft_row_tables([(0, 1)] + [(lv["n0"], lv["tb"]) for lv in st.levels], S, B,
+                                                            dev)
+        self.noise = torch.ones(B, V, dtype=F16, device=dev)
+        self.target_token = torch.zeros(B * S, **i64)
+        self.external_noise: Optional[torch.Tensor] = None    # tests: (n_iter, B, V) Exp(1) rows
+        self.graphs: Dict[str, torch.cuda.CUDAGraph] = {}
+        self.graph_launches: Dict[str, int] = {}
+        self.replays: Dict[str, int] = {}
+        self.use_graphs = True
+        self.iter = 0
+        self.frozen = [False] * B
+        self.last: List[tuple] = [None] * B
+        self.ground_truth_len = [len(p) for p in prompts]
+        self.target_kv_len = [0] * B
+        if not self.greedy:
+            r, rand = draw_random(prompts, M, S, V)
+            self.r, self.rand = r.to(dev), rand.to(dev)
+        else:
+            self.r = self.rand = None
+        st0 = torch.zeros(B, 16, dtype=torch.int32)
+        pos = torch.zeros(B, M, dtype=torch.int64)
+        for b, p in enumerate(prompts):
+            P = len(p)
+            self.tokens[b, :P] = p.to(dev)
+            pos[b, :P] = torch.arange(P)
+            pos[b, P:P + S - 1] = st.depth_cpu[1:] + P - 1
+            st0[b, ST_P], st0[b, ST_M] = P, M
+        self.position_ids.copy_(pos)
+        self.state.copy_(st0)
+        # draft prefill (SpecTree.py:67-80), one sequence at a time: rows [0, P) causal, the last row's logits -> node 0
+        with torch.inference_mode():
+            for b in range(B):
+                P = self.ground_truth_len[b]
+                self._alone(b, lambda: draft.engine.runner.forward(
+                    P, self.tokens, self.position_ids, self.storage_ids, state=self.state, n0=1 - P, kv_end=1,
+                    batch=True, logits_from=b * P + P - 1, logits_to=b * P + P, logits_out=self.draft_logits[b:b + 1],
+                    **self._mask_kw()))
+
+    # ---- helpers ---------------------------------------------------------------------------------------------------------
+    def _mask_kw(self):
+        return dict(tree_bits=self.st.tree_bits, tree_words=self.st.tree_words, tree_size=self.S)
+
+    def _alone(self, b: int, fn):
+        """Run a batched op sequence for sequence b only (prefill and first verify, whose row count depends on the
+        prompt): every other sequence gets a frozen copy of b's state row, so its kernels write nothing of it and read
+        exactly the cache range b reads; the state rows are restored afterwards."""
+        saved = self.state.clone()
+        tmp = saved[b:b + 1].repeat(self.B, 1)
+        tmp[:, ST_FROZEN] = 1
+        tmp[b] = saved[b]
+        self.state.copy_(tmp)
+        fn()
+        self.state.copy_(saved)
+
+    def freeze(self, b: int):
+        """Stop sequence b (the caller's length limit); it stays frozen until the batch ends."""
+        self.frozen[b] = True
+        self.state[b, ST_FROZEN] = 1
+
+    # ---- the op sequences ------------------------------------------------------------------------------------------------
+    def op_sample(self, i: int):
+        lv = self.st.levels[i]
+        ops.sample_level_batch(self.draft_logits, self.row_base, self.row_step, self.rand, lv["n_parents"], lv["k"],
+                               self.T, 1 if self.greedy else 0, parent_rows=lv["parents"], child_first=lv["first"],
+                               n_branch=lv["nb"], tokens=self.tokens, state=self.state)
+
+    def op_draft_level(self, i: int):
+        lv = self.st.levels[i]
+        n0, tb, B = lv["n0"], lv["tb"], self.B
+        self.draft.engine.runner.forward(tb, self.tokens, self.position_ids, self.storage_ids, state=self.state, n0=n0,
+                                         kv_end=n0 + tb, batch=True, logits_out=self.draft_logits[B * n0:B * (n0 + tb)],
+                                         **self._mask_kw())
+
+    def op_target_steady(self):
+        self.target.engine.runner.forward(self.S, self.tokens, self.position_ids, self.storage_ids, state=self.state,
+                                          n0=0, kv_end=self.S, batch=True, logits_out=self.target_logits,
+                                          **self._mask_kw())
+
+    def op_target_first(self, b: int):
+        """First verify of sequence b (SpecTree.py:164-176): rows [0, P+S-1), logits of the S tree rows."""
+        P, S = self.ground_truth_len[b], self.S
+        n = P + S - 1
+        self._alone(b, lambda: self.target.engine.runner.forward(
+            n, self.tokens, self.position_ids, self.storage_ids, state=self.state, n0=1 - P, kv_end=S, batch=True,
+            logits_from=b * n + n - S, logits_to=b * n + n, logits_out=self.target_logits[b * S:(b + 1) * S],
+            **self._mask_kw()))
+
+    def op_accept(self):
+        st = self.st
+        if self.greedy:
+            ops.argmax_rows(self.target_logits, self.target_token)
+            ops.accept_greedy_batch(self.target_token, st.succ_off, st.succ, st.depth, self.S, self.tokens,
+                                    self.position_ids, self.accept_idx, self.state, self.max_target_seq)
+            return
+        if self.top_p < 1.0:
+            ops.top_p_filter_(self.target_logits, self.top_p, self.T)
+        if self.external_noise is None:
+            self.noise.exponential_(1.0)
+        ops.accept_stochastic_batch(self.target_logits, self.draft_logits, self.row_base, self.row_step, self.r,
+                                    self.noise, st.succ_off, st.succ, st.depth, self.S, self.T, self.tokens,
+                                    self.position_ids, self.accept_idx, self.state, self.max_target_seq)
+
+    def op_kv_gather(self):
+        md = max(self.st.max_depth, 1)
+        for eng in (self.draft, self.target):
+            kv = eng.engine.kv_cache
+            ops.kv_gather_batch(kv.k_cache, kv.v_cache, self.accept_idx, self.state, md)
+
+    def op_bonus_forward(self):
+        self.draft.engine.runner.forward(1, self.tokens, self.position_ids, self.storage_ids, state=self.state, n0=0,
+                                         kv_end=1, batch=True, logits_out=self.draft_logits[0:self.B], **self._mask_kw())
+
+    def seq_draft(self):
+        for i in range(self.st.draft_step - 1):
+            self.op_sample(i)
+            self.op_draft_level(i)
+
+    def seq_post(self):
+        self.op_accept()
+        self.op_kv_gather()
+        self.op_bonus_forward()
+        self.host_state.copy_(self.state, non_blocking=True)
+
+    def seq_steady(self):
+        self.op_target_steady()
+        self.seq_post()
+
+    # ---- graphs (as sequoia_b200.tree._Runtime) --------------------------------------------------------------------------
+    def run(self, name: str, fn):
+        if not self.use_graphs:
+            fn()
+            return
+        g = self.graphs.get(name)
+        if g is None:
+            snap = self._snapshot()
+            s = torch.cuda.Stream()
+            s.wait_stream(torch.cuda.current_stream())
+            with torch.cuda.stream(s):
+                fn()
+                s.synchronize()
+            torch.cuda.current_stream().wait_stream(s)
+            self._restore(snap)
+            g = torch.cuda.CUDAGraph()
+            c0 = _lib.launch_count()
+            with torch.cuda.graph(g):
+                fn()
+            self.graph_launches[name] = _lib.launch_count() - c0
+            self._restore(snap)
+            self.graphs[name] = g
+        g.replay()
+        self.replays[name] = self.replays.get(name, 0) + 1
+
+    def _caches(self):
+        return [t for e in (self.draft, self.target) for t in (e.engine.kv_cache.k_cache, e.engine.kv_cache.v_cache)]
+
+    def _snapshot(self):
+        return dict(bufs=[t.clone() for t in (self.tokens, self.position_ids, self.state, self.draft_logits,
+                                              self.target_logits, self.noise)],
+                    kv=[t.clone() for t in self._caches()], rng=torch.cuda.get_rng_state(self.device))
+
+    def _restore(self, s):
+        for t, c in zip((self.tokens, self.position_ids, self.state, self.draft_logits, self.target_logits, self.noise),
+                        s["bufs"]):
+            t.copy_(c)
+        for t, c in zip(self._caches(), s["kv"]):
+            t.copy_(c)
+        torch.cuda.set_rng_state(s["rng"], self.device)
+
+    def kernel_launches(self) -> int:
+        return sum(self.graph_launches.get(k, 0) * v for k, v in self.replays.items())
+
+    # ---- the reference-style steps ---------------------------------------------------------------------------------------
+    @torch.inference_mode()
+    def construct_grow_map(self):
+        self.run("draft", self.seq_draft)
+
+    @torch.inference_mode()
+    def verify(self):
+        """-> [(valid_tokens, accept_length, terminal)] per sequence; a frozen sequence repeats its last result."""
+        if self.external_noise is not None and not self.greedy:
+            self.noise.copy_(self.external_noise[self.iter])
+        first = [b for b in range(self.B) if not self.frozen[b] and self.target_kv_len[b] != self.ground_truth_len[b] - 1]
+        if first:
+            # prefill + tree rows of each sequence eagerly (their row counts differ); the walk and the rest batched
+            for b in first:
+                self.op_target_first(b)
+            self.run("post", self.seq_post)
+        else:
+            self.run("steady", self.seq_steady)
+        torch.cuda.current_stream().synchronize()       # the one host sync of a verify step
+        self.iter += 1
+        hs = self.host_state
+        out = []
+        for b in range(self.B):
+            if self.frozen[b]:
+                out.append(self.last[b])
+                continue
+            a, terminal, skipped = int(hs[b, 1]), bool(hs[b, 2]), bool(hs[b, 7])
+            if terminal:
+                valid = self.tokens[b, :a]
+            elif skipped:
+                valid = self.tokens[b, :min(a + 1, self.M)]
+            else:
+                valid = self.tokens[b, :a + 1]
+                self.ground_truth_len[b] = a + 1
+                self.target_kv_len[b] = a
+            self.last[b] = (valid, a, terminal)
+            if terminal or skipped:
+                self.freeze(b)
+            out.append(self.last[b])
+        return out

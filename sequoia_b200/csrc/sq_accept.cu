@@ -195,14 +195,25 @@ __global__ void __launch_bounds__(ANT) accept_stochastic_kernel(
                 max_target_seq);
 }
 
+// BATCH: grid (B), one walk per sequence; target_token rows of S per sequence, the rest as in BatchArgs.
+template <bool BATCH>
 __global__ void accept_greedy_kernel(const int64_t* __restrict__ target_token, const int32_t* __restrict__ succ_off,
                                      const int32_t* __restrict__ succ, const int32_t* __restrict__ depth, int S,
                                      int64_t* __restrict__ tokens, int64_t* __restrict__ position_ids,
                                      int32_t* __restrict__ accept_idx, int32_t* __restrict__ state,
-                                     int max_target_seq) {
+                                     int max_target_seq, int64_t ld_seq, int64_t ld_acc) {
   __shared__ int32_t sh_acc[1024];
   __shared__ int sh_n, sh_term;
   __shared__ long long sh_bonus;
+  const int b = seq_index<BATCH>(blockIdx.x);
+  if (BATCH) {
+    state += b * ST_WORDS;
+    if (state[ST_FROZEN]) return;
+    target_token += (int64_t)b * S;
+    tokens += b * ld_seq;
+    position_ids += b * ld_seq;
+    accept_idx += b * ld_acc;
+  }
   const int P = state[ST_P];
   if (threadIdx.x == 0) {
     int cur = 0, n_new = 0, term = 0;
@@ -256,8 +267,39 @@ extern "C" int sq_accept_greedy(const int64_t* target_token, const int32_t* succ
                                 const int32_t* depth, int S, int64_t* tokens, int64_t* position_ids,
                                 int32_t* accept_idx, int32_t* state, int max_target_seq, void* stream) {
   SQ_CHECK_ARG(S >= 1 && S <= 1024, "sq_accept_greedy: S=%d unsupported", S);
-  accept_greedy_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(target_token, succ_off, succ, depth, S, tokens,
-                                                            position_ids, accept_idx, state, max_target_seq);
+  accept_greedy_kernel<false><<<1, 256, 0, (cudaStream_t)stream>>>(target_token, succ_off, succ, depth, S, tokens,
+                                                                   position_ids, accept_idx, state, max_target_seq, 0, 0);
   SQ_CHECK_LAUNCH("sq_accept_greedy");
   return SQ_OK;
+}
+
+extern "C" int sq_accept_greedy_batch(const int64_t* target_token, const int32_t* succ_off, const int32_t* succ,
+                                      const int32_t* depth, int S, int64_t* tokens, int64_t* position_ids, int64_t ld_seq,
+                                      int32_t* accept_idx, int64_t ld_acc, int32_t* state, int B, int max_target_seq,
+                                      void* stream) {
+  SQ_CHECK_ARG(S >= 1 && S <= 1024, "sq_accept_greedy_batch: S=%d unsupported", S);
+  SQ_CHECK_ARG(B >= 1 && B <= SQ_MAX_BATCH, "sq_accept_greedy_batch: B=%d (1..%d)", B, SQ_MAX_BATCH);
+  SQ_CHECK_ARG(ld_acc >= S && ld_seq >= 1, "sq_accept_greedy_batch: accept_idx rows of %lld < S=%d", (long long)ld_acc, S);
+  accept_greedy_kernel<true><<<B, 256, 0, (cudaStream_t)stream>>>(target_token, succ_off, succ, depth, S, tokens,
+                                                                  position_ids, accept_idx, state, max_target_seq, ld_seq,
+                                                                  ld_acc);
+  SQ_CHECK_LAUNCH("sq_accept_greedy_batch");
+  return SQ_OK;
+}
+
+extern "C" int sq_accept_stochastic_batch(const sq_half* target_logits, int64_t ld_t, const sq_half* draft_logits,
+                                          int64_t ld_d, const int32_t* row_base, const int32_t* row_step, const sq_half* r,
+                                          const sq_half* noise, int64_t ld_noise, const int32_t* succ_off,
+                                          const int32_t* succ, const int32_t* depth, int S, int V, float T,
+                                          int64_t* tokens, int64_t* position_ids, int64_t ld_seq, int32_t* accept_idx,
+                                          int64_t ld_acc, int32_t* state, int B, int max_target_seq, int policy,
+                                          void* stream) {
+  SQ_CHECK_ARG(S >= 1 && S <= 1024, "sq_accept_stochastic_batch: S=%d unsupported", S);
+  SQ_CHECK_ARG(B >= 1 && B <= SQ_MAX_BATCH, "sq_accept_stochastic_batch: B=%d (1..%d)", B, SQ_MAX_BATCH);
+  SQ_CHECK_ARG((policy & ~3) == 0, "sq_accept_stochastic_batch: unknown policy bits %d", policy);
+  SQ_CHECK_ARG(row_base && row_step, "sq_accept_stochastic_batch: null draft-row table");
+  SQ_CHECK_ARG(ld_acc >= S && ld_noise >= V, "sq_accept_stochastic_batch: accept_idx / noise rows too short");
+  BatchArgs ba{B, ld_seq, ld_noise, ld_acc, row_base, row_step};
+  return sq::launch_accept_cluster(target_logits, ld_t, draft_logits, ld_d, r, noise, succ_off, succ, depth, S, V, T, tokens,
+                                   position_ids, accept_idx, state, max_target_seq, policy, stream, &ba);
 }

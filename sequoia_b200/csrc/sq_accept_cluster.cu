@@ -68,16 +68,30 @@ struct ClusterCtx {
   __device__ __forceinline__ void next() { ph ^= 1; }
 };
 
+// BATCH: grid (CL, B), one cluster per sequence (see BatchArgs); a frozen sequence's cluster exits before its first
+// exchange (the whole cluster reads the same word).
+template <bool BATCH>
 __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(CNT) accept_stochastic_cluster_kernel(
     const __half* __restrict__ target_logits, int64_t ld_t, const __half* __restrict__ draft_logits, int64_t ld_d,
     const __half* __restrict__ r, const __half* __restrict__ noise, const int32_t* __restrict__ succ_off,
     const int32_t* __restrict__ succ, const int32_t* __restrict__ depth, int S, int V, float inv_T,
     int64_t* __restrict__ tokens, int64_t* __restrict__ position_ids, int32_t* __restrict__ accept_idx,
-    int32_t* __restrict__ state, int max_target_seq, int policy) {
+    int32_t* __restrict__ state, int max_target_seq, int policy, BatchArgs ba) {
   __shared__ Xch xch;
   __shared__ float red[CNW];
   __shared__ int32_t sh_acc[1024];
   __shared__ float sh_own[2];                    // owner thread -> block: {etok, flag bits as float}
+  const int b = seq_index<BATCH>(blockIdx.y);
+  if (BATCH) {
+    state += b * ST_WORDS;
+    if (state[ST_FROZEN]) return;
+    target_logits += (int64_t)b * S * ld_t;
+    r += b * ba.ld_seq;
+    noise += b * ba.ld_noise;
+    tokens += b * ba.ld_seq;
+    position_ids += b * ba.ld_seq;
+    accept_idx += b * ba.ld_acc;
+  }
   ClusterCtx cx{cg::this_cluster(), &xch, 0, 0};
   cx.rank = (int)cx.cluster.block_rank();
   const int P = state[ST_P];
@@ -94,7 +108,7 @@ __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(CNT) accept_stochas
     const bool leaf = (c0 == c1);
     // load + scale both rows; softmax statistics of both in two exchanges
     p.u = active ? reinterpret_cast<const uint4*>(target_logits + cur * ld_t)[chunk] : NEG_INF;
-    xd.u = (active && !leaf) ? reinterpret_cast<const uint4*>(draft_logits + cur * ld_d)[chunk] : NEG_INF;
+    xd.u = (active && !leaf) ? reinterpret_cast<const uint4*>(draft_logits + ba.row<BATCH>(cur, b) * ld_d)[chunk] : NEG_INF;
     float m1 = -INFINITY, m2 = -INFINITY;
 #pragma unroll
     for (int e = 0; e < 8; ++e) {
@@ -233,11 +247,19 @@ using namespace sq;
 int sq::launch_accept_cluster(const sq_half* target_logits, int64_t ld_t, const sq_half* draft_logits, int64_t ld_d,
                               const sq_half* r, const sq_half* noise, const int32_t* succ_off, const int32_t* succ,
                               const int32_t* depth, int S, int V, float T, int64_t* tokens, int64_t* position_ids,
-                              int32_t* accept_idx, int32_t* state, int max_target_seq, int policy, void* stream) {
+                              int32_t* accept_idx, int32_t* state, int max_target_seq, int policy, void* stream,
+                              const BatchArgs* batch) {
   SQ_CHECK_ARG(V % 8 == 0 && V > 0 && V <= CL * CNT * 8, "sq_accept_stochastic: V=%d unsupported", V);
-  accept_stochastic_cluster_kernel<<<CL, CNT, 0, (cudaStream_t)stream>>>(
+  if (batch) {
+    accept_stochastic_cluster_kernel<true><<<dim3(CL, batch->B), CNT, 0, (cudaStream_t)stream>>>(
+        (const __half*)target_logits, ld_t, (const __half*)draft_logits, ld_d, (const __half*)r, (const __half*)noise,
+        succ_off, succ, depth, S, V, 1.0f / T, tokens, position_ids, accept_idx, state, max_target_seq, policy, *batch);
+    SQ_CHECK_LAUNCH("sq_accept_stochastic_batch");
+    return SQ_OK;
+  }
+  accept_stochastic_cluster_kernel<false><<<CL, CNT, 0, (cudaStream_t)stream>>>(
       (const __half*)target_logits, ld_t, (const __half*)draft_logits, ld_d, (const __half*)r, (const __half*)noise,
-      succ_off, succ, depth, S, V, 1.0f / T, tokens, position_ids, accept_idx, state, max_target_seq, policy);
+      succ_off, succ, depth, S, V, 1.0f / T, tokens, position_ids, accept_idx, state, max_target_seq, policy, BatchArgs{});
   SQ_CHECK_LAUNCH("sq_accept_stochastic(cluster)");
   return SQ_OK;
 }

@@ -4,10 +4,26 @@
 
 namespace sq {
 
+// Per-sequence addressing of the batched walks (sequence b = blockIdx.y): tokens / position_ids / r rows of ld_seq
+// elements, noise rows of ld_noise, accept_idx rows of ld_acc, target logits (B*S, V), and the draft-logit row of node k
+// at row_base[k] + b * row_step[k].
+struct BatchArgs {
+  int B;
+  int64_t ld_seq, ld_noise, ld_acc;
+  const int32_t* row_base;
+  const int32_t* row_step;
+  template <bool BATCH>
+  __device__ __forceinline__ int64_t row(int node, int b) const {
+    return BATCH ? (int64_t)row_base[node] + (int64_t)b * row_step[node] : node;
+  }
+};
+
+// batch == nullptr: the single-sequence kernel
 int launch_accept_cluster(const sq_half* target_logits, int64_t ld_t, const sq_half* draft_logits, int64_t ld_d,
                           const sq_half* r, const sq_half* noise, const int32_t* succ_off, const int32_t* succ,
                           const int32_t* depth, int S, int V, float T, int64_t* tokens, int64_t* position_ids,
-                          int32_t* accept_idx, int32_t* state, int max_target_seq, int policy, void* stream);
+                          int32_t* accept_idx, int32_t* state, int max_target_seq, int policy, void* stream,
+                          const BatchArgs* batch = nullptr);
 
 // policy bits: SQ_ACCEPT_GE / SQ_ACCEPT_KEEP_Q from include/sequoia_b200.h
 

@@ -23,6 +23,7 @@
 struct sq_attn_plan {
   const __half* q;
   int ld, n_max, H, Hkv, D, L, M;
+  int B;          // sequences in the cache: (L, B, Hkv, M, D)
   const __half* k_cache;
   const __half* v_cache;
   __half* out;
@@ -50,6 +51,7 @@ struct AttnArgs {
   const __half* v_layer;
   __half* out;
   int n, H, Hkv, M, GP;
+  int B;                   // sequences of a batched launch (rows of sequence b start at b*n; grid.y = B * q tiles)
   int layer;
   const int32_t* state;
   int n0, kv_end, prefix_len_host;
@@ -181,7 +183,9 @@ constexpr float RESCALE_THRESHOLD = 8.0f;   // log2 units: P stays <= 2^8 under 
 // 256 threads = 2 warpgroups; warpgroup g owns tile rows [64 g, 64 g + 64): S, P and O of those rows live in its registers
 // in the wgmma accumulator layout -- thread holds rows r0 = 64 g + 16 (warp % 4) + lane / 4 and r0 + 8, and of every
 // 64-column chunk the columns 8 j + 2 (lane % 4) + {0, 1}: element [4 j + 2 h + e] is (row r0 + 8 h, column 8 j + 2 q + e).
-template <int D, bool DENSE>
+// BATCH (structured mask only): grid.y = B * q tiles, sequence b = blockIdx.y / q tiles reads its own state row, its Q rows
+// and writes its output rows at offset b*n, and reads cache heads (layer*B + b)*Hkv + h.
+template <int D, bool DENSE, bool BATCH>
 __global__ void __launch_bounds__(256, 1)
     tree_attn_tc_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_k,
                         const __grid_constant__ CUtensorMap tm_v, AttnArgs a) {
@@ -190,7 +194,11 @@ __global__ void __launch_bounds__(256, 1)
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // dynamic smem base is only guaranteed 16 B aligned: re-align to 1024 B for SWIZZLE_128B (same offset in every CTA)
   uint8_t* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
-  const int grp = blockIdx.x, qt = blockIdx.y, split = blockIdx.z, Z = gridDim.z;
+  const int q_tiles = BATCH ? (int)gridDim.y / a.B : (int)gridDim.y;
+  const int b = BATCH ? (int)blockIdx.y / q_tiles : 0;
+  const int grp = blockIdx.x, qt = BATCH ? (int)blockIdx.y % q_tiles : (int)blockIdx.y, split = blockIdx.z, Z = gridDim.z;
+  const int32_t* state = BATCH ? a.state + b * ST_WORDS : a.state;
+  __half* out = BATCH ? a.out + (int64_t)b * a.n * (a.H * D) : a.out;
   const int GP = a.GP, RPT = TILE_Q / GP;        // heads per tile, query rows per tile
   const int hkv = (grp * GP) / (a.H / a.Hkv);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -222,18 +230,18 @@ __global__ void __launch_bounds__(256, 1)
   if (tid == 0) {
     ptx::mbar_expect_tx(bar_q, SM::TILE_BYTES);
 #pragma unroll
-    for (int hh = 0; hh < SM::HALVES; ++hh) ptx::tma_load_3d(sQ + hh * 16384, &tm_q, bar_q, hh * 64, grp * GP, q0);
+    for (int hh = 0; hh < SM::HALVES; ++hh) ptx::tma_load_3d(sQ + hh * 16384, &tm_q, bar_q, hh * 64, grp * GP, b * a.n + q0);
   }
   uint32_t* sbits = reinterpret_cast<uint32_t*>(smem + SM::OFF_MASK);
   if (!DENSE && a.tree_words > 0 && tid < RPT) {
-    const int node = a.state ? (a.n0 + q0 + tid) : (a.n0 + q0 + tid - (a.prefix_len_host - 1));
+    const int node = state ? (a.n0 + q0 + tid) : (a.n0 + q0 + tid - (a.prefix_len_host - 1));
     const bool has = node >= 1 && node < a.tree_size;
 #pragma unroll 4
     for (int w = 0; w < a.tree_words; ++w)
       sbits[tid * a.tree_words + w] = has ? a.tree_bits[(int64_t)node * a.tree_words + w] : 0u;
   }
-  const int P = a.state ? a.state[ST_P] : a.prefix_len_host;
-  const int base = a.state ? (P - 1) : 0;
+  const int P = state ? state[ST_P] : a.prefix_len_host;
+  const int base = state ? (P - 1) : 0;
   const int kv_len = base + a.kv_end;
   // active KV tiles of this q tile (tiles wholly beyond what its last row may see are never touched), split in chunks
   int T;
@@ -246,7 +254,7 @@ __global__ void __launch_bounds__(256, 1)
   const int nsplit = (T + tps - 1) / tps;        // splits that own at least one tile
   const int t_begin = split * tps;
   const int NT = max(0, min(T, t_begin + tps) - t_begin);
-  const int kvrow = a.layer * a.Hkv + hkv;
+  const int kvrow = (BATCH ? a.layer * a.B + b : a.layer) * a.Hkv + hkv;
   SQ_STAMP(0);
 
   if (NT > 0) {
@@ -420,7 +428,7 @@ __global__ void __launch_bounds__(256, 1)
       for (int rr = warp * RPW + sub; rr < TILE_Q; rr += 8 * RPW) {
         const int qrow = q0 + rr / GP;
         if (qrow < a.n)
-          *reinterpret_cast<uint4*>(a.out + (int64_t)qrow * (a.H * D) + (grp * GP + rr % GP) * D + cc * 8) =
+          *reinterpret_cast<uint4*>(out + (int64_t)qrow * (a.H * D) + (grp * GP + rr % GP) * D + cc * 8) =
               *reinterpret_cast<const uint4*>(sO + rr * SM::O_STRIDE + cc * 8);
       }
       SQ_STAMP(8);
@@ -498,7 +506,7 @@ __global__ void __launch_bounds__(256, 1)
       Pack8 res;
 #pragma unroll
       for (int e = 0; e < 8; ++e) res.h[e] = f2h(acc[e]);
-      *reinterpret_cast<uint4*>(a.out + (int64_t)qrow * (a.H * D) + (grp * GP + rr % GP) * D + cc * 8) = res.u;
+      *reinterpret_cast<uint4*>(out + (int64_t)qrow * (a.H * D) + (grp * GP + rr % GP) * D + cc * 8) = res.u;
     }
   }
   SQ_STAMP(8);
@@ -545,14 +553,21 @@ extern "C" int64_t sq_attn_workspace_bytes(int n_max, int H, int D, int M) {
 extern "C" int sq_attn_plan_create(sq_attn_plan** plan, const sq_half* q, int ld, int n_max, int H, int Hkv, int D,
                                    const sq_half* k_cache, const sq_half* v_cache, int L, int M, sq_half* out,
                                    void* workspace, int64_t workspace_bytes) {
+  return sq_attn_plan_create_batch(plan, q, ld, n_max, H, Hkv, D, k_cache, v_cache, L, 1, M, out, workspace, workspace_bytes);
+}
+
+extern "C" int sq_attn_plan_create_batch(sq_attn_plan** plan, const sq_half* q, int ld, int n_max, int H, int Hkv, int D,
+                                         const sq_half* k_cache, const sq_half* v_cache, int L, int B, int M, sq_half* out,
+                                         void* workspace, int64_t workspace_bytes) {
   SQ_CHECK_ARG(plan != nullptr, "sq_attn_plan_create: null plan");
+  SQ_CHECK_ARG(B >= 1 && B <= SQ_MAX_BATCH, "sq_attn_plan_create: B=%d (1..%d)", B, SQ_MAX_BATCH);
   SQ_CHECK_ARG(D == 64 || D == 128, "sq_attn_plan_create: head_dim %d unsupported (64 or 128)", D);
   SQ_CHECK_ARG(H >= 1 && Hkv >= 1 && H % Hkv == 0 && ld % 8 == 0 && n_max >= 1 && M >= 1, "sq_attn_plan_create: bad shape");
   SQ_CHECK_ARG(workspace_bytes >= sq_attn_workspace_bytes(n_max, H, D, M), "sq_attn_plan_create: workspace too small");
   SQ_CHECK_ARG(((uintptr_t)q % 16 == 0) && ((uintptr_t)k_cache % 16 == 0) && ((uintptr_t)v_cache % 16 == 0),
                "sq_attn_plan_create: pointers must be 16 B aligned");
   sq_attn_plan* p = new sq_attn_plan();
-  p->q = (const __half*)q; p->ld = ld; p->n_max = n_max; p->H = H; p->Hkv = Hkv; p->D = D; p->L = L; p->M = M;
+  p->q = (const __half*)q; p->ld = ld; p->n_max = n_max; p->H = H; p->Hkv = Hkv; p->D = D; p->L = L; p->M = M; p->B = B;
   p->k_cache = (const __half*)k_cache; p->v_cache = (const __half*)v_cache; p->out = (__half*)out;
   p->splits_max = (M + TILE_KV - 1) / TILE_KV;
   {
@@ -582,7 +597,7 @@ extern "C" int sq_attn_plan_create(sq_attn_plan** plan, const sq_half* q, int ld
     if (rc) { delete p; return rc; }
   }
   {
-    cuuint64_t dims[3] = {(cuuint64_t)D, (cuuint64_t)M, (cuuint64_t)L * Hkv};
+    cuuint64_t dims[3] = {(cuuint64_t)D, (cuuint64_t)M, (cuuint64_t)L * B * Hkv};
     cuuint64_t strides[2] = {(cuuint64_t)D * 2, (cuuint64_t)M * D * 2};
     cuuint32_t box[3] = {64, (cuuint32_t)TILE_KV, 1};
     int rc = encode_map(&p->tm_k, k_cache, 3, dims, strides, box);
@@ -617,7 +632,7 @@ extern "C" int sq_attn_plan_error(sq_attn_plan* plan) {
   return v;
 }
 
-template <int D>
+template <int D, bool BATCH>
 static int launch_attn(sq_attn_plan* p, AttnArgs& a, int impl, cudaStream_t st) {
   if (impl == 1) {
     tree_attn_simt_kernel<D><<<dim3(a.n, a.H), 128, 0, st>>>(a);
@@ -625,7 +640,8 @@ static int launch_attn(sq_attn_plan* p, AttnArgs& a, int impl, cudaStream_t st) 
     return SQ_OK;
   }
   constexpr int smem = TcSmem<D>::TOTAL + 1024;
-  auto kern = a.dense_mask ? tree_attn_tc_kernel<D, true> : tree_attn_tc_kernel<D, false>;
+  auto kern = BATCH ? tree_attn_tc_kernel<D, false, true>
+                    : (a.dense_mask ? tree_attn_tc_kernel<D, true, false> : tree_attn_tc_kernel<D, false, false>);
   static bool attr_set[2] = {false, false};    // (a process drives one device: bench / tests / torchrun ranks)
   if (!attr_set[a.dense_mask ? 1 : 0]) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
@@ -643,13 +659,13 @@ static int launch_attn(sq_attn_plan* p, AttnArgs& a, int impl, cudaStream_t st) 
     cudaGetDevice(&dev);
     if (cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n_sm <= 0) n_sm = 132;
   }
-  int Z = p->splits_force > 0 ? p->splits_force : n_sm / std::max(1, groups * q_tiles);
+  int Z = p->splits_force > 0 ? p->splits_force : n_sm / std::max(1, groups * q_tiles * a.B);
   Z = std::max(1, std::min(8, Z));
   Z = std::min(Z, p->splits_max);
   if (a.state == nullptr) Z = std::max(1, std::min(Z, (a.kv_end + TILE_KV - 1) / TILE_KV));
   p->last_splits = Z;
   cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(groups, q_tiles, Z);
+  cfg.gridDim = dim3(groups, q_tiles * a.B, Z);
   cfg.blockDim = dim3(256);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = st;
@@ -675,6 +691,7 @@ extern "C" int sq_tree_attn(sq_attn_plan* plan, int layer, int n, const int32_t*
                             int prefix_len_host, const sq_half* dense_mask, int64_t mask_ld, const uint32_t* tree_bits,
                             int tree_words, int tree_size, int impl, void* stream) {
   SQ_CHECK_ARG(plan != nullptr, "sq_tree_attn: null plan");
+  SQ_CHECK_ARG(plan->B == 1, "sq_tree_attn: the plan holds %d sequences (use sq_tree_attn_batch)", plan->B);
   SQ_CHECK_ARG(n >= 0 && n <= plan->n_max, "sq_tree_attn: n=%d exceeds plan n_max=%d", n, plan->n_max);
   SQ_CHECK_ARG(layer >= 0 && layer < plan->L, "sq_tree_attn: bad layer %d", layer);
   SQ_CHECK_ARG(tree_words <= 32, "sq_tree_attn: tree_size > 1024 unsupported (32 mask words per row)");
@@ -685,13 +702,36 @@ extern "C" int sq_tree_attn(sq_attn_plan* plan, int layer, int n, const int32_t*
   a.k_layer = plan->k_cache + (int64_t)layer * plan->Hkv * plan->M * plan->D;
   a.v_layer = plan->v_cache + (int64_t)layer * plan->Hkv * plan->M * plan->D;
   a.out = plan->out;
-  a.n = n; a.H = plan->H; a.Hkv = plan->Hkv; a.M = plan->M; a.GP = plan->GP; a.layer = layer;
+  a.n = n; a.H = plan->H; a.Hkv = plan->Hkv; a.M = plan->M; a.GP = plan->GP; a.B = 1; a.layer = layer;
   a.state = state; a.n0 = n0; a.kv_end = kv_end; a.prefix_len_host = prefix_len_host;
   a.dense_mask = (const __half*)dense_mask; a.mask_ld = mask_ld;
   a.tree_bits = tree_bits; a.tree_words = tree_bits ? tree_words : 0; a.tree_size = tree_bits ? tree_size : 0;
   a.scale = 1.0f / sqrtf((float)plan->D);
   a.debug_flags = plan->debug_flags; a.err_flag = plan->err_flag; a.dbg = plan->dbg;
   cudaStream_t st = (cudaStream_t)stream;
-  if (plan->D == 64) return launch_attn<64>(plan, a, impl, st);
-  return launch_attn<128>(plan, a, impl, st);
+  if (plan->D == 64) return launch_attn<64, false>(plan, a, impl, st);
+  return launch_attn<128, false>(plan, a, impl, st);
+}
+
+extern "C" int sq_tree_attn_batch(sq_attn_plan* plan, int layer, int n, int B, const int32_t* state, int n0, int kv_end,
+                                  const uint32_t* tree_bits, int tree_words, int tree_size, void* stream) {
+  SQ_CHECK_ARG(plan != nullptr, "sq_tree_attn_batch: null plan");
+  SQ_CHECK_ARG(B == plan->B, "sq_tree_attn_batch: B=%d but the plan's cache holds %d sequences", B, plan->B);
+  SQ_CHECK_ARG(n >= 0 && (int64_t)n * B <= plan->n_max, "sq_tree_attn_batch: %d x %d rows exceed plan n_max=%d", B, n,
+               plan->n_max);
+  SQ_CHECK_ARG(layer >= 0 && layer < plan->L, "sq_tree_attn_batch: bad layer %d", layer);
+  SQ_CHECK_ARG(tree_words <= 32, "sq_tree_attn_batch: tree_size > 1024 unsupported (32 mask words per row)");
+  SQ_CHECK_ARG(state != nullptr, "sq_tree_attn_batch: needs the state array");
+  if (n == 0) return SQ_OK;
+  AttnArgs a{};
+  a.q = plan->q; a.ld = plan->ld;
+  a.out = plan->out;
+  a.n = n; a.H = plan->H; a.Hkv = plan->Hkv; a.M = plan->M; a.GP = plan->GP; a.B = B; a.layer = layer;
+  a.state = state; a.n0 = n0; a.kv_end = kv_end; a.prefix_len_host = 0;
+  a.tree_bits = tree_bits; a.tree_words = tree_bits ? tree_words : 0; a.tree_size = tree_bits ? tree_size : 0;
+  a.scale = 1.0f / sqrtf((float)plan->D);
+  a.debug_flags = plan->debug_flags; a.err_flag = plan->err_flag; a.dbg = plan->dbg;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (plan->D == 64) return launch_attn<64, true>(plan, a, 0, st);
+  return launch_attn<128, true>(plan, a, 0, st);
 }

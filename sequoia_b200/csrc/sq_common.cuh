@@ -63,8 +63,13 @@ enum StateWord : int {
   ST_NAN = 6,        // residual had a NaN
   ST_SKIPPED = 7,    // prepare_for_next_iter was skipped (a + 1 > max_target_seq, or the tree would overrun the buffers)
   ST_M = 8,          // length of the tokens / position_ids buffers (max_length), written by the host once per prompt
+  ST_FROZEN = 9,     // batched entry points only: nonzero = finished sequence, its tokens / state / KV rows are not written
   ST_WORDS = 16
 };
+
+// Batched entry points: sequence b is the grid's batch index.  BATCH = false compiles the single-sequence kernel unchanged.
+template <bool BATCH>
+__device__ __forceinline__ int seq_index(unsigned grid_coord) { return BATCH ? (int)grid_coord : 0; }
 
 __device__ __forceinline__ int row_base(const int32_t* P_ptr, int n0) {
   return (P_ptr ? (P_ptr[ST_P] - 1) : 0) + n0;

@@ -7,11 +7,20 @@
 namespace sq {
 
 // threads: ROWS_PER_PASS rows x (D/8) 16-byte lanes.  Dynamic shared memory holds all n rows when n > ROWS_PER_PASS.
+// BATCH: the cache is (L, B, Hkv, M, D); plane x belongs to sequence (x / Hkv) % B, which reads its own state row and
+// index row (idx + b * ld_idx) and is skipped when frozen.
+template <bool BATCH>
 __global__ void kv_gather_kernel(__half* __restrict__ k_cache, __half* __restrict__ v_cache, int M, int D,
                                  const int32_t* __restrict__ idx, int n_host, int offset_host,
-                                 const int32_t* __restrict__ state, int max_n) {
+                                 const int32_t* __restrict__ state, int max_n, int Hkv, int B, int ld_idx) {
   extern __shared__ uint4 stage[];
   __half* plane = (blockIdx.y == 0 ? k_cache : v_cache) + (int64_t)blockIdx.x * M * D;
+  if (BATCH) {
+    const int b = (blockIdx.x / Hkv) % B;
+    state += b * ST_WORDS;
+    idx += b * ld_idx;
+    if (state[ST_FROZEN]) return;
+  }
   int n = n_host, offset = offset_host;
   if (state) { n = state[ST_N_NEW]; offset = state[ST_P_OLD]; }
   if (n > max_n) n = max_n;
@@ -90,6 +99,36 @@ extern "C" int sq_kv_gather_big(sq_half* k_cache, sq_half* v_cache, int L, int H
   return SQ_OK;
 }
 
+template <bool BATCH>
+static int launch_gather(sq_half* k_cache, sq_half* v_cache, int planes, int M, int D, const int32_t* idx, int n, int offset,
+                         const int32_t* state, int max_n, int Hkv, int B, int ld_idx, cudaStream_t st) {
+  const size_t smem = (size_t)max_n * D * 2;
+  if (smem > 48 * 1024) {
+    cudaError_t e = cudaFuncSetAttribute(kv_gather_kernel<BATCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) { set_error("sq_kv_gather: smem attr: %s", cudaGetErrorString(e)); return SQ_ERR_CUDA; }
+  }
+  int threads = max_n * (D / 8);
+  threads = threads < 64 ? 64 : (threads > 512 ? 512 : ((threads + 31) / 32) * 32);
+  kv_gather_kernel<BATCH><<<dim3(planes, 2), threads, smem, st>>>((__half*)k_cache, (__half*)v_cache, M, D, idx, n, offset,
+                                                                  state, max_n, Hkv, B, ld_idx);
+  return SQ_OK;
+}
+
+extern "C" int sq_kv_gather_batch(sq_half* k_cache, sq_half* v_cache, int L, int B, int Hkv, int M, int D,
+                                  const int32_t* accept_idx, int ld_idx, const int32_t* state, int max_n, void* stream) {
+  SQ_CHECK_ARG(D % 8 == 0, "sq_kv_gather_batch: D %% 8 != 0");
+  SQ_CHECK_ARG(B >= 1 && B <= SQ_MAX_BATCH && state != nullptr && accept_idx != nullptr,
+               "sq_kv_gather_batch: B=%d (1..%d) needs a state array and an index array", B, SQ_MAX_BATCH);
+  SQ_CHECK_ARG(max_n >= 0 && max_n <= ld_idx && (int64_t)max_n * D * 2 <= 200 * 1024,
+               "sq_kv_gather_batch: max_n=%d rows do not fit on chip or in an index row of %d", max_n, ld_idx);
+  if (max_n == 0) return SQ_OK;
+  const int rc = launch_gather<true>(k_cache, v_cache, L * B * Hkv, M, D, accept_idx, 0, 0, state, max_n, Hkv, B, ld_idx,
+                                     (cudaStream_t)stream);
+  if (rc) return rc;
+  SQ_CHECK_LAUNCH("sq_kv_gather_batch");
+  return SQ_OK;
+}
+
 extern "C" int sq_kv_gather(sq_half* k_cache, sq_half* v_cache, int L, int Hkv, int M, int D, const int32_t* idx,
                             int n, int offset, const int32_t* state, int max_n, int zero_tail, void* stream) {
   SQ_CHECK_ARG(D % 8 == 0, "sq_kv_gather: D %% 8 != 0");
@@ -99,15 +138,8 @@ extern "C" int sq_kv_gather(sq_half* k_cache, sq_half* v_cache, int L, int Hkv, 
   cudaStream_t st = (cudaStream_t)stream;
   const int planes = L * Hkv;
   if (max_n > 0) {
-    const size_t smem = (size_t)max_n * D * 2;
-    if (smem > 48 * 1024) {
-      cudaError_t e = cudaFuncSetAttribute(kv_gather_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-      if (e != cudaSuccess) { set_error("sq_kv_gather: smem attr: %s", cudaGetErrorString(e)); return SQ_ERR_CUDA; }
-    }
-    int threads = max_n * (D / 8);
-    threads = threads < 64 ? 64 : (threads > 512 ? 512 : ((threads + 31) / 32) * 32);
-    kv_gather_kernel<<<dim3(planes, 2), threads, smem, st>>>((__half*)k_cache, (__half*)v_cache, M, D, idx, n, offset,
-                                                            state, max_n);
+    const int rc = launch_gather<false>(k_cache, v_cache, planes, M, D, idx, n, offset, state, max_n, Hkv, 1, 0, st);
+    if (rc) return rc;
     SQ_CHECK_LAUNCH("sq_kv_gather");
   }
   if (zero_tail) {

@@ -88,23 +88,35 @@ __global__ void __launch_bounds__(NT) softmax_T_kernel(const __half* __restrict_
 }
 
 // ---------------------------------------------------------------------------------------------
+// BATCH: grid (n_parents, B); sequence b reads the logits row drow_base[node] + b * drow_step[node] of parent node `node`,
+// its rand rows at rand + b * ld_rand_seq, writes tokens + b * ld_seq, and does nothing when frozen.
+template <bool BATCH>
 __global__ void __launch_bounds__(NT) sample_level_kernel(
     const __half* __restrict__ logits, int64_t ld_logits, const __half* __restrict__ rand, int64_t ld_rand,
     const int32_t* __restrict__ parent_rows, const int32_t* __restrict__ child_first,
     const int32_t* __restrict__ n_branch, int k_max, int V, float inv_T, int mode, int64_t* __restrict__ positions,
-    int64_t* __restrict__ tokens, const int32_t* __restrict__ state) {
+    int64_t* __restrict__ tokens, const int32_t* __restrict__ state, const int32_t* __restrict__ drow_base,
+    const int32_t* __restrict__ drow_step, int64_t ld_rand_seq, int64_t ld_seq) {
   __shared__ float red[NW];
   __shared__ uint32_t redu[NW];
   const int j = blockIdx.x;
+  const int b = seq_index<BATCH>(blockIdx.y);
+  if (BATCH) {
+    state += b * ST_WORDS;
+    if (state[ST_FROZEN]) return;
+    tokens += b * ld_seq;
+  }
   const int nb = n_branch ? n_branch[j] : 0;
   const int k_need = positions ? k_max : min(nb, k_max);   // children this row actually needs (block-uniform)
   if (k_need == 0) return;
   const int prow = parent_rows ? parent_rows[j] : j;
+  const int64_t lrow = BATCH ? (int64_t)drow_base[prow] + (int64_t)b * drow_step[prow] : prow;
+  if (BATCH && rand) rand += b * ld_rand_seq;
   const int nvec = V / 8;
   uint32_t key[CH * 8];
   {
     Pack8 x[CH];
-    load_row(logits + prow * ld_logits, V, x);
+    load_row(logits + lrow * ld_logits, V, x);
     if (mode == 0) {
       float mx, sum;
       scale_and_stats(x, inv_T, red, mx, sum);
@@ -507,10 +519,29 @@ extern "C" int sq_sample_level(const sq_half* logits, int64_t ld_logits, const s
   SQ_CHECK_ARG(mode == 1 || rand != nullptr, "sq_sample_level: rand required for mode 0");
   SQ_CHECK_ARG(tokens == nullptr || (child_first && n_branch), "sq_sample_level: tokens needs child_first/n_branch");
   SQ_CHECK_ARG(k_max <= V, "sq_sample_level: k_max > V");
-  sample_level_kernel<<<n_parents, NT, 0, (cudaStream_t)stream>>>((const __half*)logits, ld_logits, (const __half*)rand,
-                                                                 ld_rand, parent_rows, child_first, n_branch, k_max, V,
-                                                                 1.0f / T, mode, positions, tokens, state);
+  sample_level_kernel<false><<<n_parents, NT, 0, (cudaStream_t)stream>>>(
+      (const __half*)logits, ld_logits, (const __half*)rand, ld_rand, parent_rows, child_first, n_branch, k_max, V, 1.0f / T,
+      mode, positions, tokens, state, nullptr, nullptr, 0, 0);
   SQ_CHECK_LAUNCH("sq_sample_level");
+  return SQ_OK;
+}
+
+extern "C" int sq_sample_level_batch(const sq_half* logits, int64_t ld_logits, const int32_t* row_base,
+                                     const int32_t* row_step, const sq_half* rand, int64_t ld_rand, int64_t ld_rand_seq,
+                                     const int32_t* parent_rows, const int32_t* child_first, const int32_t* n_branch,
+                                     int n_parents, int k_max, int V, float T, int mode, int64_t* tokens, int64_t ld_seq,
+                                     const int32_t* state, int B, void* stream) {
+  SQ_CHECK_V(V);
+  SQ_CHECK_ARG(B >= 1 && B <= SQ_MAX_BATCH, "sq_sample_level_batch: B=%d (1..%d)", B, SQ_MAX_BATCH);
+  if (n_parents == 0 || k_max == 0) return SQ_OK;
+  SQ_CHECK_ARG(mode == 1 || rand != nullptr, "sq_sample_level_batch: rand required for mode 0");
+  SQ_CHECK_ARG(tokens && child_first && n_branch && parent_rows && state && row_base && row_step,
+               "sq_sample_level_batch: null table or buffer");
+  SQ_CHECK_ARG(k_max <= V, "sq_sample_level_batch: k_max > V");
+  sample_level_kernel<true><<<dim3(n_parents, B), NT, 0, (cudaStream_t)stream>>>(
+      (const __half*)logits, ld_logits, (const __half*)rand, ld_rand, parent_rows, child_first, n_branch, k_max, V, 1.0f / T,
+      mode, nullptr, tokens, state, row_base, row_step, ld_rand_seq, ld_seq);
+  SQ_CHECK_LAUNCH("sq_sample_level_batch");
   return SQ_OK;
 }
 

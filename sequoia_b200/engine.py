@@ -14,7 +14,7 @@ from typing import List, Optional
 
 import torch
 
-from .kv import KV_Cache
+from .kv import MAX_BATCH, KV_Cache
 from .model import LlamaRunner
 
 F16 = torch.float16
@@ -33,27 +33,44 @@ def _prep_mask(attention_mask: torch.Tensor, n: int):
     return m
 
 
+def _check_batch(batch_size: int, tp_group):
+    if not 1 <= batch_size <= MAX_BATCH:
+        raise ValueError(f"batch_size must be in 1..{MAX_BATCH}, got {batch_size}")
+    if batch_size > 1 and tp_group is not None:
+        raise NotImplementedError("a batch of several sequences runs on one GPU: tensor parallelism needs batch_size=1")
+
+
 class InferenceEngine:
-    """Engine/Engine.py:8-60 (draft)."""
+    """Engine/Engine.py:8-60 (draft).  batch_size > 1: caches and activations for that many sequences
+    (sequoia_b200.batch.BatchTree); the dense-mask methods then refuse, they address one sequence."""
 
     _TG = False
 
-    def __init__(self, max_length: int, model_name_or_path, dtype=torch.float16, device="cuda:0", tp_group=None):
+    def __init__(self, max_length: int, model_name_or_path, dtype=torch.float16, device="cuda:0", tp_group=None,
+                 batch_size: int = 1):
+        _check_batch(batch_size, tp_group)
         if dtype != torch.float16:
             raise NotImplementedError("sequoia_b200 engines are fp16 (reference default)")
         self.device = device
         self.dtype = dtype
         self.max_length = max_length
-        self.runner = LlamaRunner(model_name_or_path, max_length, device=device, tp_group=tp_group)
+        self.batch_size = batch_size
+        self.runner = LlamaRunner(model_name_or_path, max_length, device=device, tp_group=tp_group, batch_size=batch_size)
         self.model = self.runner                      # reference attribute name
         self.model_config = self.runner.cfg
-        self.kv_cache = KV_Cache(config=self.model_config, max_length=max_length, device=device, dtype=dtype,
-                                 k_cache=self.runner.k_cache, v_cache=self.runner.v_cache)
+        self.kv_cache = KV_Cache(config=self.model_config, batch_size=batch_size, max_length=max_length, device=device,
+                                 dtype=dtype, k_cache=self.runner.k_cache, v_cache=self.runner.v_cache)
+
+    def _single(self, what: str):
+        if self.batch_size != 1:
+            raise RuntimeError(f"{what} takes one sequence's dense mask; this engine holds a batch of {self.batch_size} "
+                               "(drive it through sequoia_b200.batch.BatchTree)")
 
     @torch.inference_mode()
     def model_run(self, input_ids: torch.LongTensor, storage_ids: torch.LongTensor,
                   attention_mask: Optional[torch.Tensor] = None, position_ids: Optional[torch.LongTensor] = None,
                   debug: bool = False):
+        self._single("model_run")
         n = input_ids.shape[1]
         if debug:
             assert storage_ids.shape[0] == n
@@ -82,6 +99,7 @@ class InferenceEngine:
         self.kv_cache.initialize_kv(k_cache, v_cache, kv_len)
 
     def gather_kv(self, indices: List[int]):
+        self._single("gather_kv")
         self.kv_cache.gather_kv(indices)
 
     def get_kv_cache(self, in_place=False):
@@ -96,8 +114,9 @@ class InferenceEngineTG(InferenceEngine):
     _TG = True
 
     def __init__(self, max_length: int, model_name_or_path, dtype=torch.float16, device="cuda:0", offloading=False,
-                 tp_group=None):
-        super().__init__(max_length, model_name_or_path, dtype=dtype, device=device, tp_group=tp_group)
+                 tp_group=None, batch_size: int = 1):
+        super().__init__(max_length, model_name_or_path, dtype=dtype, device=device, tp_group=tp_group,
+                         batch_size=batch_size)
         self.offloading = offloading
 
     def set_kv_len(self, kv_len: int):
@@ -139,17 +158,20 @@ def capture_graph(engine: InferenceEngine, decoding_seqlen: int = 1, mempool=Non
 class GraphInferenceEngine:
     """Engine/Engine.py:168-244."""
 
-    def __init__(self, max_length: int, model_name_or_path, dtype=torch.float16, device="cuda:0", tp_group=None):
+    def __init__(self, max_length: int, model_name_or_path, dtype=torch.float16, device="cuda:0", tp_group=None,
+                 batch_size: int = 1):
+        _check_batch(batch_size, tp_group)
         self.device = device
         self.dtype = dtype
         self.max_length = max_length
         self.engine = InferenceEngine(max_length=max_length, model_name_or_path=model_name_or_path, dtype=dtype,
-                                      device=device, tp_group=tp_group)
+                                      device=device, tp_group=tp_group, batch_size=batch_size)
         self.callables = {}
         self.mempool = None
 
     @torch.inference_mode()
     def initialize_cuda_graph(self, decoding_seqlens: List[int], n_warmups=3):
+        self.engine._single("initialize_cuda_graph")
         gc.collect()
         self.mempool = torch.cuda.graphs.graph_pool_handle()
         for decoding_seqlen in decoding_seqlens:
@@ -196,12 +218,13 @@ class GraphInferenceEngineTG:
     """Engine/Engine.py:247-289."""
 
     def __init__(self, max_length: int, model_name_or_path, dtype=torch.float16, device="cuda:0", offloading=False,
-                 tp_group=None):
+                 tp_group=None, batch_size: int = 1):
+        _check_batch(batch_size, tp_group)
         self.device = device
         self.dtype = dtype
         self.max_length = max_length
         self.engine = InferenceEngineTG(max_length=max_length, model_name_or_path=model_name_or_path, dtype=dtype,
-                                        device=device, offloading=offloading, tp_group=tp_group)
+                                        device=device, offloading=offloading, tp_group=tp_group, batch_size=batch_size)
 
     def clear_kv(self):
         drv = getattr(self, "_tp_driver", None)

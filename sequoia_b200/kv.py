@@ -7,9 +7,12 @@ import torch
 
 from . import ops
 
+MAX_BATCH = 8            # SQ_MAX_BATCH (include/sequoia_b200.h)
+
 
 class KV_Cache:
-    """(L, 1, H_kv, M, D) K and V; scatter by storage ids, accepted-path gather / compaction.
+    """(L, B, H_kv, M, D) K and V; scatter by storage ids, accepted-path gather / compaction.  B = batch_size sequences
+    (sequoia_b200.batch); the host-index methods (initialize_kv, gather_kv*) serve B = 1 only.
 
     Mirrors Engine/Llama_KV.py: same constructor, attributes (k_cache, v_cache, kv_offset, num_layers,
     max_length) and methods.  `k_cache` / `v_cache` may be handed in preallocated (the engine binds its TMA
@@ -19,8 +22,9 @@ class KV_Cache:
                  k_cache: Optional[torch.Tensor] = None, v_cache: Optional[torch.Tensor] = None):
         if dtype != torch.float16:
             raise NotImplementedError("sequoia_b200 kernels are fp16 (the reference default dtype)")
-        if batch_size != 1:
-            raise NotImplementedError("batch_size must be 1 (as everywhere in the reference)")
+        if not 1 <= batch_size <= MAX_BATCH:
+            raise ValueError(f"batch_size must be in 1..{MAX_BATCH}, got {batch_size}")
+        self.batch_size = batch_size
         self.config = config
         self.max_length = max_length
         self.device = device
@@ -36,11 +40,18 @@ class KV_Cache:
 
     # Llama_KV.py:38-46
     def initialize_kv(self, k_cache: torch.Tensor, v_cache: torch.Tensor, kv_len: int):
+        self._single("initialize_kv")
         self.k_cache[..., :kv_len, :].copy_(k_cache[..., :kv_len, :])
         self.v_cache[..., :kv_len, :].copy_(v_cache[..., :kv_len, :])
         self.kv_offset = kv_len
 
+    def _single(self, what: str):
+        if self.batch_size != 1:
+            raise RuntimeError(f"KV_Cache.{what} addresses one sequence; this cache holds {self.batch_size} "
+                               "(a batch compacts through ops.kv_gather_batch)")
+
     def _gather(self, indices: List[int], offset: int, zero_tail: bool = True):
+        self._single("gather_kv")
         n = len(indices)
         idx = torch.tensor(list(indices), dtype=torch.int32).to(self.k_cache.device, non_blocking=False) if n else None
         if n:
@@ -64,11 +75,13 @@ class KV_Cache:
         The caller updates kv_offset once it has read the accept length back.  Unlike Llama_KV.py:65-66 the tail rows
         (>= offset + n) are left stale here: every consumer of this path uses the packed tree mask, under which rows
         >= kv_len are never visible (the reference-API gather_kv* methods above do zero the tail, bit-exact)."""
+        self._single("gather_from_state")
         ops.kv_gather(self.k_cache, self.v_cache, accept_idx, 0, 0, state=state, max_n=max_n, zero_tail=zero_tail)
 
     # Llama_KV.py:72-89 (kept for API completeness; the engine's forward appends K/V inside its RoPE kernel)
     def update_kv_cache(self, new_k_cache: torch.Tensor, new_v_cache: torch.Tensor, layer_idx: int,
                         storage_ids: torch.LongTensor, debug: bool = False):
+        self._single("update_kv_cache")
         input_length = len(storage_ids)
         if debug:
             assert input_length == new_k_cache.shape[-2]

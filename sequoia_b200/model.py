@@ -216,15 +216,17 @@ def load_sharded_weights(cfg: LlamaConfigLite, src, rank: int, tp: int) -> dict:
 class LlamaRunner:
     """Weights + preallocated activations + attention plan of one engine."""
 
-    def __init__(self, model_name_or_path, max_length: int, device="cuda:0", tp_group=None, n_max: Optional[int] = None):
+    def __init__(self, model_name_or_path, max_length: int, device="cuda:0", tp_group=None, n_max: Optional[int] = None,
+                 batch_size: int = 1):
         self.device = torch.device(device)
+        self.B = batch_size
         self.cfg, src = resolve_model(model_name_or_path, self.device)
         cfg = self.cfg
         self.tp = TPInfo(tp_group)
         tp, r = self.tp.size, self.tp.rank
         assert cfg.num_attention_heads % tp == 0 and cfg.num_key_value_heads % tp == 0 and cfg.intermediate_size % tp == 0
         self.M = max_length
-        self.n_max = n_max or max_length
+        self.n_max = n_max or max_length * batch_size        # batch: B sequences' rows, sequence-major
         self.H, self.Hkv, self.D = cfg.num_attention_heads // tp, cfg.num_key_value_heads // tp, cfg.head_dim
         self.I = cfg.intermediate_size // tp
         h, D, V = cfg.hidden_size, self.D, cfg.vocab_size
@@ -241,7 +243,7 @@ class LlamaRunner:
         self.attn_out, self.proj = z(n, self.H * D), z(n, h)
         self.gate_up, self.act = z(n, 2 * self.I), z(n, self.I)
         self.logits = z(n, V)
-        self.k_cache = torch.zeros(self.L, 1, self.Hkv, max_length, D, dtype=F16, device=dev)
+        self.k_cache = torch.zeros(self.L, batch_size, self.Hkv, max_length, D, dtype=F16, device=dev)
         self.v_cache = torch.zeros_like(self.k_cache)
         self.plan = ops.AttnPlan(self.qkv, n, self.H, self.Hkv, D, self.k_cache, self.v_cache, self.attn_out)
         # Dense GEMMs.  Default ("auto"): the weight-streaming shapes given to the hand-written wgmma kernel (csrc/sq_gemm.cu) -- gate_up with the SwiGLU epilogue fused (weights interleaved + pre-tiled, `act` written directly: no
@@ -280,7 +282,7 @@ class LlamaRunner:
         self.draft_plan = None
         self.draft_fused = os.environ.get("SQ_DRAFT_FUSED", "0") not in ("0", "")
         self.draft_attn = os.environ.get("SQ_DRAFT_ATTN", "1") != "0"
-        if ((self.draft_fused or self.draft_attn) and tp == 1 and not self.gu_interleaved and
+        if ((self.draft_fused or self.draft_attn) and tp == 1 and batch_size == 1 and not self.gu_interleaved and
                 ops.draft_supported(h, self.I, self.L, self.H, self.Hkv, D, V, max_length)):
             self.draft_plan = ops.DraftPlan(h, self.I, self.H, V, max_length, self.eps, self.embed, self.layers, self.norm,
                                             self.lm_head, self.cos, self.sin, self.k_cache, self.v_cache)
@@ -360,32 +362,50 @@ class LlamaRunner:
     def forward(self, n: int, tokens: torch.Tensor, position_ids: torch.Tensor, storage_ids: torch.Tensor, *,
                 state=None, n0: int = 0, kv_end: int = 0, prefix_len: int = 0, dense_mask=None, mask_ld: int = 0,
                 tree_bits=None, tree_words: int = 0, tree_size: int = 0, logits_out: Optional[torch.Tensor] = None,
-                logits_from: int = 0, skip_lm_head: bool = False) -> Optional[torch.Tensor]:
+                logits_from: int = 0, skip_lm_head: bool = False, batch: bool = False,
+                logits_to: Optional[int] = None) -> Optional[torch.Tensor]:
         """Forward `n` rows.  Row r is token tokens[base+r] at position position_ids[base+r], written to cache slot
         storage_ids[base+r], base = (state ? P-1 : 0) + n0.  Attends slots [0, (state ? P-1 : 0) + kv_end).
-        Logits of rows [logits_from, n) are written to `logits_out` (default: the internal buffer) and returned."""
-        assert 0 < n <= self.n_max
+        Logits of rows [logits_from, logits_to or n) are written to `logits_out` (default: the internal buffer) and
+        returned.
+        batch=True: `n` rows for each of the B sequences of the engine, in tree-relative addressing of each one's state
+        row (state (B, 16), tokens / position_ids / storage_ids (B, M)); activation rows are sequence-major, so the
+        row-wise ops and the GEMMs see B*n rows and logits_from / logits_to index those."""
+        B = self.B if batch else 1
+        N = n * B
+        assert 0 < N <= self.n_max
+        assert not batch or (state is not None and dense_mask is None)
         H, Hkv, D, M = self.H, self.Hkv, self.D, self.M
-        small = (self.draft_plan is not None and state is not None and n <= ops.DraftPlan.MAX_ROWS and dense_mask is None
-                 and self.attn_impl == 0)
+        small = (not batch and self.draft_plan is not None and state is not None and n <= ops.DraftPlan.MAX_ROWS
+                 and dense_mask is None and self.attn_impl == 0)
         if small and self.draft_fused and logits_from == 0 and not skip_lm_head:
             out = logits_out if logits_out is not None else self.logits[:n]
             self.draft_plan.forward(n, tokens, position_ids, storage_ids, state, n0, kv_end, tree_bits, tree_words,
                                     tree_size, out)
             return out
-        hid, nrm = self.hidden[:n], self.normed[:n]
-        ops.embed_rows(self.embed, tokens, n, self.hidden, state=state, n0=n0)
+        if batch:
+            ops.embed_rows_batch(self.embed, tokens, n, self.hidden, state, n0=n0)
+        else:
+            ops.embed_rows(self.embed, tokens, n, self.hidden, state=state, n0=n0)
+        n_seq, n = n, N                                # from here on n counts the rows of all sequences
         ops.rmsnorm(self.hidden, self.layers[0]["ln1"], self.normed, n, self.eps)
         for l, ly in enumerate(self.layers):
             self._prefetch_join()
             self._linear(l, "qkv", self.normed, ly["wqkv"], self.qkv, n)
             if self.pf_budget is not None:          # window A: RoPE + attention
                 self._prefetch(0, [(ly["wo"], 0), (ly["wgu"], 0)])
-            ops.rope_kv_append(self.qkv, H, Hkv, D, self.cos, self.sin, position_ids, storage_ids, n,
-                               self.k_cache[l], self.v_cache[l], M, state=state, n0=n0)
-            if small and self.draft_attn:
+            if batch:
+                ops.rope_kv_append_batch(self.qkv, H, Hkv, D, self.cos, self.sin, position_ids, storage_ids, n_seq,
+                                         self.k_cache[l], self.v_cache[l], M, state, n0=n0)
+                ops.tree_attn_batch(self.plan, l, n_seq, state=state, n0=n0, kv_end=kv_end, tree_bits=tree_bits,
+                                    tree_words=tree_words, tree_size=tree_size)
+            elif small and self.draft_attn:
+                ops.rope_kv_append(self.qkv, H, Hkv, D, self.cos, self.sin, position_ids, storage_ids, n,
+                                   self.k_cache[l], self.v_cache[l], M, state=state, n0=n0)
                 self.draft_plan.attention(l, n, self.qkv, self.attn_out, state, n0, kv_end, tree_bits, tree_words, tree_size)
             else:
+                ops.rope_kv_append(self.qkv, H, Hkv, D, self.cos, self.sin, position_ids, storage_ids, n,
+                                   self.k_cache[l], self.v_cache[l], M, state=state, n0=n0)
                 ops.tree_attn(self.plan, l, n, state=state, n0=n0, kv_end=kv_end, prefix_len=prefix_len,
                               dense_mask=dense_mask, mask_ld=mask_ld, tree_bits=tree_bits, tree_words=tree_words,
                               tree_size=tree_size, impl=self.attn_impl)
@@ -420,10 +440,11 @@ class LlamaRunner:
             self._prefetch_join()
             return None
         self._prefetch_join()
-        m = n - logits_from
+        end = n if logits_to is None else logits_to
+        m = end - logits_from
         out = logits_out if logits_out is not None else self.logits[:m]
         if self.lm_plan is not None and m <= 128 and out.stride(-1) == 1 and out.stride(0) % 8 == 0 and out.data_ptr() % 16 == 0:
             self.lm_plan.run(m, a_row0=logits_from, out=out)
         else:
-            torch.mm(self.normed[logits_from:n], self.lm_head.t(), out=out)
+            torch.mm(self.normed[logits_from:end], self.lm_head.t(), out=out)
         return out

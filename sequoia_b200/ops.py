@@ -70,19 +70,21 @@ def kv_gather_big(k_cache, v_cache, idx, n, offset, zero_tail=False):
 
 
 class AttnPlan:
-    """TMA descriptors + split-KV workspace for one (qkv buffer, KV cache, output buffer) triple."""
+    """TMA descriptors + split-KV workspace for one (qkv buffer, KV cache, output buffer) triple.  A (L, B, Hkv, M, D) cache
+    with B > 1 makes a batch plan, launched through `tree_attn_batch` (n_max then counts the rows of all B sequences)."""
 
     def __init__(self, qkv: torch.Tensor, n_max: int, H: int, Hkv: int, D: int, k_cache, v_cache, out):
         lib = _lib.load()
-        L, _, hk, M, d = k_cache.shape
+        L, B, hk, M, d = k_cache.shape
         assert hk == Hkv and d == D
         nbytes = lib.sq_attn_workspace_bytes(n_max, H, D, M)
         self.workspace = torch.zeros(nbytes, dtype=torch.uint8, device=qkv.device)
         self.handle = C.c_void_p()
         self._keep = (qkv, k_cache, v_cache, out)
-        check(lib.sq_attn_plan_create(C.byref(self.handle), ptr(qkv), qkv.shape[-1], n_max, H, Hkv, D, ptr(k_cache),
-                                      ptr(v_cache), L, M, ptr(out), ptr(self.workspace), nbytes), "sq_attn_plan_create")
-        self.n_max, self.M = n_max, M
+        check(lib.sq_attn_plan_create_batch(C.byref(self.handle), ptr(qkv), qkv.shape[-1], n_max, H, Hkv, D, ptr(k_cache),
+                                            ptr(v_cache), L, B, M, ptr(out), ptr(self.workspace), nbytes),
+              "sq_attn_plan_create_batch")
+        self.n_max, self.M, self.B = n_max, M, B
 
     def error(self) -> int:
         return _lib.load().sq_attn_plan_error(self.handle)
@@ -315,3 +317,89 @@ class DraftPlan:
                 self.handle = None
         except Exception:
             pass
+
+
+# ---- batches of B sequences sharing one growmap (include/sequoia_b200.h, "batches") ------------------------------------------
+# Per-sequence buffers are (B, ...) tensors: state (B, 16) int32, tokens / position_ids / storage_ids / r (B, M), accept_idx
+# (B, >= S) int32, noise (B, >= V); activation rows are sequence-major (sequence b's n rows start at row b * n).  Draft logits:
+# node k of sequence b at row row_base[k] + b * row_step[k] (see draft_row_tables).
+def _rows(t, name):
+    if t.dim() != 2 or t.stride(-1) != 1:
+        raise ValueError(f"{name}: expected a (B, ...) tensor with contiguous rows, got {tuple(t.shape)}")
+    return t.stride(0)
+
+
+def draft_row_tables(levels, S: int, B: int, device):
+    """(row_base, row_step) int32 tables of S entries for a draft-logit buffer holding each tree level (n0, tb) as one block
+    of B * tb rows at row B * n0: row of node k of sequence b = row_base[k] + b * row_step[k].  Node 0 (the root) is
+    level (0, 1)."""
+    base, step = [0] * S, [1] * S
+    for n0, tb in levels:
+        for k in range(n0, n0 + tb):
+            base[k], step[k] = B * n0 + (k - n0), tb
+    i32 = lambda x: torch.tensor(x, dtype=torch.int32, device=device)
+    return i32(base), i32(step)
+
+
+def embed_rows_batch(table, tokens, n, out, state, n0=0):
+    B = state.shape[0]
+    check(_lib.load().sq_embed_rows_batch(ptr(table), ptr(tokens), _rows(tokens, "tokens"), ptr(state), n0, n, B,
+                                          table.shape[1], ptr(out), stream_ptr()), "sq_embed_rows_batch")
+
+
+def rope_kv_append_batch(qkv, H, Hkv, D, cos, sin, position_ids, storage_ids, n, k_layer, v_layer, M, state, n0=0):
+    """k_layer / v_layer: (B, Hkv, M, D) = one layer of a (L, B, Hkv, M, D) cache."""
+    B = state.shape[0]
+    ld = _rows(position_ids, "position_ids")
+    assert _rows(storage_ids, "storage_ids") == ld and k_layer.shape[0] == B
+    check(_lib.load().sq_rope_kv_append_batch(ptr(qkv), qkv.shape[-1], H, Hkv, D, ptr(cos), ptr(sin), ptr(position_ids),
+                                              ptr(storage_ids), ld, ptr(state), n0, n, B, ptr(k_layer), ptr(v_layer), M,
+                                              stream_ptr()), "sq_rope_kv_append_batch")
+
+
+def kv_gather_batch(k_cache, v_cache, accept_idx, state, max_n):
+    L, B, Hkv, M, D = k_cache.shape
+    assert state.shape[0] == B and accept_idx.dtype == torch.int32
+    check(_lib.load().sq_kv_gather_batch(ptr(k_cache), ptr(v_cache), L, B, Hkv, M, D, ptr(accept_idx),
+                                         _rows(accept_idx, "accept_idx"), ptr(state), max_n, stream_ptr()),
+          "sq_kv_gather_batch")
+
+
+def tree_attn_batch(plan: AttnPlan, layer, n, *, state, n0=0, kv_end=0, tree_bits=None, tree_words=0, tree_size=0):
+    check(_lib.load().sq_tree_attn_batch(plan.handle, layer, n, state.shape[0], ptr(state), n0, kv_end, ptr(tree_bits),
+                                         tree_words, tree_size, stream_ptr()), "sq_tree_attn_batch")
+
+
+def sample_level_batch(logits, row_base, row_step, rand, n_parents, k_max, T, mode, *, parent_rows, child_first, n_branch,
+                       tokens, state):
+    """rand: (B, S, V) (mode 0) or None (mode 1, top-k)."""
+    if rand is not None:
+        assert rand.dim() == 3 and rand.stride(-1) == 1
+    check(_lib.load().sq_sample_level_batch(
+        ptr(logits), logits.stride(0), ptr(row_base), ptr(row_step), ptr(rand), rand.stride(1) if rand is not None else 0,
+        rand.stride(0) if rand is not None else 0, ptr(parent_rows), ptr(child_first), ptr(n_branch), n_parents, k_max,
+        logits.shape[-1], T, mode, ptr(tokens), _rows(tokens, "tokens"), ptr(state), state.shape[0], stream_ptr()),
+        "sq_sample_level_batch")
+
+
+def accept_stochastic_batch(target_logits, draft_logits, row_base, row_step, r, noise, succ_off, succ, depth, S, T, tokens,
+                            position_ids, accept_idx, state, max_target_seq, policy=0):
+    """target_logits (B*S, V); r, tokens, position_ids (B, M); noise (B, V); accept_idx (B, >= S)."""
+    V = target_logits.shape[-1]
+    ld = _rows(tokens, "tokens")
+    assert _rows(position_ids, "position_ids") == ld and _rows(r, "r") == ld
+    check(_lib.load().sq_accept_stochastic_batch(
+        ptr(target_logits), target_logits.stride(0), ptr(draft_logits), draft_logits.stride(0), ptr(row_base),
+        ptr(row_step), ptr(r), ptr(noise), _rows(noise, "noise"), ptr(succ_off), ptr(succ), ptr(depth), S, V, T,
+        ptr(tokens), ptr(position_ids), ld, ptr(accept_idx), _rows(accept_idx, "accept_idx"), ptr(state), state.shape[0],
+        max_target_seq, policy, stream_ptr()), "sq_accept_stochastic_batch")
+
+
+def accept_greedy_batch(target_token, succ_off, succ, depth, S, tokens, position_ids, accept_idx, state, max_target_seq):
+    """target_token (B*S) int64."""
+    ld = _rows(tokens, "tokens")
+    assert _rows(position_ids, "position_ids") == ld
+    check(_lib.load().sq_accept_greedy_batch(ptr(target_token), ptr(succ_off), ptr(succ), ptr(depth), S, ptr(tokens),
+                                             ptr(position_ids), ld, ptr(accept_idx), _rows(accept_idx, "accept_idx"),
+                                             ptr(state), state.shape[0], max_target_seq, stream_ptr()),
+          "sq_accept_greedy_batch")

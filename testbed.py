@@ -171,6 +171,45 @@ def simulation_baseline(target, prompts, T, top_p, M, new_tokens: int = 32):
     return dict(decoded_tokens=decoded, seconds=total_time, latency=total_time / max(decoded, 1))
 
 
+@torch.inference_mode()
+def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: int):
+    """--batch B: the same metric loop with B prompts decoded together (sequoia_b200.batch.BatchTree)."""
+    from sequoia_b200.batch import BatchTree
+    steps = decoded = 0                          # steps: target steps summed over sequences (per-sequence tokens / step)
+    total_time = 0.0
+    for i in range(0, len(prompts), B):
+        chunk = [p.to(DEV) for p in prompts[i:i + B]]
+        tree = BatchTree(draft, target, chunk, grow_map, policy=policy, temperature=T, top_p=top_p, max_length=M,
+                         max_target_seq=M)
+        length = [len(p) for p in chunk]
+        done = set()
+        torch.cuda.synchronize()
+        t1 = time.time()
+        while not all(tree.frozen):
+            tree.construct_grow_map()
+            for b, (valid, _, terminate) in enumerate(tree.verify()):
+                if b in done:
+                    continue
+                decoded += valid.shape[0] - length[b]
+                steps += 1
+                length[b] = valid.shape[0]
+                last = int(valid[-1]) if valid.shape[0] else 0
+                if terminate or last in (0, 2) or length[b] >= MAX_NEW_LEN:
+                    done.add(b)
+                    if not tree.frozen[b]:
+                        tree.freeze(b)
+        torch.cuda.synchronize()
+        total_time += time.time() - t1
+        draft.clear_kv()
+        target.clear_kv()
+    steps = max(steps, 1)
+    print("total time :{:.5f}s, latency :{:.5f}s, decoding step: {}, large model step: {}, {}".format(
+        total_time, total_time / max(decoded, 1), decoded, steps, decoded / steps))
+    print("batch {}: aggregate {:.2f} tokens/s".format(B, decoded / total_time if total_time > 0 else 0.0))
+    return dict(decoded_tokens=decoded, target_steps=steps, tokens_per_step=decoded / steps, seconds=total_time,
+                tokens_per_second=decoded / total_time if total_time > 0 else 0.0, batch=B)
+
+
 def build_parser():
     ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
     ap.add_argument("--model", type=str, default="random-init:llama-68m", help="draft model")
@@ -186,6 +225,8 @@ def build_parser():
     ap.add_argument("--Mode", type=str, default="greedy", choices=["greedy", "benchmark", "baseline"])
     ap.add_argument("--tree", type=str, default="spec", choices=["spec", "greedy", "specinfer", "greedys"])
     ap.add_argument("--offloading", action="store_true", help="use OffloadEngine for the target (weights stay resident)")
+    ap.add_argument("--batch", type=int, default=1,
+                    help="decode this many prompts together (--Mode greedy, --tree spec|greedy; the prompt count must divide)")
     return ap
 
 
@@ -197,6 +238,21 @@ def main(argv=None):
     from Engine.offload_engine import OffloadEngine
     prompts = load_prompts(args.dataset, args.start, args.end, args.seed)
     tcls = OffloadEngine if args.offloading else GraphInferenceEngineTG
+    if args.batch != 1:
+        if args.Mode != "greedy" or args.tree not in ("spec", "greedy") or args.offloading:
+            raise SystemExit("--batch runs --Mode greedy with --tree spec or greedy, without --offloading")
+        if len(prompts) % args.batch:
+            raise SystemExit(f"--batch {args.batch} must divide the {len(prompts)} prompts")
+        target = GraphInferenceEngineTG(max_length=args.M, model_name_or_path=args.target, dtype=torch.float16,
+                                        device=DEV, batch_size=args.batch)
+        draft = GraphInferenceEngine(max_length=args.M, model_name_or_path=args.model, dtype=torch.float16, device=DEV,
+                                     batch_size=args.batch)
+        path = args.growmap if os.path.isabs(args.growmap) or os.path.exists(args.growmap) else os.path.join(ROOT, args.growmap)
+        grow_map = torch.load(path)
+        assert args.M >= MAX_NEW_LEN + grow_map["size"], "--M must hold 256 tokens + the tree (README.md:47 of the reference)"
+        res = simulation_batch(target, draft, prompts, grow_map, args.tree, args.T, args.P, args.M, args.batch)
+        print(json.dumps({k: (round(v, 5) if isinstance(v, float) else v) for k, v in res.items()}))
+        return res
     target = tcls(max_length=args.M, model_name_or_path=args.target, dtype=torch.float16, device=DEV)
     if args.Mode == "baseline":
         res = simulation_baseline(target, prompts, args.T, args.P, args.M)
