@@ -193,11 +193,6 @@ int sq_accept_greedy(const int64_t* target_token, const int32_t* succ_off, const
                      const int32_t* depth, int S, int64_t* tokens, int64_t* position_ids, int32_t* accept_idx,
                      int32_t* state, int max_target_seq, void* stream);
 
-/* ---- L2 prefetch of upcoming weights (no reference counterpart; a hint, never changes results) ----
- * Issues cp.async.bulk.prefetch.L2 for the panel base[r*pitch + off, + seg) of rows r < rows (all in bytes, multiples
- * of 16).  Meant for a forked stream next to the latency-bound kernels between two weight GEMMs. */
-int sq_l2_prefetch(const void* base, int64_t pitch_bytes, int rows, int64_t off_bytes, int64_t seg_bytes, void* stream);
-
 /* ---- weight-streaming GEMM for <= 128 rows (nn.Linear, Llama_modules.py:108-110,138,270-272; Llama_model.py:213) ---- */
 
 /* C[n, N] = A[n, K] * W[N, K]^T, fp16 in / fp32 accumulate / fp16 out, n <= 128.  A: (n_max, lda), W: (N, K) row-major
@@ -282,28 +277,19 @@ int sq_tp_ll_publish(void* const* host_mbox_ptrs, int n_peers, int cap_words, ui
 int sq_tp_ll_consume(const void* mbox_local, int cap_words, uint32_t* epoch, uint32_t* err, void* dst0, int words0, void* dst1,
                      int words1, void* dst2, int words2, void* stream);
 
-/* ---- fused draft forward (csrc/sq_draft.cu): one persistent cooperative kernel per tree level for small draft models
- * (Engine/Engine.py:158-164 replays a ~25-kernel graph per level; Tree/SpecTree.py:245-259).  Supported: head_dim 64,
- * n_heads * 64 == hidden, no GQA, intermediate %% hidden == 0, <= 16 layers, max_length <= 640 (the attention phase keeps
- * a head's K and V in shared memory; see sq_draft_supported).
- * layer_weights: 6 pointers per layer {wqkv (3h,h), wo (h,h), wgu (2I,h), wd (h,I), input_layernorm, post_attention_layernorm}.
- * workspace: sq_draft_workspace_bytes(hidden, intermediate) bytes of device memory owned by the caller. ---- */
+/* ---- draft attention (csrc/sq_draft.cu): tree-masked attention of the small draft model's forwards of <= 64 rows
+ * (Engine/Llama_modules.py:127-134 inside the per-level graph of Engine/Engine.py:158-164).  Supported: head_dim 64,
+ * n_heads * 64 == hidden, no GQA, max_length <= 640 (a head's K and V live in shared memory; see sq_draft_supported).
+ * k_cache / v_cache: (n_layers, 1, n_heads, max_length, 64). ---- */
 typedef struct sq_draft_plan sq_draft_plan;
-int64_t sq_draft_workspace_bytes(int hidden, int inter);
-int sq_draft_supported(int hidden, int inter, int n_layers, int n_heads, int n_kv_heads, int head_dim, int vocab, int max_length);
-int sq_draft_plan_create(sq_draft_plan** plan, int hidden, int inter, int n_layers, int n_heads, int vocab, int max_length,
-                         float eps, const sq_half* embed, const sq_half* const* layer_weights, const sq_half* final_norm,
-                         const sq_half* lm_head, const sq_half* cos, const sq_half* sin, sq_half* k_cache, sq_half* v_cache,
-                         void* workspace, int64_t workspace_bytes);
+int sq_draft_supported(int hidden, int n_heads, int n_kv_heads, int head_dim, int max_length);
+int sq_draft_plan_create(sq_draft_plan** plan, int hidden, int n_layers, int n_heads, int max_length, sq_half* k_cache,
+                         sq_half* v_cache);
 int sq_draft_plan_destroy(sq_draft_plan* plan);
-/* Forward n (<= 64) rows = tree nodes [n0, n0+n) in tree-relative addressing (base = state[P]-1: tokens / positions / cache
- * slots at base+n0+r; keys [0, base+kv_end) under the packed tree mask); appends their K/V, writes logits_out (n, V). */
-int sq_draft_forward(sq_draft_plan* plan, int n, const int64_t* tokens, const int64_t* position_ids, const int64_t* storage_ids,
-                     const int32_t* state, int n0, int kv_end, const uint32_t* tree_bits, int tree_words, int tree_size,
-                     sq_half* logits_out, int64_t ld_logits, void* stream);
 
-/* Only the attention phase of `layer`, as one launch on caller-owned buffers: q rows from `qkv` (n, 3*hidden), K/V from the
- * plan's caches (rows already appended), output (n, hidden).  Small-shape alternative to sq_tree_attn for draft forwards. */
+/* Attention of `layer` for n (<= 64) rows = tree nodes [n0, n0+n) in tree-relative addressing (base = state[P]-1; keys
+ * [0, base+kv_end) under the packed tree mask), as one launch on caller-owned buffers: q rows from `qkv` (n, 3*hidden),
+ * K/V from the plan's caches (rows already appended), output (n, hidden).  Small-shape alternative to sq_tree_attn. */
 int sq_draft_attention(sq_draft_plan* plan, int layer, int n, const sq_half* qkv, sq_half* attn_out, const int32_t* state,
                        int n0, int kv_end, const uint32_t* tree_bits, int tree_words, int tree_size, void* stream);
 

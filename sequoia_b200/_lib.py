@@ -46,7 +46,6 @@ _SIGNATURES = {
     "sq_top_p_filter": (i32, [vp, i64, i32, i32, f32, f32, vp]),
     "sq_accept_stochastic": (i32, [vp, i64, vp, i64, vp, vp, vp, vp, vp, i32, i32, f32, vp, vp, vp, vp, i32, i32, vp]),
     "sq_accept_greedy": (i32, [vp, vp, vp, vp, i32, vp, vp, vp, vp, i32, vp]),
-    "sq_l2_prefetch": (i32, [vp, i64, i32, i64, i64, vp]),
     "sq_gemm_plan_create": (i32, [C.POINTER(vp), vp, i32, i32, vp, i32, i32, vp, i32, vp]),
     "sq_gemm_pick_tiles": (i32, [i32, i32, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32)]),
     "sq_gemm_pick_tiles_ex": (i32, [i32, i32, i32, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32)]),
@@ -68,12 +67,10 @@ _SIGNATURES = {
     "sq_tp_allreduce_ll_add_rmsnorm": (i32, [vp, vp, vp, vp, vp, i32, i32, i32, i32, vp, vp, i32, i32, f32, vp]),
     "sq_tp_ll_publish": (i32, [vp, i32, i32, vp, vp, i32, vp, i32, vp, i32, vp]),
     "sq_tp_ll_consume": (i32, [vp, i32, vp, vp, vp, i32, vp, i32, vp, i32, vp]),
-    "sq_draft_workspace_bytes": (i64, [i32, i32]),
-    "sq_draft_supported": (i32, [i32, i32, i32, i32, i32, i32, i32, i32]),
-    "sq_draft_plan_create": (i32, [C.POINTER(vp), i32, i32, i32, i32, i32, i32, f32, vp, vp, vp, vp, vp, vp, vp, vp, vp, i64]),
+    "sq_draft_supported": (i32, [i32, i32, i32, i32, i32]),
+    "sq_draft_plan_create": (i32, [C.POINTER(vp), i32, i32, i32, i32, vp, vp]),
     "sq_draft_plan_destroy": (i32, [vp]),
     "sq_draft_attention": (i32, [vp, i32, i32, vp, vp, vp, i32, i32, vp, i32, i32, vp]),
-    "sq_draft_forward": (i32, [vp, i32, vp, vp, vp, vp, i32, i32, vp, i32, i32, vp, i64, vp]),
     "sq_embed_rows_batch": (i32, [vp, vp, i64, vp, i32, i32, i32, i32, vp, vp]),
     "sq_rope_kv_append_batch": (i32, [vp, i32, i32, i32, i32, vp, vp, vp, vp, i64, vp, i32, i32, i32, vp, vp, i32, vp]),
     "sq_kv_gather_batch": (i32, [vp, vp, i32, i32, i32, i32, i32, vp, i32, vp, i32, vp]),

@@ -1,57 +1,38 @@
-// Draft-model forward of one tree level as ONE persistent cooperative kernel (SURVEY.md 8f.2; the reference's cost centre
-// Engine/Engine.py:158-164 + Tree/SpecTree.py:245-259: one CUDA-graph replay of a ~25-launch forward per level).
+// Tree-masked attention for the small draft model's forwards of <= 64 rows (the reference's draft SDPA,
+// Engine/Llama_modules.py:127-134, inside the per-level graph replay of Engine/Engine.py:158-164).
 //
-// The JackFram-68m-class draft (hidden 768, 2 layers, ~77 MB of weights incl. lm_head; mostly L2-resident in the H100's
-// 50 MB L2) has at most a few dozen rows per tree level, so the forward is launch / dependency latency: ~22 kernels.  Here
-// all SMs stay resident and walk through the phases of the forward separated by grid barriers:
-//
-//   P0  embed rows -> hidden
-//   per layer:  A  RMSNorm (prologue, recomputed per CTA) + q/k/v GEMM + RoPE + KV append (epilogue)
-//               B  tree-masked attention, one (head, 16-row tile) per CTA, 8 warps split the keys (flash-decoding)
-//               C  o_proj GEMM + residual add (epilogue)
-//               D  RMSNorm (prologue) + gate/up GEMM + SiLU * up (epilogue)
-//               E  down_proj GEMM, split along K into chunks of `hidden` columns -> fp32 partials
-//               E2 residual add of the summed partials (row-parallel)
-//   F   final RMSNorm (prologue) + lm_head GEMM -> logits
-//
-// GEMMs: mma.sync m16n8k16 (fp16 in, fp32 accumulate) -- at <= 64 rows and L2-resident weights the tensor-core generation
-// is irrelevant, what matters is the number of dependent phases; activations (<= 64 x hidden) sit in shared memory as the A
-// operand, weight rows are streamed with cp.async in double-buffered 32-row sub-tiles.  Rounding points are those of the
-// multi-kernel path (csrc/sq_elementwise.cu, reference fp16 semantics): GEMM outputs, RMSNorm (x*inv -> fp16 -> *w ->
-// fp16), RoPE products, SiLU, residual adds all round to fp16 where torch does.
-#include <cooperative_groups.h>
-
-#include <cstdio>
-#include <cstdlib>
-
+// A JackFram-68m-class draft (head_dim 64, no GQA) runs each tree level as a forward of a few dozen rows against a prefix
+// of at most max_length keys.  At that size the wgmma tree attention's 128-row tiles are mostly padding, so this kernel
+// takes one (head, 16-row tile) per CTA: the head's whole K and V are staged into shared memory with cp.async, the 8
+// warps take 32-key blocks round-robin (mma.sync m16n8k16, fp16 in, fp32 accumulate, online softmax per warp), and the
+// per-warp (max, sum, O) partials are combined through shared memory in warp order (deterministic).  Rounding points:
+// P rounds to fp16 as the A operand of PV, the output rounds to fp16 once.  The shared-memory footprint bounds max_length
+// (640 for head_dim 64, see sq_draft_supported).
 #include "sq_common.cuh"
 #include "sq_mask.cuh"
-
-namespace cg = cooperative_groups;
 
 namespace sq {
 
 constexpr int DT = 256;            // threads per CTA (8 warps)
 constexpr int DPAD = 8;            // shared-memory row padding (halfs): conflict-free ldmatrix
-constexpr int D_MAXL = 16;
-constexpr int D_ROWS = 64;         // max rows per forward
+constexpr int D_ROWS = 64;         // max rows per launch
 constexpr int HD = 64;             // head dim
 
-struct DraftArgs {
-  int h, I, L, H, V, M, n, n0, kv_end, ks;
-  float eps, scale;
-  const __half *embed, *fnorm, *lm_head, *cosc, *sinc;
-  const __half* w[D_MAXL][6];      // wqkv (3h,h), wo (h,h), wgu (2I,h), wd (h,I), ln1, ln2
-  __half *k_cache, *v_cache;       // (L,1,H,M,64)
-  __half *hidden, *qkv, *attn, *act;
-  float* partial;                  // (ks, 64, h)
-  const int64_t *tokens, *position_ids, *storage_ids;
+struct DraftAttnArgs {
+  int h, H, M, n, n0, kv_end;
+  float scale;
+  const __half *k_cache, *v_cache;   // this layer's (H, M, 64) planes
+  const __half* qkv;                 // (n, 3h): q part read
+  __half* attn;                      // (n, h)
   const int32_t* state;
   const uint32_t* tree_bits;
   int tree_words, tree_size;
-  __half* logits;
-  int64_t ld_logits;
 };
+
+// dynamic shared memory: K_s, V_s [kv_pad][72] | Q_s [16][72] halfs | O partials [8][16][64] | max, sum [8][16] floats
+static size_t draft_attn_smem(int max_length) {
+  return (size_t)(2 * ((max_length + 31) & ~31) + 16) * (HD + DPAD) * 2 + (8 * 16 * 64 + 2 * 8 * 16) * 4;
+}
 
 __device__ __forceinline__ uint32_t s_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void cp16(void* smem, const void* g) {
@@ -77,535 +58,181 @@ __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
   return *reinterpret_cast<const uint32_t*>(&h);
 }
 
-// Shared memory: A_s [64][K+8] | W_s 2 x [32][K+8] | red (K-split partial accumulators) | misc
-struct DraftSmem {
-  __half* A;
-  __half* W[2];
-  float* red;
-  int ld;      // row pitch in halfs (K + 8)
-};
-
-// A_s <- rows of `src` (pitch ld_src halfs, `cols` columns starting at col0), rows >= n zero-filled; optional RMSNorm with
-// weight `nw` (nullptr = plain copy).  cols % 8 == 0.  All rows are fetched with cp.async first (one L2 round trip for the
-// whole tile instead of one per loop iteration), the norm then runs out of shared memory.  Waits for ALL outstanding
-// cp.async groups of the thread (weight sub-tiles issued before the call land under the same wait) and ends with a block
-// barrier.
-__device__ void load_A(const DraftSmem& sm, const __half* src, int64_t ld_src, int col0, int cols, int n, int n_pad,
-                       const __half* nw, float eps, bool chain) {
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int cv = cols / 8;
-  if (chain) pdl_wait();      // chained launches: the activations come from the previous kernel (weights were requested before)
-  for (int i = tid; i < n_pad * cv; i += DT) {
-    const int r = i / cv, c = i % cv;
-    __half* dst = sm.A + r * sm.ld + c * 8;
-    if (r < n) cp16(dst, src + r * ld_src + col0 + c * 8);
-    else *reinterpret_cast<uint4*>(dst) = make_uint4(0, 0, 0, 0);
-  }
-  cp_commit();
-  cp_wait<0>();
-  __syncthreads();
-  if (nw != nullptr) {
-    // one warp per row: sum of squares, then x * inv -> fp16 -> * w -> fp16   (rmsnorm_kernel's arithmetic)
-    for (int r = warp; r < n; r += DT / 32) {
-      float ss = 0.f;
-      for (int c = lane; c < cv; c += 32) {
-        Pack8 v;
-        v.u = *reinterpret_cast<const uint4*>(sm.A + r * sm.ld + c * 8);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) { const float f = h2f(v.h[j]); ss += f * f; }
-      }
-      ss = warp_sum(ss);
-      const float inv = rsqrtf(ss / (float)cols + eps);
-      for (int c = lane; c < cv; c += 32) {
-        Pack8 v, wv, o;
-        v.u = *reinterpret_cast<const uint4*>(sm.A + r * sm.ld + c * 8);
-        wv.u = *reinterpret_cast<const uint4*>(nw + c * 8);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) o.h[j] = f2h(h2f(wv.h[j]) * h2f(f2h(h2f(v.h[j]) * inv)));
-        *reinterpret_cast<uint4*>(sm.A + r * sm.ld + c * 8) = o.u;
-      }
-    }
-    __syncthreads();
-  }
-}
-
-// async copy of `rows` weight rows (K columns from column k0) into W_s[buf]; `rowmap(i)` = global row of smem row i (< 0: zeros)
-template <class RowMap>
-__device__ __forceinline__ void load_W_async(const DraftSmem& sm, int buf, const __half* w, int64_t ldw, int k0, int K, int rows,
-                                             RowMap rowmap) {
-  const int cv = K / 8;
-  for (int i = threadIdx.x; i < rows * cv; i += DT) {
-    const int r = i / cv, c = i % cv;
-    const int gr = rowmap(r);
-    __half* dst = sm.W[buf] + r * sm.ld + c * 8;
-    if (gr >= 0) cp16(dst, w + (int64_t)gr * ldw + k0 + c * 8);
-    else *reinterpret_cast<uint4*>(dst) = make_uint4(0, 0, 0, 0);
-  }
-  cp_commit();
-}
-
-// C[16*MT x 16*NP] = A_s[.. x K] * W_s[buf][16*NP x K]^T with all 8 warps: units (m-tile, n16 pair, K part); epi(mt, np, acc)
-// gets acc[0] = n-tile 2np (W_s rows 16np..16np+7) and acc[1] = n-tile 2np+1 (rows 16np+8..+15) in the mma C layout
-// (c0,c1: row g, cols 2t,2t+1; c2,c3: row g+8).  The caller synchronises the block before W_s[buf] / red are reused.
-template <class Epi>
-__device__ __forceinline__ void gemm_subtile(const DraftSmem& sm, int buf, int K, int MT, int NP, Epi epi) {
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int units = MT * NP;
-  int KQ = 1;
-  if (units <= 2) KQ = 4; else if (units <= 4) KQ = 2;
-  while ((K / 16) % KQ) KQ >>= 1;
-  const int ksteps = K / 16 / KQ;
-  const uint32_t a_base = s_u32(sm.A), w_base = s_u32(sm.W[buf]);
-  const int ldb = sm.ld * 2;
-  for (int u0 = 0; u0 < units * KQ; u0 += 8) {
-    const int u = u0 + warp;
-    const bool act = u < units * KQ;
-    const int pair = act ? u / KQ : 0, kq = act ? u % KQ : 0;
-    const int mt = pair / NP, np = pair % NP;
-    float acc[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
-    if (act) {
-      const uint32_t a_addr = a_base + (mt * 16 + (lane & 15)) * ldb + (lane >> 4) * 16;
-      const uint32_t b_addr = w_base + (np * 16 + (lane & 7) + (lane >> 4) * 8) * ldb + ((lane >> 3) & 1) * 16;
-#pragma unroll 4
-      for (int s = 0; s < ksteps; ++s) {
-        const int kk = (kq * ksteps + s) * 32;       // byte offset of the k-step
-        uint32_t a[4], b[4];
-        ldsm4(a, a_addr + kk);
-        ldsm4(b, b_addr + kk);
-        mma16816(acc[0], a, b[0], b[1]);
-        mma16816(acc[1], a, b[2], b[3]);
-      }
-    }
-    if (KQ > 1) {
-      // fixed-order reduction of the K parts through shared memory (deterministic)
-      float* slot = sm.red + ((size_t)(warp) * 32 + lane) * 8;
-      if (act && kq > 0) {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) { slot[i] = acc[0][i]; slot[4 + i] = acc[1][i]; }
-      }
-      __syncthreads();
-      if (act && kq == 0) {
-        for (int q = 1; q < KQ; ++q) {
-          const float* o = sm.red + ((size_t)(warp + q) * 32 + lane) * 8;
-#pragma unroll
-          for (int i = 0; i < 4; ++i) { acc[0][i] += o[i]; acc[1][i] += o[4 + i]; }
-        }
-        epi(mt, np, acc);
-      }
-      __syncthreads();
-    } else if (act) {
-      epi(mt, np, acc);
-    }
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------------------------
-// Two ways to run the phases: coop = 1, ONE cooperative launch walks phases [phase_lo, phase_hi) with a grid barrier after
-// each; coop = 0, one launch per phase (phase_hi = phase_lo + 1), chained with programmatic dependent launch: weight
-// sub-tiles are requested before `griddepcontrol.wait`, activations after.  Phase ids: 0 = P0, 1 + 6l + {0..5} = A, B, C, D,
-// E, E2 of layer l, 1 + 6L = F.
-__global__ void __launch_bounds__(DT, 1) draft_forward_kernel(const DraftArgs a, int phase_lo, int phase_hi, int coop) {
+// Item = (head, 16-row tile); CTAs stride over the items.  Row r is tree-relative slot base + n0 + r (base = P - 1); keys
+// [0, base + kv_end) are visible under the structured tree mask.
+__global__ void __launch_bounds__(DT, 1) draft_attention_kernel(const DraftAttnArgs a) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
-  const bool chain = !coop;
-  if (chain) pdl_trigger();
-  auto run = [&](int ph) { return ph >= phase_lo && ph < phase_hi; };
-  auto phase_end = [&](int ph) { if (coop && run(ph) && ph + 1 < phase_hi) cg::this_grid().sync(); };
+  pdl_trigger();
+  pdl_wait();
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int g = lane >> 2, t4 = lane & 3;
   const int h = a.h, n = a.n;
-  const int n_pad = (n + 15) & ~15, MT = n_pad / 16;
-  DraftSmem sm;
-  sm.ld = h + DPAD;
-  sm.A = reinterpret_cast<__half*>(smem_raw);
-  sm.W[0] = sm.A + D_ROWS * sm.ld;
-  sm.W[1] = sm.W[0] + 32 * sm.ld;
-  sm.red = reinterpret_cast<float*>(sm.W[1] + 32 * sm.ld);       // 8 warps x 32 lanes x 8 floats = 8 KB
-  // (the prefix length only changes in the verify step, never between the launches of one draft phase)
+  const int MT = (n + 15) / 16;
   const int P = a.state[ST_P];
   const int base = P - 1;
   const int kv_len = base + a.kv_end;
   const int nblk = gridDim.x, bid = blockIdx.x;
-
-  // ---- P0: hidden <- embedding rows -------------------------------------------------------------------------------------
-  if (run(0)) {
-    if (chain) pdl_wait();
-    for (int r = bid; r < n; r += nblk) {
-      const int64_t tok = a.tokens[base + a.n0 + r];
-      const uint4* src = reinterpret_cast<const uint4*>(a.embed + tok * (int64_t)h);
-      uint4* dst = reinterpret_cast<uint4*>(a.hidden + (int64_t)r * h);
-      for (int i = tid; i < h / 8; i += DT) dst[i] = src[i];
-    }
-  }
-  phase_end(0);
-
-  for (int l = 0; l < a.L; ++l) {
-    const __half* wqkv = a.w[l][0];
-    const __half* wo = a.w[l][1];
-    const __half* wgu = a.w[l][2];
-    const __half* wd = a.w[l][3];
-    __half* kc = a.k_cache + (int64_t)l * a.H * a.M * HD;
-    __half* vc = a.v_cache + (int64_t)l * a.H * a.M * HD;
-
-    // ---- A: RMSNorm + q/k/v GEMM + RoPE + KV append.  Item = 16 dims of the first half of a head + their 16 partners in
-    // the second half (rotate_half pairs dim d with d + 32): W_s rows [lo 0-7 | hi 0-7 | lo 8-15 | hi 8-15].
-    if (run(1 + 6 * l + 0)) {
-      const int items = 3 * a.H * 2;
-      for (int it = bid; it < items; it += nblk) {
-        const int hd3 = it >> 1, q = it & 1;              // hd3: 0..H-1 q heads, H..2H-1 k heads, 2H..3H-1 v heads
-        const int row0 = hd3 * HD + q * 16;
-        load_W_async(sm, 0, wqkv, h, 0, h, 32, [&](int i) { return row0 + (i & 7) + ((i >> 4) << 3) + ((i >> 3) & 1) * 32; });
-        if (it == bid) load_A(sm, a.hidden, h, 0, h, n, n_pad, a.w[l][4], a.eps, chain);      // (waits for the weights too)
-        cp_wait<0>();
-        __syncthreads();
-        const int kind = hd3 / a.H, head = hd3 % a.H;     // 0 q, 1 k, 2 v
-        gemm_subtile(sm, 0, h, MT, 2, [&](int mt, int np, float (&acc)[2][4]) {
-#pragma unroll
-          for (int half = 0; half < 2; ++half) {
-            const int r = mt * 16 + g + half * 8;
-            if (r >= n) continue;
-            const int d = q * 16 + np * 8 + t4 * 2;        // dims d, d+1 (first half) and d+32, d+33
-            const float x1[2] = {h2f(f2h(acc[0][half * 2])), h2f(f2h(acc[0][half * 2 + 1]))};
-            const float x2[2] = {h2f(f2h(acc[1][half * 2])), h2f(f2h(acc[1][half * 2 + 1]))};
-            float o1[2], o2[2];
-            if (kind < 2) {
-              const int64_t pos = a.position_ids[base + a.n0 + r];
-              const __half2 c1 = *reinterpret_cast<const __half2*>(a.cosc + pos * HD + d);
-              const __half2 c2 = *reinterpret_cast<const __half2*>(a.cosc + pos * HD + d + 32);
-              const __half2 s1 = *reinterpret_cast<const __half2*>(a.sinc + pos * HD + d);
-              const __half2 s2 = *reinterpret_cast<const __half2*>(a.sinc + pos * HD + d + 32);
-              const float cf1[2] = {__low2float(c1), __high2float(c1)}, cf2[2] = {__low2float(c2), __high2float(c2)};
-              const float sf1[2] = {__low2float(s1), __high2float(s1)}, sf2[2] = {__low2float(s2), __high2float(s2)};
-#pragma unroll
-              for (int e = 0; e < 2; ++e) {                // q*cos + rotate_half(q)*sin, every op rounded to fp16
-                o1[e] = h2f(f2h(rnd16(x1[e] * cf1[e]) + rnd16(-x2[e] * sf1[e])));
-                o2[e] = h2f(f2h(rnd16(x2[e] * cf2[e]) + rnd16(x1[e] * sf2[e])));
-              }
-            } else {
-              o1[0] = x1[0]; o1[1] = x1[1]; o2[0] = x2[0]; o2[1] = x2[1];
-            }
-            __half* dst;
-            if (kind == 0) dst = a.qkv + (int64_t)r * (3 * h) + head * HD;
-            else {
-              const int64_t slot = a.storage_ids[base + a.n0 + r];
-              dst = (kind == 1 ? kc : vc) + ((int64_t)head * a.M + slot) * HD;
-            }
-            *reinterpret_cast<uint32_t*>(dst + d) = pack_h2(o1[0], o1[1]);
-            *reinterpret_cast<uint32_t*>(dst + d + 32) = pack_h2(o2[0], o2[1]);
-          }
-        });
-        __syncthreads();
+  const int items = a.H * MT;
+  const int ldk = HD + DPAD;                                       // 72 halfs
+  __half* Ks = reinterpret_cast<__half*>(smem_raw);
+  const int kv_pad = (kv_len + 31) & ~31;
+  __half* Vs = Ks + (size_t)kv_pad * ldk;
+  __half* Qs = Vs + (size_t)kv_pad * ldk;
+  float* sO = reinterpret_cast<float*>(Qs + 16 * ldk);             // [8][16][64]
+  float* sM = sO + 8 * 16 * 64;                                    // [8][16]
+  float* sL = sM + 8 * 16;
+  for (int it = bid; it < items; it += nblk) {
+    const int head = it / MT, mt = it % MT;
+    const __half* kg = a.k_cache + (int64_t)head * a.M * HD;
+    const __half* vg = a.v_cache + (int64_t)head * a.M * HD;
+    for (int i = tid; i < kv_pad * 8; i += DT) {
+      const int r = i >> 3, c = i & 7;
+      if (r < kv_len) {
+        cp16(Ks + r * ldk + c * 8, kg + (int64_t)r * HD + c * 8);
+        cp16(Vs + r * ldk + c * 8, vg + (int64_t)r * HD + c * 8);
+      } else {
+        *reinterpret_cast<uint4*>(Ks + r * ldk + c * 8) = make_uint4(0, 0, 0, 0);
+        *reinterpret_cast<uint4*>(Vs + r * ldk + c * 8) = make_uint4(0, 0, 0, 0);
       }
     }
-    phase_end(1 + 6 * l + 0);
-
-    // ---- B: attention.  Item = (head, 16-row tile); the 8 warps take 32-key blocks round-robin (online softmax per warp),
-    // partial (max, sum, O) combined through shared memory.
-    if (run(1 + 6 * l + 1)) {
-      const int items = a.H * MT;
-      const int ldk = HD + DPAD;                                       // 72 halfs
-      __half* Ks = reinterpret_cast<__half*>(smem_raw);
-      const int kv_pad = (kv_len + 31) & ~31;
-      __half* Vs = Ks + (size_t)kv_pad * ldk;
-      __half* Qs = Vs + (size_t)kv_pad * ldk;
-      float* sO = reinterpret_cast<float*>(Qs + 16 * ldk);             // [8][16][64]
-      float* sM = sO + 8 * 16 * 64;                                    // [8][16]
-      float* sL = sM + 8 * 16;
-      if (chain) pdl_wait();
-      for (int it = bid; it < items; it += nblk) {
-        const int head = it / MT, mt = it % MT;
-        const __half* kg = kc + (int64_t)head * a.M * HD;
-        const __half* vg = vc + (int64_t)head * a.M * HD;
-        for (int i = tid; i < kv_pad * 8; i += DT) {
-          const int r = i >> 3, c = i & 7;
-          if (r < kv_len) {
-            cp16(Ks + r * ldk + c * 8, kg + (int64_t)r * HD + c * 8);
-            cp16(Vs + r * ldk + c * 8, vg + (int64_t)r * HD + c * 8);
-          } else {
-            *reinterpret_cast<uint4*>(Ks + r * ldk + c * 8) = make_uint4(0, 0, 0, 0);
-            *reinterpret_cast<uint4*>(Vs + r * ldk + c * 8) = make_uint4(0, 0, 0, 0);
-          }
+    if (tid < 128) {
+      const int r = tid >> 3, c = tid & 7;
+      const int row = mt * 16 + r;
+      uint4 v = make_uint4(0, 0, 0, 0);
+      if (row < n) v = *reinterpret_cast<const uint4*>(a.qkv + (int64_t)row * (3 * h) + head * HD + c * 8);
+      *reinterpret_cast<uint4*>(Qs + r * ldk + c * 8) = v;
+    }
+    cp_commit();
+    cp_wait<0>();
+    __syncthreads();
+    // this thread's two rows
+    const int row_lo = mt * 16 + g, row_hi = row_lo + 8;
+    const RowMask rm_lo = row_mask(base + a.n0 + row_lo, P), rm_hi = row_mask(base + a.n0 + row_hi, P);
+    const uint32_t* bits_lo = (rm_lo.node >= 1 && rm_lo.node < a.tree_size) ? a.tree_bits + (int64_t)rm_lo.node * a.tree_words : nullptr;
+    const uint32_t* bits_hi = (rm_hi.node >= 1 && rm_hi.node < a.tree_size) ? a.tree_bits + (int64_t)rm_hi.node * a.tree_words : nullptr;
+    RowMask rl = rm_lo, rh = rm_hi;
+    if (bits_lo == nullptr) rl.node = -1;
+    if (bits_hi == nullptr) rh.node = -1;
+    uint32_t qa[4][4];
+    {
+      const uint32_t q_addr = s_u32(Qs) + ((lane & 15) * ldk) * 2 + (lane >> 4) * 16;
+#pragma unroll
+      for (int s = 0; s < 4; ++s) ldsm4(qa[s], q_addr + s * 32);
+    }
+    float m[2] = {-INFINITY, -INFINITY}, lsum[2] = {0.f, 0.f};
+    float o[8][4];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) { o[j][0] = o[j][1] = o[j][2] = o[j][3] = 0.f; }
+    const float sc = a.scale * 1.4426950408889634f;
+    for (int kb = warp; kb * 32 < kv_len; kb += 8) {
+      const int c0 = kb * 32;
+      float s[4][4];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) { s[j][0] = s[j][1] = s[j][2] = s[j][3] = 0.f; }
+      const uint32_t k_addr = s_u32(Ks) + ((c0 + (lane & 7) + (lane >> 4) * 8) * ldk) * 2 + ((lane >> 3) & 1) * 16;
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks) {
+#pragma unroll
+        for (int jp = 0; jp < 2; ++jp) {
+          uint32_t b[4];
+          ldsm4(b, k_addr + (jp * 16 * ldk) * 2 + ks * 32);
+          mma16816(s[jp * 2], qa[ks], b[0], b[1]);
+          mma16816(s[jp * 2 + 1], qa[ks], b[2], b[3]);
         }
-        if (tid < 128) {
-          const int r = tid >> 3, c = tid & 7;
-          const int row = mt * 16 + r;
-          uint4 v = make_uint4(0, 0, 0, 0);
-          if (row < n) v = *reinterpret_cast<const uint4*>(a.qkv + (int64_t)row * (3 * h) + head * HD + c * 8);
-          *reinterpret_cast<uint4*>(Qs + r * ldk + c * 8) = v;
-        }
-        cp_commit();
-        cp_wait<0>();
-        __syncthreads();
-        // this thread's two rows
-        const int row_lo = mt * 16 + g, row_hi = row_lo + 8;
-        const RowMask rm_lo = row_mask(base + a.n0 + row_lo, P), rm_hi = row_mask(base + a.n0 + row_hi, P);
-        const uint32_t* bits_lo = (rm_lo.node >= 1 && rm_lo.node < a.tree_size) ? a.tree_bits + (int64_t)rm_lo.node * a.tree_words : nullptr;
-        const uint32_t* bits_hi = (rm_hi.node >= 1 && rm_hi.node < a.tree_size) ? a.tree_bits + (int64_t)rm_hi.node * a.tree_words : nullptr;
-        RowMask rl = rm_lo, rh = rm_hi;
-        if (bits_lo == nullptr) rl.node = -1;
-        if (bits_hi == nullptr) rh.node = -1;
-        uint32_t qa[4][4];
-        {
-          const uint32_t q_addr = s_u32(Qs) + ((lane & 15) * ldk) * 2 + (lane >> 4) * 16;
+      }
+      const uint32_t vl = vis_word(rl, c0, P, kv_len, bits_lo, a.tree_words);
+      const uint32_t vh = vis_word(rh, c0, P, kv_len, bits_hi, a.tree_words);
+      float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
-          for (int s = 0; s < 4; ++s) ldsm4(qa[s], q_addr + s * 32);
-        }
-        float m[2] = {-INFINITY, -INFINITY}, lsum[2] = {0.f, 0.f};
-        float o[8][4];
+      for (int j = 0; j < 4; ++j)
 #pragma unroll
-        for (int j = 0; j < 8; ++j) { o[j][0] = o[j][1] = o[j][2] = o[j][3] = 0.f; }
-        const float sc = a.scale * 1.4426950408889634f;
-        for (int kb = warp; kb * 32 < kv_len; kb += 8) {
-          const int c0 = kb * 32;
-          float s[4][4];
-#pragma unroll
-          for (int j = 0; j < 4; ++j) { s[j][0] = s[j][1] = s[j][2] = s[j][3] = 0.f; }
-          const uint32_t k_addr = s_u32(Ks) + ((c0 + (lane & 7) + (lane >> 4) * 8) * ldk) * 2 + ((lane >> 3) & 1) * 16;
-#pragma unroll
-          for (int ks = 0; ks < 4; ++ks) {
-#pragma unroll
-            for (int jp = 0; jp < 2; ++jp) {
-              uint32_t b[4];
-              ldsm4(b, k_addr + (jp * 16 * ldk) * 2 + ks * 32);
-              mma16816(s[jp * 2], qa[ks], b[0], b[1]);
-              mma16816(s[jp * 2 + 1], qa[ks], b[2], b[3]);
-            }
-          }
-          const uint32_t vl = vis_word(rl, c0, P, kv_len, bits_lo, a.tree_words);
-          const uint32_t vh = vis_word(rh, c0, P, kv_len, bits_hi, a.tree_words);
-          float mx[2] = {-INFINITY, -INFINITY};
-#pragma unroll
-          for (int j = 0; j < 4; ++j)
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-              const int c = j * 8 + t4 * 2 + e;
-              s[j][e] = ((vl >> c) & 1u) ? s[j][e] * sc : -INFINITY;
-              s[j][2 + e] = ((vh >> c) & 1u) ? s[j][2 + e] * sc : -INFINITY;
-              mx[0] = fmaxf(mx[0], s[j][e]);
-              mx[1] = fmaxf(mx[1], s[j][2 + e]);
-            }
-#pragma unroll
-          for (int r2 = 0; r2 < 2; ++r2) {
-            mx[r2] = fmaxf(mx[r2], __shfl_xor_sync(0xffffffffu, mx[r2], 1));
-            mx[r2] = fmaxf(mx[r2], __shfl_xor_sync(0xffffffffu, mx[r2], 2));
-          }
-          float alpha[2], mref[2];
-#pragma unroll
-          for (int r2 = 0; r2 < 2; ++r2) {
-            const float mn = fmaxf(m[r2], mx[r2]);
-            alpha[r2] = (m[r2] == -INFINITY) ? 0.f : exp2f(m[r2] - mn);
-            m[r2] = mn;
-            mref[r2] = (mn == -INFINITY) ? 0.f : mn;
-            lsum[r2] *= alpha[r2];
-          }
-#pragma unroll
-          for (int j = 0; j < 8; ++j) { o[j][0] *= alpha[0]; o[j][1] *= alpha[0]; o[j][2] *= alpha[1]; o[j][3] *= alpha[1]; }
-          uint32_t pa[2][4];                               // P as the A operand of two 16-key k-steps
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const float p0 = exp2f(s[j][0] - mref[0]), p1 = exp2f(s[j][1] - mref[0]);
-            const float p2 = exp2f(s[j][2] - mref[1]), p3 = exp2f(s[j][3] - mref[1]);
-            lsum[0] += p0 + p1;
-            lsum[1] += p2 + p3;
-            pa[j >> 1][(j & 1) * 2] = pack_h2(p0, p1);     // a0 / a2: row g
-            pa[j >> 1][(j & 1) * 2 + 1] = pack_h2(p2, p3); // a1 / a3: row g+8
-          }
-          // O += P V : V_s is [key][dim] -> transposed ldmatrix gives the (k = key, n = dim) B fragments
-#pragma unroll
-          for (int ks = 0; ks < 2; ++ks) {
-            const uint32_t v_addr = s_u32(Vs) + ((c0 + ks * 16 + (lane & 15)) * ldk) * 2 + (lane >> 4) * 16;
-#pragma unroll
-            for (int jp = 0; jp < 4; ++jp) {
-              uint32_t b[4];
-              ldsm4t(b, v_addr + jp * 32);
-              mma16816(o[jp * 2], pa[ks], b[0], b[1]);
-              mma16816(o[jp * 2 + 1], pa[ks], b[2], b[3]);
-            }
-          }
+        for (int e = 0; e < 2; ++e) {
+          const int c = j * 8 + t4 * 2 + e;
+          s[j][e] = ((vl >> c) & 1u) ? s[j][e] * sc : -INFINITY;
+          s[j][2 + e] = ((vh >> c) & 1u) ? s[j][2 + e] * sc : -INFINITY;
+          mx[0] = fmaxf(mx[0], s[j][e]);
+          mx[1] = fmaxf(mx[1], s[j][2 + e]);
         }
 #pragma unroll
-        for (int r2 = 0; r2 < 2; ++r2) {
-          lsum[r2] += __shfl_xor_sync(0xffffffffu, lsum[r2], 1);
-          lsum[r2] += __shfl_xor_sync(0xffffffffu, lsum[r2], 2);
-        }
-        if (t4 == 0) {
-          sM[warp * 16 + g] = m[0]; sM[warp * 16 + g + 8] = m[1];
-          sL[warp * 16 + g] = lsum[0]; sL[warp * 16 + g + 8] = lsum[1];
-        }
+      for (int r2 = 0; r2 < 2; ++r2) {
+        mx[r2] = fmaxf(mx[r2], __shfl_xor_sync(0xffffffffu, mx[r2], 1));
+        mx[r2] = fmaxf(mx[r2], __shfl_xor_sync(0xffffffffu, mx[r2], 2));
+      }
+      float alpha[2], mref[2];
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          float* d0 = sO + ((warp * 16 + g) * 64) + j * 8 + t4 * 2;
-          d0[0] = o[j][0]; d0[1] = o[j][1];
-          d0[8 * 64] = o[j][2]; d0[8 * 64 + 1] = o[j][3];
-        }
-        __syncthreads();
-        {
-          const int r = tid >> 4, d0 = (tid & 15) * 4;
-          float mm = -INFINITY;
+      for (int r2 = 0; r2 < 2; ++r2) {
+        const float mn = fmaxf(m[r2], mx[r2]);
+        alpha[r2] = (m[r2] == -INFINITY) ? 0.f : exp2f(m[r2] - mn);
+        m[r2] = mn;
+        mref[r2] = (mn == -INFINITY) ? 0.f : mn;
+        lsum[r2] *= alpha[r2];
+      }
 #pragma unroll
-          for (int w = 0; w < 8; ++w) mm = fmaxf(mm, sM[w * 16 + r]);
-          float den = 0.f, acc[4] = {0.f, 0.f, 0.f, 0.f};
+      for (int j = 0; j < 8; ++j) { o[j][0] *= alpha[0]; o[j][1] *= alpha[0]; o[j][2] *= alpha[1]; o[j][3] *= alpha[1]; }
+      uint32_t pa[2][4];                               // P as the A operand of two 16-key k-steps
 #pragma unroll
-          for (int w = 0; w < 8; ++w) {
-            const float mw = sM[w * 16 + r];
-            if (mw == -INFINITY) continue;
-            const float f = exp2f(mw - mm);
-            den += f * sL[w * 16 + r];
-            const float4 ov = *reinterpret_cast<const float4*>(sO + (w * 16 + r) * 64 + d0);
-            acc[0] += f * ov.x; acc[1] += f * ov.y; acc[2] += f * ov.z; acc[3] += f * ov.w;
-          }
-          const float inv = den > 0.f ? 1.f / den : 0.f;
-          const int row = mt * 16 + r;
-          if (row < n) {
-            uint2 pk;
-            pk.x = pack_h2(acc[0] * inv, acc[1] * inv);
-            pk.y = pack_h2(acc[2] * inv, acc[3] * inv);
-            *reinterpret_cast<uint2*>(a.attn + (int64_t)row * h + head * HD + d0) = pk;
-          }
+      for (int j = 0; j < 4; ++j) {
+        const float p0 = exp2f(s[j][0] - mref[0]), p1 = exp2f(s[j][1] - mref[0]);
+        const float p2 = exp2f(s[j][2] - mref[1]), p3 = exp2f(s[j][3] - mref[1]);
+        lsum[0] += p0 + p1;
+        lsum[1] += p2 + p3;
+        pa[j >> 1][(j & 1) * 2] = pack_h2(p0, p1);     // a0 / a2: row g
+        pa[j >> 1][(j & 1) * 2 + 1] = pack_h2(p2, p3); // a1 / a3: row g+8
+      }
+      // O += P V : V_s is [key][dim] -> transposed ldmatrix gives the (k = key, n = dim) B fragments
+#pragma unroll
+      for (int ks = 0; ks < 2; ++ks) {
+        const uint32_t v_addr = s_u32(Vs) + ((c0 + ks * 16 + (lane & 15)) * ldk) * 2 + (lane >> 4) * 16;
+#pragma unroll
+        for (int jp = 0; jp < 4; ++jp) {
+          uint32_t b[4];
+          ldsm4t(b, v_addr + jp * 32);
+          mma16816(o[jp * 2], pa[ks], b[0], b[1]);
+          mma16816(o[jp * 2 + 1], pa[ks], b[2], b[3]);
         }
-        __syncthreads();
       }
     }
-    phase_end(1 + 6 * l + 1);
-
-    // ---- C: o_proj + residual add.  Item = 32 output columns.
-    if (run(1 + 6 * l + 2)) {
-      const int items = h / 32;
-      for (int it = bid; it < items; it += nblk) {
-        const int c0 = it * 32;
-        load_W_async(sm, 0, wo, h, 0, h, 32, [&](int i) { return c0 + i; });
-        if (it == bid) load_A(sm, a.attn, h, 0, h, n, n_pad, nullptr, 0.f, chain);
-        cp_wait<0>();
-        __syncthreads();
-        gemm_subtile(sm, 0, h, MT, 2, [&](int mt, int np, float (&acc)[2][4]) {
 #pragma unroll
-          for (int half = 0; half < 2; ++half) {
-            const int r = mt * 16 + g + half * 8;
-            if (r >= n) continue;
+    for (int r2 = 0; r2 < 2; ++r2) {
+      lsum[r2] += __shfl_xor_sync(0xffffffffu, lsum[r2], 1);
+      lsum[r2] += __shfl_xor_sync(0xffffffffu, lsum[r2], 2);
+    }
+    if (t4 == 0) {
+      sM[warp * 16 + g] = m[0]; sM[warp * 16 + g + 8] = m[1];
+      sL[warp * 16 + g] = lsum[0]; sL[warp * 16 + g + 8] = lsum[1];
+    }
 #pragma unroll
-            for (int j = 0; j < 2; ++j) {
-              __half* p = a.hidden + (int64_t)r * h + c0 + np * 16 + j * 8 + t4 * 2;
-              const __half2 old = *reinterpret_cast<const __half2*>(p);
-              *reinterpret_cast<uint32_t*>(p) = pack_h2(__low2float(old) + h2f(f2h(acc[j][half * 2])),
-                                                        __high2float(old) + h2f(f2h(acc[j][half * 2 + 1])));
-            }
-          }
-        });
-        __syncthreads();
+    for (int j = 0; j < 8; ++j) {
+      float* d0 = sO + ((warp * 16 + g) * 64) + j * 8 + t4 * 2;
+      d0[0] = o[j][0]; d0[1] = o[j][1];
+      d0[8 * 64] = o[j][2]; d0[8 * 64 + 1] = o[j][3];
+    }
+    __syncthreads();
+    {
+      const int r = tid >> 4, d0 = (tid & 15) * 4;
+      float mm = -INFINITY;
+#pragma unroll
+      for (int w = 0; w < 8; ++w) mm = fmaxf(mm, sM[w * 16 + r]);
+      float den = 0.f, acc[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+      for (int w = 0; w < 8; ++w) {
+        const float mw = sM[w * 16 + r];
+        if (mw == -INFINITY) continue;
+        const float f = exp2f(mw - mm);
+        den += f * sL[w * 16 + r];
+        const float4 ov = *reinterpret_cast<const float4*>(sO + (w * 16 + r) * 64 + d0);
+        acc[0] += f * ov.x; acc[1] += f * ov.y; acc[2] += f * ov.z; acc[3] += f * ov.w;
+      }
+      const float inv = den > 0.f ? 1.f / den : 0.f;
+      const int row = mt * 16 + r;
+      if (row < n) {
+        uint2 pk;
+        pk.x = pack_h2(acc[0] * inv, acc[1] * inv);
+        pk.y = pack_h2(acc[2] * inv, acc[3] * inv);
+        *reinterpret_cast<uint2*>(a.attn + (int64_t)row * h + head * HD + d0) = pk;
       }
     }
-    phase_end(1 + 6 * l + 2);
-
-    // ---- D: RMSNorm + gate/up + SiLU*up.  Item = 32 act columns = two 32-row sub-tiles [gate 0-7 | up 0-7 | gate 8-15 | up 8-15].
-    if (run(1 + 6 * l + 3)) {
-      const int items = a.I / 32;
-      for (int it = bid; it < items; it += nblk) {
-        const int c0 = it * 32;
-        auto rowmap = [&](int sub) {
-          return [=](int i) { const int col = c0 + sub * 16 + (i & 7) + ((i >> 4) << 3); return ((i >> 3) & 1) ? a.I + col : col; };
-        };
-        load_W_async(sm, 0, wgu, h, 0, h, 32, rowmap(0));
-        load_W_async(sm, 1, wgu, h, 0, h, 32, rowmap(1));
-        if (it == bid) load_A(sm, a.hidden, h, 0, h, n, n_pad, a.w[l][5], a.eps, chain);
-        for (int sub = 0; sub < 2; ++sub) {
-          if (sub == 0) cp_wait<1>(); else cp_wait<0>();
-          __syncthreads();
-          gemm_subtile(sm, sub, h, MT, 2, [&](int mt, int np, float (&acc)[2][4]) {
-#pragma unroll
-            for (int half = 0; half < 2; ++half) {
-              const int r = mt * 16 + g + half * 8;
-              if (r >= n) continue;
-              float ov[2];
-#pragma unroll
-              for (int e = 0; e < 2; ++e) {
-                const float x = h2f(f2h(acc[0][half * 2 + e]));
-                const __half act = f2h(x / (1.0f + expf(-x)));
-                ov[e] = h2f(act) * h2f(f2h(acc[1][half * 2 + e]));
-              }
-              *reinterpret_cast<uint32_t*>(a.act + (int64_t)r * a.I + c0 + sub * 16 + np * 8 + t4 * 2) = pack_h2(ov[0], ov[1]);
-            }
-          });
-        }
-        __syncthreads();
-      }
-    }
-    phase_end(1 + 6 * l + 3);
-
-    // ---- E: down_proj, split along K in chunks of h columns.  Item = (32 output columns, K chunk) -> fp32 partials.
-    if (run(1 + 6 * l + 4)) {
-      const int ncol = h / 32;
-      const int items = ncol * a.ks;
-      for (int it = bid; it < items; it += nblk) {
-        const int kq = it / ncol, c0 = (it % ncol) * 32;
-        load_W_async(sm, 0, wd, a.I, kq * h, h, 32, [&](int i) { return c0 + i; });
-        load_A(sm, a.act, a.I, kq * h, h, n, n_pad, nullptr, 0.f, chain);
-        cp_wait<0>();
-        __syncthreads();
-        gemm_subtile(sm, 0, h, MT, 2, [&](int mt, int np, float (&acc)[2][4]) {
-#pragma unroll
-          for (int half = 0; half < 2; ++half) {
-            const int r = mt * 16 + g + half * 8;
-            if (r >= n) continue;
-#pragma unroll
-            for (int j = 0; j < 2; ++j)
-              *reinterpret_cast<float2*>(a.partial + ((int64_t)kq * D_ROWS + r) * h + c0 + np * 16 + j * 8 + t4 * 2) =
-                  make_float2(acc[j][half * 2], acc[j][half * 2 + 1]);
-          }
-        });
-        __syncthreads();
-      }
-    }
-    phase_end(1 + 6 * l + 4);
-
-    // ---- E2: hidden += fp16(sum of the K-chunk partials), in chunk order.
-    if (run(1 + 6 * l + 5)) {
-    if (chain) pdl_wait();
-    for (int r = bid; r < n; r += nblk) {
-      for (int c = tid * 2; c < h; c += DT * 2) {
-        float s0 = 0.f, s1 = 0.f;
-        for (int q = 0; q < a.ks; ++q) {
-          const float2 pv = *reinterpret_cast<const float2*>(a.partial + ((int64_t)q * D_ROWS + r) * h + c);
-          s0 += pv.x; s1 += pv.y;
-        }
-        __half* p = a.hidden + (int64_t)r * h + c;
-        const __half2 old = *reinterpret_cast<const __half2*>(p);
-        *reinterpret_cast<uint32_t*>(p) = pack_h2(__low2float(old) + h2f(f2h(s0)), __high2float(old) + h2f(f2h(s1)));
-      }
-    }
-    }
-    phase_end(1 + 6 * l + 5);
-  }
-
-  // ---- F: final RMSNorm + lm_head.  Item = `fcols` vocabulary columns, streamed in double-buffered 32-row sub-tiles.
-  if (run(1 + 6 * a.L)) {
-    const int per = ((a.V + nblk - 1) / nblk + 31) & ~31;            // columns per CTA, multiple of 32
-    const int c_begin = bid * per;
-    if (c_begin < a.V) {
-      const int nsub = (min(per, a.V - c_begin) + 31) / 32;
-      auto rowmap = [&](int sub) {
-        return [=](int i) { const int col = c_begin + sub * 32 + i; return col < a.V ? col : -1; };
-      };
-      load_W_async(sm, 0, a.lm_head, h, 0, h, 32, rowmap(0));
-      load_A(sm, a.hidden, h, 0, h, n, n_pad, a.fnorm, a.eps, chain);
-      for (int sub = 0; sub < nsub; ++sub) {
-        if (sub + 1 < nsub) { load_W_async(sm, (sub + 1) & 1, a.lm_head, h, 0, h, 32, rowmap(sub + 1)); cp_wait<1>(); }
-        else cp_wait<0>();
-        __syncthreads();
-        const int cs = c_begin + sub * 32;
-        gemm_subtile(sm, sub & 1, h, MT, 2, [&](int mt, int np, float (&acc)[2][4]) {
-#pragma unroll
-          for (int half = 0; half < 2; ++half) {
-            const int r = mt * 16 + g + half * 8;
-            if (r >= n) continue;
-#pragma unroll
-            for (int j = 0; j < 2; ++j) {
-              const int col = cs + np * 16 + j * 8 + t4 * 2;
-              if (col < a.V) *reinterpret_cast<uint32_t*>(a.logits + (int64_t)r * a.ld_logits + col) = pack_h2(acc[j][half * 2], acc[j][half * 2 + 1]);
-            }
-          }
-        });
-        __syncthreads();
-      }
-    }
+    __syncthreads();
   }
 }
 
@@ -614,78 +241,34 @@ __global__ void __launch_bounds__(DT, 1) draft_forward_kernel(const DraftArgs a,
 using namespace sq;
 
 struct sq_draft_plan {
-  DraftArgs base;
+  int h, L, H, M;
+  const __half *k_cache, *v_cache;     // (L, 1, H, M, 64)
   int n_sm, smem;
-  int coop;          // 1: one cooperative launch per forward (grid barriers); 0: one PDL-chained launch per phase
-  size_t ws_bytes;
 };
 
-static size_t draft_ws_layout(int h, int I, int ks, size_t* off_hidden, size_t* off_qkv, size_t* off_attn, size_t* off_act,
-                              size_t* off_partial) {
-  size_t o = 0;
-  auto take = [&](size_t bytes) { const size_t at = o; o += (bytes + 255) & ~(size_t)255; return at; };
-  *off_hidden = take((size_t)D_ROWS * h * 2);
-  *off_qkv = take((size_t)D_ROWS * 3 * h * 2);
-  *off_attn = take((size_t)D_ROWS * h * 2);
-  *off_act = take((size_t)D_ROWS * I * 2);
-  *off_partial = take((size_t)ks * D_ROWS * h * 4);
-  return o;
+/* 1 if the draft attention supports a model of these shapes (else the draft forward uses sq_tree_attn). */
+extern "C" int sq_draft_supported(int hidden, int n_heads, int n_kv_heads, int head_dim, int max_length) {
+  return head_dim == HD && n_heads == n_kv_heads && n_heads * HD == hidden && max_length >= 1 &&
+         draft_attn_smem(max_length) <= 220 * 1024;
 }
 
-extern "C" int64_t sq_draft_workspace_bytes(int hidden, int inter) {
-  if (hidden <= 0 || inter % hidden) return -1;
-  size_t a, b, c, d, e;
-  return (int64_t)draft_ws_layout(hidden, inter, inter / hidden, &a, &b, &c, &d, &e);
-}
-
-/* 1 if a model of these shapes can run on the fused draft kernel (else use the multi-kernel forward). */
-extern "C" int sq_draft_supported(int hidden, int inter, int n_layers, int n_heads, int n_kv_heads, int head_dim, int vocab,
-                                  int max_length) {
-  const size_t smem_gemm = (size_t)(D_ROWS + 64) * (hidden + DPAD) * 2 + 8 * 32 * 8 * 4;
-  const size_t smem_attn = (size_t)(2 * ((max_length + 31) & ~31) + 16) * (HD + DPAD) * 2 + (8 * 16 * 64 + 2 * 8 * 16) * 4;
-  return head_dim == HD && n_heads == n_kv_heads && n_heads * HD == hidden && hidden % 32 == 0 && inter % hidden == 0 &&
-         inter % 32 == 0 && n_layers >= 1 && n_layers <= D_MAXL && vocab % 8 == 0 && smem_gemm <= 220 * 1024 &&
-         smem_attn <= 220 * 1024;
-}
-
-extern "C" int sq_draft_plan_create(sq_draft_plan** plan, int hidden, int inter, int n_layers, int n_heads, int vocab,
-                                    int max_length, float eps, const sq_half* embed, const sq_half* const* layer_weights,
-                                    const sq_half* final_norm, const sq_half* lm_head, const sq_half* cos, const sq_half* sin,
-                                    sq_half* k_cache, sq_half* v_cache, void* workspace, int64_t workspace_bytes) {
-  SQ_CHECK_ARG(plan && embed && layer_weights && final_norm && lm_head && cos && sin && k_cache && v_cache && workspace,
-               "sq_draft_plan_create: null pointer");
-  SQ_CHECK_ARG(sq_draft_supported(hidden, inter, n_layers, n_heads, n_heads, HD, vocab, max_length),
-               "sq_draft_plan_create: unsupported model shape (hidden %d, inter %d, layers %d, heads %d, M %d)", hidden, inter,
-               n_layers, n_heads, max_length);
-  SQ_CHECK_ARG(workspace_bytes >= sq_draft_workspace_bytes(hidden, inter), "sq_draft_plan_create: workspace too small");
+extern "C" int sq_draft_plan_create(sq_draft_plan** plan, int hidden, int n_layers, int n_heads, int max_length,
+                                    sq_half* k_cache, sq_half* v_cache) {
+  SQ_CHECK_ARG(plan && k_cache && v_cache, "sq_draft_plan_create: null pointer");
+  SQ_CHECK_ARG(n_layers >= 1 && sq_draft_supported(hidden, n_heads, n_heads, HD, max_length),
+               "sq_draft_plan_create: unsupported model shape (hidden %d, layers %d, heads %d, M %d)", hidden, n_layers,
+               n_heads, max_length);
   sq_draft_plan* p = new sq_draft_plan();
-  DraftArgs& a = p->base;
-  a.h = hidden; a.I = inter; a.L = n_layers; a.H = n_heads; a.V = vocab; a.M = max_length; a.ks = inter / hidden;
-  a.eps = eps; a.scale = 1.0f / sqrtf((float)HD);
-  a.embed = (const __half*)embed; a.fnorm = (const __half*)final_norm; a.lm_head = (const __half*)lm_head;
-  a.cosc = (const __half*)cos; a.sinc = (const __half*)sin;
-  for (int l = 0; l < n_layers; ++l)
-    for (int k = 0; k < 6; ++k) a.w[l][k] = (const __half*)layer_weights[l * 6 + k];
-  a.k_cache = (__half*)k_cache; a.v_cache = (__half*)v_cache;
-  size_t oh, oq, oa, oc, op;
-  p->ws_bytes = draft_ws_layout(hidden, inter, a.ks, &oh, &oq, &oa, &oc, &op);
-  char* ws = (char*)workspace;
-  a.hidden = (__half*)(ws + oh); a.qkv = (__half*)(ws + oq); a.attn = (__half*)(ws + oa); a.act = (__half*)(ws + oc);
-  a.partial = (float*)(ws + op);
-  const size_t smem_gemm = (size_t)(D_ROWS + 64) * (hidden + DPAD) * 2 + 8 * 32 * 8 * 4;
-  const size_t smem_attn = (size_t)(2 * ((max_length + 31) & ~31) + 16) * (HD + DPAD) * 2 + (8 * 16 * 64 + 2 * 8 * 16) * 4;
-  p->smem = (int)(smem_gemm > smem_attn ? smem_gemm : smem_attn);
-  {
-    const char* e = getenv("SQ_DRAFT_FUSED");     // "coop": cooperative megakernel; anything else: chained phase kernels
-    p->coop = (e && e[0] == 'c' && e[1] == 'o') ? 1 : 0;
-  }
+  p->h = hidden; p->L = n_layers; p->H = n_heads; p->M = max_length;
+  p->k_cache = (const __half*)k_cache; p->v_cache = (const __half*)v_cache;
+  p->smem = (int)draft_attn_smem(max_length);
   int dev = 0;
   cudaGetDevice(&dev);
   if (cudaDeviceGetAttribute(&p->n_sm, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || p->n_sm <= 0) p->n_sm = 132;
-  cudaError_t e = cudaFuncSetAttribute(draft_forward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, p->smem);
+  cudaError_t e = cudaFuncSetAttribute(draft_attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, p->smem);
   if (e != cudaSuccess) { set_error("sq_draft_plan_create: smem attr: %s", cudaGetErrorString(e)); delete p; return SQ_ERR_CUDA; }
   int occ = 0;
-  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, draft_forward_kernel, DT, p->smem);
+  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, draft_attention_kernel, DT, p->smem);
   if (e != cudaSuccess || occ < 1) { set_error("sq_draft_plan_create: kernel does not fit an SM"); delete p; return SQ_ERR_CUDA; }
   *plan = p;
   return SQ_OK;
@@ -696,82 +279,27 @@ extern "C" int sq_draft_plan_destroy(sq_draft_plan* plan) {
   return SQ_OK;
 }
 
-/* Forward `n` (<= 64) rows of tree nodes [n0, n0+n) in tree-relative addressing (base = state[P]-1): tokens / positions /
- * cache slots at index base+n0+r, keys [0, base+kv_end) visible under the packed tree mask.  Writes K/V of the rows to the
- * cache and their logits to logits_out (row pitch ld_logits). */
-/* Only the attention phase of layer `layer` (one PDL-chained launch), on caller-owned buffers: q rows in `qkv` (n, 3*hidden;
- * q part read), output to `attn_out` (n, hidden).  K/V come from the plan's caches (the rows of this forward must already
- * be appended).  A small-shape alternative to sq_tree_attn for the draft model's <= 64-row forwards. */
+/* Attention of layer `layer` for `n` (<= 64) rows = tree nodes [n0, n0+n) in tree-relative addressing (base = state[P]-1),
+ * on caller-owned buffers: q rows in `qkv` (n, 3*hidden; q part read), output to `attn_out` (n, hidden).  K/V come from
+ * the plan's caches (the rows of this forward must already be appended); keys [0, base+kv_end) are visible under the
+ * packed tree mask.  A small-shape alternative to sq_tree_attn for the draft model's forwards. */
 extern "C" int sq_draft_attention(sq_draft_plan* plan, int layer, int n, const sq_half* qkv, sq_half* attn_out,
                                   const int32_t* state, int n0, int kv_end, const uint32_t* tree_bits, int tree_words,
                                   int tree_size, void* stream) {
   SQ_CHECK_ARG(plan != nullptr && state != nullptr && qkv && attn_out, "sq_draft_attention: null argument");
-  SQ_CHECK_ARG(n >= 1 && n <= D_ROWS && layer >= 0 && layer < plan->base.L, "sq_draft_attention: n=%d / layer=%d out of range", n, layer);
+  SQ_CHECK_ARG(n >= 1 && n <= D_ROWS && layer >= 0 && layer < plan->L, "sq_draft_attention: n=%d / layer=%d out of range", n, layer);
   SQ_CHECK_ARG(tree_words <= 32, "sq_draft_attention: tree_size > 1024 unsupported");
-  DraftArgs a = plan->base;
-  a.n = n; a.n0 = n0; a.kv_end = kv_end; a.state = state;
-  a.tokens = nullptr; a.position_ids = nullptr; a.storage_ids = nullptr;
-  a.qkv = (__half*)qkv; a.attn = (__half*)attn_out;
+  DraftAttnArgs a;
+  a.h = plan->h; a.H = plan->H; a.M = plan->M; a.n = n; a.n0 = n0; a.kv_end = kv_end;
+  a.scale = 1.0f / sqrtf((float)HD);
+  a.k_cache = plan->k_cache + (int64_t)layer * plan->H * plan->M * HD;
+  a.v_cache = plan->v_cache + (int64_t)layer * plan->H * plan->M * HD;
+  a.qkv = (const __half*)qkv; a.attn = (__half*)attn_out; a.state = state;
   a.tree_bits = tree_bits; a.tree_words = tree_bits ? tree_words : 0; a.tree_size = tree_bits ? tree_size : 0;
-  a.logits = nullptr; a.ld_logits = 0;
-  const int ph = 1 + 6 * layer + 1;
   int grid = a.H * ((n + 15) / 16);
   if (grid > plan->n_sm) grid = plan->n_sm;
-  cudaError_t e = launch_k(draft_forward_kernel, dim3(grid), dim3(DT), (size_t)plan->smem, (cudaStream_t)stream, a, ph, ph + 1, 0);
+  cudaError_t e = launch_k(draft_attention_kernel, dim3(grid), dim3(DT), (size_t)plan->smem, (cudaStream_t)stream, a);
   if (e != cudaSuccess) { set_error("sq_draft_attention: launch failed: %s", cudaGetErrorString(e)); return SQ_ERR_CUDA; }
   SQ_CHECK_LAUNCH("sq_draft_attention");
-  return SQ_OK;
-}
-
-extern "C" int sq_draft_forward(sq_draft_plan* plan, int n, const int64_t* tokens, const int64_t* position_ids,
-                                const int64_t* storage_ids, const int32_t* state, int n0, int kv_end,
-                                const uint32_t* tree_bits, int tree_words, int tree_size, sq_half* logits_out,
-                                int64_t ld_logits, void* stream) {
-  SQ_CHECK_ARG(plan != nullptr && state != nullptr, "sq_draft_forward: plan / state required (tree-relative addressing only)");
-  SQ_CHECK_ARG(n >= 1 && n <= D_ROWS, "sq_draft_forward: n=%d must be in [1, %d]", n, D_ROWS);
-  SQ_CHECK_ARG(ld_logits % 2 == 0 && ((uintptr_t)logits_out % 4) == 0, "sq_draft_forward: logits pitch / alignment");
-  SQ_CHECK_ARG(tree_words <= 32, "sq_draft_forward: tree_size > 1024 unsupported");
-  DraftArgs a = plan->base;
-  a.n = n; a.n0 = n0; a.kv_end = kv_end;
-  a.tokens = tokens; a.position_ids = position_ids; a.storage_ids = storage_ids; a.state = state;
-  a.tree_bits = tree_bits; a.tree_words = tree_bits ? tree_words : 0; a.tree_size = tree_bits ? tree_size : 0;
-  a.logits = (__half*)logits_out; a.ld_logits = ld_logits;
-  const int n_phases = 2 + 6 * a.L;
-  if (plan->coop) {
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(plan->n_sm);
-    cfg.blockDim = dim3(DT);
-    cfg.dynamicSmemBytes = plan->smem;
-    cfg.stream = (cudaStream_t)stream;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeCooperative;
-    at[0].val.cooperative = 1;
-    cfg.attrs = at;
-    cfg.numAttrs = 1;
-    cudaError_t e = cudaLaunchKernelEx(&cfg, draft_forward_kernel, a, 0, n_phases, 1);
-    if (e != cudaSuccess) { set_error("sq_draft_forward: launch failed: %s", cudaGetErrorString(e)); return SQ_ERR_CUDA; }
-  } else {
-    const int MT = (n + 15) / 16;
-    for (int ph = 0; ph < n_phases; ++ph) {
-      int grid;
-      if (ph == 0) grid = n;
-      else if (ph == n_phases - 1) grid = plan->n_sm;
-      else {
-        switch ((ph - 1) % 6) {
-          case 0: grid = 6 * a.H; break;
-          case 1: grid = a.H * MT; break;
-          case 2: grid = a.h / 32; break;
-          case 3: grid = a.I / 32; break;
-          case 4: grid = (a.h / 32) * a.ks; break;
-          default: grid = n; break;
-        }
-      }
-      if (grid > plan->n_sm) grid = plan->n_sm;
-      cudaError_t e = launch_k(draft_forward_kernel, dim3(grid), dim3(DT), (size_t)plan->smem, (cudaStream_t)stream, a, ph, ph + 1, 0);
-      if (e != cudaSuccess) { set_error("sq_draft_forward: launch failed: %s", cudaGetErrorString(e)); return SQ_ERR_CUDA; }
-      if (ph + 1 < n_phases) sq::count_launch(1);
-    }
-  }
-  SQ_CHECK_LAUNCH("sq_draft_forward");
   return SQ_OK;
 }

@@ -246,22 +246,13 @@ class LlamaRunner:
         self.k_cache = torch.zeros(self.L, batch_size, self.Hkv, max_length, D, dtype=F16, device=dev)
         self.v_cache = torch.zeros_like(self.k_cache)
         self.plan = ops.AttnPlan(self.qkv, n, self.H, self.Hkv, D, self.k_cache, self.v_cache, self.attn_out)
-        # Dense GEMMs.  Default ("auto"): the weight-streaming shapes given to the hand-written wgmma kernel (csrc/sq_gemm.cu) -- gate_up with the SwiGLU epilogue fused (weights interleaved + pre-tiled, `act` written directly: no
-        # gate_up round trip, no silu_mul launch) and the target's lm_head (pre-tiled) -- for models whose layers are
-        # HBM-stream-sized (hidden >= 2048); q/k/v, o_proj and down_proj stay on cuBLASLt (torch.mm).  SQ_GEMM=1 routes
-        # those through sq_gemm too
-        # (tuning), SQ_GEMM=0 keeps everything on cuBLASLt + sq_silu_mul.
-        mode = os.environ.get("SQ_GEMM", "auto")
-        self.gemm = None
+        # Dense GEMMs.  The weight-streaming shapes go to the hand-written wgmma kernel (csrc/sq_gemm.cu) -- gate_up with the
+        # SwiGLU epilogue fused (weights interleaved, `act` written directly: no gate_up round trip, no silu_mul launch)
+        # and the target's lm_head -- for models whose layers are HBM-stream-sized (hidden >= 2048); q/k/v, o_proj and
+        # down_proj stay on cuBLASLt (torch.mm), which is faster at those shapes.
         self.gemm_err = torch.zeros(4, dtype=torch.int32, device=dev)
         self.lm_plan = None
         stream_sized = h >= 2048
-        if mode == "1":
-            self.gemm = []
-            for ly in self.layers:
-                self.gemm.append(dict(qkv=self._plan(self.normed, ly["wqkv"], self.qkv),
-                                      o=self._plan(self.attn_out, ly["wo"], self.proj),
-                                      d=self._plan(self.act, ly["wd"], self.proj)))
         # (a fused-epilogue plan cannot split K, so a narrow shard -- TP-4/8 of a 7B -- would leave most SMs idle: those
         # stay on cuBLASLt + sq_silu_mul).  The plans serve forwards of <= 128 rows; larger ones (prefill, the 768-row verify
         # of config 4: compute-bound, not a weight stream) go to cuBLASLt on the SAME weight tensor, which is why gate_up is
@@ -269,68 +260,23 @@ class LlamaRunner:
         gu_bn, gu_split, _ = ops.gemm_pick_tiles(2 * self.I, h, ops.GEMM_SWIGLU) if self.I % 16 == 0 and h % 64 == 0 else (0, 1, 1)
         gu_ctas = (-(-2 * self.I // gu_bn)) * gu_split if gu_bn else 0
         self.gu_interleaved = False
-        if mode in ("1", "auto") and stream_sized and gu_ctas >= 120:
+        if stream_sized and gu_ctas >= 120:
             self.gu_interleaved = True
             for ly in self.layers:
                 ly["wgu"] = ops.interleave_gate_up(ly["wgu"][:self.I], ly["wgu"][self.I:])
                 ly["gu_plan"] = ops.GemmPlan(self.normed, ly["wgu"], self.act, self.gemm_err, swiglu=True)
-        if mode in ("1", "auto") and stream_sized and V % 32 == 0 and h % 64 == 0:
+        if stream_sized and V % 32 == 0 and h % 64 == 0:
             self.lm_plan = ops.GemmPlan(self.normed, self.lm_head, self.logits, self.gemm_err)
-        # Small draft models (csrc/sq_draft.cu).  SQ_DRAFT_FUSED = "chain" | "coop": the whole forward of a tree level as
-        # PDL-chained phase kernels / ONE persistent cooperative kernel (opt-in: the multi-kernel path is the default).  Default: only its attention
-        # phase replaces sq_tree_attn for the draft's tree-relative forwards of <= 64 rows (SQ_DRAFT_ATTN=0 turns that off).
+        # Small draft models (csrc/sq_draft.cu): a dedicated attention kernel replaces sq_tree_attn for the draft's
+        # tree-relative forwards of <= 64 rows (SQ_DRAFT_ATTN=0 turns it off).
         self.draft_plan = None
-        self.draft_fused = os.environ.get("SQ_DRAFT_FUSED", "0") not in ("0", "")
-        self.draft_attn = os.environ.get("SQ_DRAFT_ATTN", "1") != "0"
-        if ((self.draft_fused or self.draft_attn) and tp == 1 and batch_size == 1 and not self.gu_interleaved and
-                ops.draft_supported(h, self.I, self.L, self.H, self.Hkv, D, V, max_length)):
-            self.draft_plan = ops.DraftPlan(h, self.I, self.H, V, max_length, self.eps, self.embed, self.layers, self.norm,
-                                            self.lm_head, self.cos, self.sin, self.k_cache, self.v_cache)
+        if (os.environ.get("SQ_DRAFT_ATTN", "1") != "0" and tp == 1 and batch_size == 1 and
+                ops.draft_supported(h, self.H, self.Hkv, D, max_length)):
+            self.draft_plan = ops.DraftPlan(h, self.L, self.H, max_length, self.k_cache, self.v_cache)
         self.peer = None
         if self.tp.size > 1 and os.environ.get("SQ_TP_MODE", "fused") == "fused":
             from .peer import PeerBuffers
             self.peer = PeerBuffers(tp_group, self.device, n, h)
-        self.attn_impl = int(os.environ.get("SQ_ATTN_IMPL", "0"))
-        # L2 prefetch of the next GEMM's weights while the latency-bound kernels between two GEMMs leave HBM idle
-        # (csrc/sq_prefetch.cu).  SQ_L2_PREFETCH = "A,B,C,D" MB budgets for the four windows of a layer (after qkv /
-        # o_proj / gate_up / down_proj), "0" = off; "1" = a preset that stays below the H100's 50 MB L2 (not tuned).  A hint
-        # only: results are identical with or without it.
-        pf = os.environ.get("SQ_L2_PREFETCH", "0")
-        self.pf_budget = None
-        if pf not in ("0", "") and self.peer is None and h >= 2048:      # pointless for the small draft models
-            vals = [24, 12, 14, 14] if pf == "1" else [float(x) for x in pf.split(",")]
-            assert len(vals) == 4, "SQ_L2_PREFETCH: 1 | 0 | A,B,C,D (MB)"
-            self.pf_budget = [int(v * 1e6) for v in vals]
-            self.pf_stream = torch.cuda.Stream(device=self.device)
-
-    def _prefetch(self, window: int, weights):
-        """Fork: on the side stream, pull the leading columns of `weights` (in order, until the window's byte budget is
-        spent) into L2.  Joined by `_prefetch_join` before the next GEMM."""
-        if self.pf_budget is None:
-            return
-        left = self.pf_budget[window]
-        cur = torch.cuda.current_stream()
-        self.pf_stream.wait_stream(cur)
-        with torch.cuda.stream(self.pf_stream):
-            for w, col0 in weights:
-                row_bytes = w.shape[0] * w.element_size()
-                cols = min((left // row_bytes) // 64 * 64, w.shape[1] - col0)
-                if cols <= 0:
-                    continue
-                ops.l2_prefetch(w, col0, col0 + cols)
-                left -= cols * row_bytes
-        self._pf_fork = True
-
-    def _prefetch_join(self):
-        if self.pf_budget is not None and getattr(self, "_pf_fork", False):
-            torch.cuda.current_stream().wait_stream(self.pf_stream)
-            self._pf_fork = False
-
-    def _plan(self, a, w, c):
-        try:
-            return ops.GemmPlan(a, w, c, self.gemm_err)
-        except Exception:
-            return None                                   # shape outside the kernel's tiling (K % 64, N % 32): cuBLASLt
 
     def _gate_up_act(self, ly, n: int):
         """act[:n] = silu(normed[:n] @ Wg.T) * (normed[:n] @ Wu.T)   (Engine/Llama_modules.py:272)"""
@@ -342,15 +288,6 @@ class LlamaRunner:
             return
         torch.mm(self.normed[:n], ly["wgu"].t(), out=self.gate_up[:n])
         ops.silu_mul(self.gate_up, self.act, n, interleaved=self.gu_interleaved)
-
-    def _linear(self, l: int, key: str, x: torch.Tensor, w: torch.Tensor, out: torch.Tensor, n: int):
-        """out[:n] = x[:n] @ w.T"""
-        if self.gemm is not None and n <= 128 and self.peer is None:
-            plan = self.gemm[l][key]
-            if plan is not None:
-                plan.run(n)
-                return
-        torch.mm(x[:n], w.t(), out=out[:n])
 
     def weight_bytes(self) -> int:
         b = self.embed.numel() + self.lm_head.numel() + self.norm.numel()
@@ -377,12 +314,7 @@ class LlamaRunner:
         assert not batch or (state is not None and dense_mask is None)
         H, Hkv, D, M = self.H, self.Hkv, self.D, self.M
         small = (not batch and self.draft_plan is not None and state is not None and n <= ops.DraftPlan.MAX_ROWS
-                 and dense_mask is None and self.attn_impl == 0)
-        if small and self.draft_fused and logits_from == 0 and not skip_lm_head:
-            out = logits_out if logits_out is not None else self.logits[:n]
-            self.draft_plan.forward(n, tokens, position_ids, storage_ids, state, n0, kv_end, tree_bits, tree_words,
-                                    tree_size, out)
-            return out
+                 and dense_mask is None)
         if batch:
             ops.embed_rows_batch(self.embed, tokens, n, self.hidden, state, n0=n0)
         else:
@@ -390,25 +322,22 @@ class LlamaRunner:
         n_seq, n = n, N                                # from here on n counts the rows of all sequences
         ops.rmsnorm(self.hidden, self.layers[0]["ln1"], self.normed, n, self.eps)
         for l, ly in enumerate(self.layers):
-            self._prefetch_join()
-            self._linear(l, "qkv", self.normed, ly["wqkv"], self.qkv, n)
-            if self.pf_budget is not None:          # window A: RoPE + attention
-                self._prefetch(0, [(ly["wo"], 0), (ly["wgu"], 0)])
+            torch.mm(self.normed[:n], ly["wqkv"].t(), out=self.qkv[:n])
             if batch:
                 ops.rope_kv_append_batch(self.qkv, H, Hkv, D, self.cos, self.sin, position_ids, storage_ids, n_seq,
                                          self.k_cache[l], self.v_cache[l], M, state, n0=n0)
                 ops.tree_attn_batch(self.plan, l, n_seq, state=state, n0=n0, kv_end=kv_end, tree_bits=tree_bits,
                                     tree_words=tree_words, tree_size=tree_size)
-            elif small and self.draft_attn:
-                ops.rope_kv_append(self.qkv, H, Hkv, D, self.cos, self.sin, position_ids, storage_ids, n,
-                                   self.k_cache[l], self.v_cache[l], M, state=state, n0=n0)
-                self.draft_plan.attention(l, n, self.qkv, self.attn_out, state, n0, kv_end, tree_bits, tree_words, tree_size)
             else:
                 ops.rope_kv_append(self.qkv, H, Hkv, D, self.cos, self.sin, position_ids, storage_ids, n,
                                    self.k_cache[l], self.v_cache[l], M, state=state, n0=n0)
-                ops.tree_attn(self.plan, l, n, state=state, n0=n0, kv_end=kv_end, prefix_len=prefix_len,
-                              dense_mask=dense_mask, mask_ld=mask_ld, tree_bits=tree_bits, tree_words=tree_words,
-                              tree_size=tree_size, impl=self.attn_impl)
+                if small:
+                    self.draft_plan.attention(l, n, self.qkv, self.attn_out, state, n0, kv_end, tree_bits, tree_words,
+                                              tree_size)
+                else:
+                    ops.tree_attn(self.plan, l, n, state=state, n0=n0, kv_end=kv_end, prefix_len=prefix_len,
+                                  dense_mask=dense_mask, mask_ld=mask_ld, tree_bits=tree_bits, tree_words=tree_words,
+                                  tree_size=tree_size)
             nxt = self.layers[l + 1]["ln1"] if l + 1 < self.L else self.norm
             if self.peer is not None:
                 torch.mm(self.attn_out[:n], ly["wo"].t(), out=self.peer.buf[0][:n])
@@ -417,29 +346,15 @@ class LlamaRunner:
                 torch.mm(self.act[:n], ly["wd"].t(), out=self.peer.buf[1][:n])
                 self.peer.allreduce_add_rmsnorm(1, self.hidden, nxt, self.normed, n, self.eps)
                 continue
-            self._prefetch_join()
-            self._linear(l, "o", self.attn_out, ly["wo"], self.proj, n)
-            if self.pf_budget is not None:          # window B: residual + RMSNorm; continue gate_up where window A stopped
-                wo_b = ly["wo"].numel() * 2
-                done = 0 if self.pf_budget[0] <= wo_b else \
-                    min(((self.pf_budget[0] - wo_b) // (ly["wgu"].shape[0] * 2)) // 64 * 64, ly["wgu"].shape[1])
-                self._prefetch(1, [(ly["wgu"], done)])
+            torch.mm(self.attn_out[:n], ly["wo"].t(), out=self.proj[:n])
             self.tp.all_reduce(self.proj[:n])
             ops.add_rmsnorm(self.hidden, self.proj, ly["ln2"], self.normed, n, self.eps)
-            self._prefetch_join()
             self._gate_up_act(ly, n)
-            self._prefetch_join()
-            self._linear(l, "d", self.act, ly["wd"], self.proj, n)
-            if self.pf_budget is not None:          # window D: residual + RMSNorm before the next layer's qkv / lm_head
-                nw = self.layers[l + 1]["wqkv"] if l + 1 < self.L else (None if skip_lm_head else self.lm_head)
-                if nw is not None:
-                    self._prefetch(3, [(nw, 0)])
+            torch.mm(self.act[:n], ly["wd"].t(), out=self.proj[:n])
             self.tp.all_reduce(self.proj[:n])
             ops.add_rmsnorm(self.hidden, self.proj, nxt, self.normed, n, self.eps)
         if skip_lm_head:                               # TP follower ranks: only rank 0 consumes logits
-            self._prefetch_join()
             return None
-        self._prefetch_join()
         end = n if logits_to is None else logits_to
         m = end - logits_from
         out = logits_out if logits_out is not None else self.logits[:m]

@@ -186,16 +186,6 @@ def accept_greedy(target_token, succ_off, succ, depth, S, tokens, position_ids, 
           "sq_accept_greedy")
 
 
-def l2_prefetch(w: torch.Tensor, col_from: int, col_to: int):
-    """Hint: pull columns [col_from, col_to) of every row of the 2-D row-major tensor `w` into L2 (current stream)."""
-    es = w.element_size()
-    col_to = min(col_to, w.shape[1])
-    if col_to <= col_from:
-        return
-    check(_lib.load().sq_l2_prefetch(ptr(w), w.stride(0) * es, w.shape[0], col_from * es, (col_to - col_from) * es,
-                                     stream_ptr()), "sq_l2_prefetch")
-
-
 GEMM_TILED, GEMM_SWIGLU = 1, 2          # sq_gemm_plan_create_ex flags (include/sequoia_b200.h)
 
 
@@ -271,40 +261,22 @@ class GemmPlan:
             pass
 
 
-# ---- fused draft forward (csrc/sq_draft.cu) -------------------------------------------------------------------------------
-def draft_supported(hidden, inter, n_layers, n_heads, n_kv_heads, head_dim, vocab, max_length) -> bool:
-    return bool(_lib.load().sq_draft_supported(hidden, inter, n_layers, n_heads, n_kv_heads, head_dim, vocab, max_length))
+# ---- draft attention (csrc/sq_draft.cu) -----------------------------------------------------------------------------------
+def draft_supported(hidden, n_heads, n_kv_heads, head_dim, max_length) -> bool:
+    return bool(_lib.load().sq_draft_supported(hidden, n_heads, n_kv_heads, head_dim, max_length))
 
 
 class DraftPlan:
-    """One persistent cooperative kernel per draft-tree level: embed -> L decoder layers -> lm_head for <= 64 rows."""
+    """Tree-masked attention of the small draft model's forwards of <= 64 rows, K/V read from the engine's caches."""
     MAX_ROWS = 64
 
-    def __init__(self, hidden, inter, n_heads, vocab, max_length, eps, embed, layers, final_norm, lm_head, cos, sin,
-                 k_cache, v_cache):
-        lib = _lib.load()
-        dev = embed.device
-        ws_bytes = lib.sq_draft_workspace_bytes(hidden, inter)
-        if ws_bytes <= 0:
-            raise _lib.SequoiaLibError("sq_draft_workspace_bytes: unsupported shape")
-        self.workspace = torch.zeros(ws_bytes, dtype=torch.uint8, device=dev)
-        flat = []
-        for ly in layers:
-            flat += [ly["wqkv"], ly["wo"], ly["wgu"], ly["wd"], ly["ln1"], ly["ln2"]]
-        for t in flat + [embed, final_norm, lm_head, cos, sin, k_cache, v_cache]:
+    def __init__(self, hidden, n_layers, n_heads, max_length, k_cache, v_cache):
+        for t in (k_cache, v_cache):
             assert t.dtype == F16 and t.is_contiguous()
-        self._keep = (flat, embed, final_norm, lm_head, cos, sin, k_cache, v_cache)
-        arr = (C.c_void_p * len(flat))(*[t.data_ptr() for t in flat])
+        self._keep = (k_cache, v_cache)
         self.handle = C.c_void_p()
-        check(lib.sq_draft_plan_create(C.byref(self.handle), hidden, inter, len(layers), n_heads, vocab, max_length, float(eps),
-                                       ptr(embed), arr, ptr(final_norm), ptr(lm_head), ptr(cos), ptr(sin), ptr(k_cache),
-                                       ptr(v_cache), ptr(self.workspace), ws_bytes), "sq_draft_plan_create")
-
-    def forward(self, n, tokens, position_ids, storage_ids, state, n0, kv_end, tree_bits, tree_words, tree_size, logits_out):
-        assert logits_out.dtype == F16 and logits_out.stride(-1) == 1 and logits_out.shape[0] >= n
-        check(_lib.load().sq_draft_forward(self.handle, n, ptr(tokens), ptr(position_ids), ptr(storage_ids), ptr(state), n0,
-                                           kv_end, ptr(tree_bits), tree_words, tree_size, ptr(logits_out),
-                                           logits_out.stride(0), stream_ptr()), "sq_draft_forward")
+        check(_lib.load().sq_draft_plan_create(C.byref(self.handle), hidden, n_layers, n_heads, max_length, ptr(k_cache),
+                                               ptr(v_cache)), "sq_draft_plan_create")
 
     def attention(self, layer, n, qkv, attn_out, state, n0, kv_end, tree_bits, tree_words, tree_size):
         check(_lib.load().sq_draft_attention(self.handle, layer, n, ptr(qkv), ptr(attn_out), ptr(state), n0, kv_end,

@@ -77,12 +77,14 @@ def test_gemm_dispatch_table_is_swept():
     assert table == cases.GEMM_VARIANTS
 
 
-def test_draft_attention_max_length_limit():
-    """The draft kernel keeps the whole K/V of a head in shared memory: for the 68m draft shape (h = 768, 12 heads of 64,
-    2 layers) 640 is the longest max_length that fits, and 672 (the next multiple of 32) must be refused."""
+def test_draft_attention_supported_shapes():
+    """The draft attention keeps the whole K/V of a head in shared memory: for the 68m draft shape (h = 768, 12 heads of
+    64) 640 is the longest max_length that fits, and 672 (the next multiple of 32) must be refused.  A 7B shape (head_dim
+    128) is refused at any length."""
     from sequoia_b200 import ops
-    assert ops.draft_supported(768, 3072, 2, 12, 12, 64, 32000, 640)
-    assert not ops.draft_supported(768, 3072, 2, 12, 12, 64, 32000, 672)
+    assert ops.draft_supported(768, 12, 12, 64, 640)
+    assert not ops.draft_supported(768, 12, 12, 64, 672)
+    assert not ops.draft_supported(4096, 32, 32, 128, 384)
 
 
 def test_product_never_imports_oracle():

@@ -894,7 +894,7 @@ def test_kv_gather_long_index_list():
 @pytest.mark.parametrize("N,K,n,expect", [(1536, 512, 128, None), (768, 3072, 31, None), (6144, 768, 128, None),
                                           (32000, 768, 19, None), (512, 1024, 1, None)])
 def test_weight_streaming_gemm_matches_cublas(N, K, n, expect):
-    """csrc/sq_gemm.cu (experimental, SQ_GEMM=1) vs an fp32 reference and vs cuBLASLt on the same inputs: same fp32
+    """csrc/sq_gemm.cu vs an fp32 reference and vs cuBLASLt on the same inputs: same fp32
     accumulation, one fp16 rounding -> relative error within 1 fp16 ulp of the fp32 result."""
     g = torch.Generator().manual_seed(N + K)
     a = (torch.randn(128, K, generator=g) * 0.5).to(F16).to(DEV)
@@ -1112,34 +1112,24 @@ def test_gemm_swiglu_variant_sweep(bn, stages, mc, tiled):
                    f"2I=[{4 * bn},{3 * bn + 32}] n=[1,64,65,128]: bit-identical, plain GEMM worst err/bound {worst:.3f}")
 
 
-# ------------------------------------------------------------------------------------------------ fused draft forward
-@pytest.mark.parametrize("mode", ["attn", "chain", "coop"])
+# ------------------------------------------------------------------------------------------------ draft attention in the forward
 @pytest.mark.parametrize("hidden,inter,heads,layers,M", [(768, 3072, 12, 2, 384), (512, 1024, 8, 3, 256)])
-def test_fused_draft_forward_matches_multi_kernel_path(hidden, inter, heads, layers, M, mode):
-    """csrc/sq_draft.cu (one persistent cooperative kernel per tree level) against the multi-kernel forward of the same
-    LlamaRunner weights: same prefill, then every level of the 128-node config-2 tree, a 1-row forward (the bonus token of
-    prepare_for_next_iter) and a 64-row level.  Logits within 3e-3 of the row's max |logit| (different GEMM tiling /
-    attention reduction order, same fp16 rounding points), appended K/V rows within 2 fp16 ulp."""
+def test_draft_attention_forward_matches_wgmma_attention(hidden, inter, heads, layers, M):
+    """LlamaRunner forwards with the draft attention kernel (csrc/sq_draft.cu, the default for tree-relative forwards of
+    <= 64 rows) against the same weights with the wgmma tree attention (SQ_DRAFT_ATTN=0): same prefill, then every level
+    of the 128-node config-2 tree, a 1-row forward (the bonus token of prepare_for_next_iter) and a 64-row level.  Logits
+    within 3e-3 of the row's max |logit| (different attention reduction order, same fp16 rounding points), appended K/V
+    rows within 2 fp16 ulp."""
     from sequoia_b200.model import LlamaRunner
     from sequoia_b200.tree import pack_tree_mask
     cfg = O.LlamaCfg(hidden_size=hidden, intermediate_size=inter, num_hidden_layers=layers, num_attention_heads=heads,
                      num_key_value_heads=heads, vocab_size=cases.V)
     w = O.init_llama_weights(cfg, 4242)
     spec = {"config": cfg, "state_dict": w}
-    os.environ["SQ_DRAFT_FUSED"] = "0"
-    os.environ["SQ_DRAFT_ATTN"] = "0"
-    try:
-        ref = LlamaRunner(spec, M, device=DEV)   # pure multi-kernel path incl. the wgmma attention kernel
-        # "attn" (the default): only the small-shape attention phase replaces sq_tree_attn; "chain": the whole forward as
-        # PDL-chained phase launches; "coop": one cooperative launch
-        os.environ["SQ_DRAFT_ATTN"] = "1"
-        os.environ["SQ_DRAFT_FUSED"] = "0" if mode == "attn" else mode
-        fused = LlamaRunner(spec, M, device=DEV)
-    finally:
-        os.environ.pop("SQ_DRAFT_FUSED", None)
-        os.environ.pop("SQ_DRAFT_ATTN", None)
-    assert ref.draft_plan is None and fused.draft_plan is not None, "the draft kernels must engage for this shape"
-    assert fused.draft_fused == (mode != "attn")
+    with _env(SQ_DRAFT_ATTN="0"):
+        ref = LlamaRunner(spec, M, device=DEV)   # the wgmma attention kernel in every forward
+    dra = LlamaRunner(spec, M, device=DEV)
+    assert ref.draft_plan is None and dra.draft_plan is not None, "the draft attention must engage for this shape"
     gm = cases.load_growmap("A100_growmaps/68m_7b/growmaps/A100-CNN-68m-7b-stochastic.pt")
     S = gm["size"]
     P = 96
@@ -1154,9 +1144,9 @@ def test_fused_draft_forward_matches_multi_kernel_path(hidden, inter, heads, lay
     state[0] = P
     bits = pack_tree_mask(gm["mask"]).to(DEV)
     kw = dict(tree_bits=bits, tree_words=bits.shape[1], tree_size=S)
-    for rn in (ref, fused):          # causal prefill of the P prompt rows (multi-kernel path in both: state=None)
+    for rn in (ref, dra):          # causal prefill of the P prompt rows (multi-kernel path in both: state=None)
         rn.forward(P, tokens, pos, sto, state=None, n0=0, kv_end=P, prefix_len=P, logits_from=P - 1)
-    assert torch.equal(ref.k_cache, fused.k_cache)
+    assert torch.equal(ref.k_cache, dra.k_cache)
     levels = []
     first = 1
     for br in gm["branches"][:-1]:
@@ -1169,18 +1159,18 @@ def test_fused_draft_forward_matches_multi_kernel_path(hidden, inter, heads, lay
         la = torch.zeros(n, cases.V, dtype=F16, device=DEV)
         lb = torch.zeros(n, cases.V, dtype=F16, device=DEV)
         ref.forward(n, tokens, pos, sto, state=state, n0=n0, kv_end=n0 + n, logits_out=la, **kw)
-        fused.forward(n, tokens, pos, sto, state=state, n0=n0, kv_end=n0 + n, logits_out=lb, **kw)
+        dra.forward(n, tokens, pos, sto, state=state, n0=n0, kv_end=n0 + n, logits_out=lb, **kw)
         torch.cuda.synchronize()
         scale = la.float().abs().amax(dim=-1, keepdim=True)
         rel = ((la.float() - lb.float()).abs() / scale).max().item()
         worst = max(worst, rel)
-        # measured: 1.2e-3 - 1.4e-3 (chain / coop); two fp16 implementations of the same layer stack differ by ~2e-3 at most
-        # (cf. the 7B-shaped layer test), so the bound is 3e-3
-        assert rel < 3e-3, f"level n0={n0} n={n}: fused draft logits differ by {rel:.3e}"
+        # two fp16 implementations of the same layer stack differ by ~2e-3 at most (cf. the 7B-shaped layer test), so the
+        # bound is 3e-3
+        assert rel < 3e-3, f"level n0={n0} n={n}: draft-attention logits differ by {rel:.3e}"
         sl = slice(P - 1 + n0, P - 1 + n0 + n)
         # V rows are GEMM outputs: the two fp32 accumulation orders round to the same or the neighbouring fp16 value.  K rows
         # went through RoPE (a*cos - b*sin of two such values, with cancellation): bounded relative to the row's magnitude.
-        va, vb = ref.v_cache[:, :, :, sl], fused.v_cache[:, :, :, sl]
+        va, vb = ref.v_cache[:, :, :, sl], dra.v_cache[:, :, :, sl]
         if n0 == 0 and n == 1:
             # layer-0 V of the root row depends only on embed -> RMSNorm -> Wv: exact (fp32) value as the arbiter
             x = w["model.embed_tokens.weight"][int(tokens[P - 1])].float()
@@ -1188,33 +1178,40 @@ def test_fused_draft_forward_matches_multi_kernel_path(hidden, inter, heads, lay
             xn = (w["model.layers.0.input_layernorm.weight"] * xn).float()
             v_exact = (w["model.layers.0.self_attn.v_proj.weight"].float() @ xn).to(F16).view(heads, -1)
             bad_ref, _ = ulp_close(va[0, 0, :, 0].cpu(), v_exact, 1, atol=1e-4)
-            bad_fused, _ = ulp_close(vb[0, 0, :, 0].cpu(), v_exact, 1, atol=1e-4)
-            _log(f"fused draft (h={hidden}): layer-0 V row of the root vs fp32: multi-kernel path {bad_ref} / fused {bad_fused} of "
-                 f"{v_exact.numel()} values beyond 1 ulp")
-            assert bad_fused <= v_exact.numel() * 5e-3, f"fused draft kernel: {bad_fused} V values beyond 1 ulp of the exact product"
+            bad_dra, _ = ulp_close(vb[0, 0, :, 0].cpu(), v_exact, 1, atol=1e-4)
+            _log(f"draft attention (h={hidden}): layer-0 V row of the root vs fp32: wgmma attention {bad_ref} / draft attention "
+                 f"{bad_dra} of {v_exact.numel()} values beyond 1 ulp")
+            assert bad_dra <= v_exact.numel() * 5e-3, f"draft attention: {bad_dra} V values beyond 1 ulp of the exact product"
         nbad, _ = ulp_close(va, vb, 2, atol=2e-3)
         assert nbad <= va.numel() * 5e-3, f"level n0={n0}: {nbad} appended V values beyond 2 ulp"
-        ka, kb = ref.k_cache[:, :, :, sl].float(), fused.k_cache[:, :, :, sl].float()
+        ka, kb = ref.k_cache[:, :, :, sl].float(), dra.k_cache[:, :, :, sl].float()
         kerr = ((ka - kb).abs().amax(dim=-1) / ka.abs().amax(dim=-1).clamp(min=1e-3)).max().item()
         assert kerr < 4e-3, f"level n0={n0}: appended K rows differ by {kerr:.3e} of the row's max"
-    _log(f"fused draft forward [{mode}] (h={hidden} I={inter} L={layers}): max rel logit diff vs the multi-kernel path {worst:.3e}")
+    _log(f"draft attention forward (h={hidden} I={inter} L={layers}): max rel logit diff vs the wgmma attention {worst:.3e}")
 
 
 # ------------------------------------------------------------------------------------------------ draft attention phase
-@pytest.fixture(scope="module")
-def draft68m():
-    """LlamaRunner of the 68m draft shape (h = 768, 12 heads of 64, 2 layers) at the longest max_length the draft
-    attention phase supports (its K/V of a head live in shared memory)."""
+_DRAFT_SHAPES = [(768, 3072, 12), (2048, 5632, 32)]       # (hidden, inter, heads of 64)
+
+
+def _draft_runner(hidden, inter, heads):
+    """LlamaRunner of a draft shape at the longest max_length the draft attention supports (its K/V of a head live in
+    shared memory), 2 layers, random caches: the 68m draft (h = 768, 12 heads) and a wide one (h = 2048, 32 heads,
+    inter % h != 0)."""
     from sequoia_b200.model import LlamaRunner
-    cfg = O.LlamaCfg(hidden_size=768, intermediate_size=3072, num_hidden_layers=2, num_attention_heads=12,
-                     num_key_value_heads=12, vocab_size=cases.V)
-    with _env(SQ_DRAFT_FUSED="0", SQ_DRAFT_ATTN="1"):
-        runner = LlamaRunner({"config": cfg, "state_dict": O.init_llama_weights(cfg, 68)}, 640, device=DEV)
-    assert runner.draft_plan is not None, "the draft attention phase must engage for the 68m shape at max_length 640"
+    cfg = O.LlamaCfg(hidden_size=hidden, intermediate_size=inter, num_hidden_layers=2, num_attention_heads=heads,
+                     num_key_value_heads=heads, vocab_size=cases.V)
+    runner = LlamaRunner({"config": cfg, "state_dict": O.init_llama_weights(cfg, 68)}, 640, device=DEV)
+    assert runner.draft_plan is not None, f"the draft attention must engage for h={hidden} at max_length 640"
     g = torch.Generator(device=DEV).manual_seed(680)
     runner.k_cache.copy_(torch.randn(runner.k_cache.shape, generator=g, device=DEV).to(F16))
     runner.v_cache.copy_(torch.randn(runner.v_cache.shape, generator=g, device=DEV).to(F16))
     return runner
+
+
+@pytest.fixture(scope="module", params=_DRAFT_SHAPES, ids=["h768", "h2048"])
+def draft_runner(request):
+    return _draft_runner(*request.param)
 
 
 def _draft_attn_rows():
@@ -1229,7 +1226,7 @@ def _draft_attn_rows():
 
 
 def _draft_attn_run(runner, gm, bits, layer, n0, n, P, qkv, out, state):
-    H, D = 12, 64
+    H, D = runner.H, runner.D
     kv_end = n0 + n
     kv_len = P - 1 + kv_end
     out.fill_(SENT)
@@ -1243,20 +1240,22 @@ def _draft_attn_run(runner, gm, bits, layer, n0, n, P, qkv, out, state):
 
 
 @pytest.mark.parametrize("P", [40, 200, 513])
-def test_draft_attention_phase_vs_float64(draft68m, P):
+def test_draft_attention_phase_vs_float64(draft_runner, P):
     """sq_draft_attention (the default attention of every draft forward of <= 64 rows) against the float64 reference:
-    every level of the config-2 tree and n = 1, 15, 16, 17, 33, 64, in layers 0 and 1.  P = 40 keeps kv_len below 256
-    (one 32-key block per warp), 200 crosses it (the 8-warp round-robin wraps), 513 reaches kv_len = 640 = max_length;
-    most kv_len are not multiples of 32 (zero-padded last block).  In layer 1 the late prefix keys [P-65, P-33) are
-    boosted 8x: the running maximum jumps there and every earlier block of that warp is rescaled.  Rows n..63 of the
-    output buffer keep their sentinel.  Bound: _attn_tol (two fp16 roundings here -- P and the output -- within its three)."""
-    runner = draft68m
+    every level of the config-2 tree and n = 1, 15, 16, 17, 33, 64, in layers 0 and 1, for both draft_runner shapes.
+    P = 40 keeps kv_len below 256 (one 32-key block per warp), 200 crosses it (the 8-warp round-robin wraps), 513 reaches
+    kv_len = 640 = max_length; most kv_len are not multiples of 32 (zero-padded last block).  In layer 1 the late prefix
+    keys [P-65, P-33) are boosted 8x: the running maximum jumps there and every earlier block of that warp is rescaled.
+    Rows n..63 of the output buffer keep their sentinel.  Bound: _attn_tol (two fp16 roundings here -- P and the output --
+    within its three)."""
+    runner = draft_runner
+    h = runner.h
     gm, rows = _draft_attn_rows()
     from sequoia_b200.tree import pack_tree_mask
     bits = pack_tree_mask(gm["mask"]).to(DEV)
     g = torch.Generator(device=DEV).manual_seed(P)
-    qkv = torch.randn(64, 3 * 768, generator=g, device=DEV).to(F16)
-    out = torch.full((64, 768), SENT, dtype=F16, device=DEV)
+    qkv = torch.randn(64, 3 * h, generator=g, device=DEV).to(F16)
+    out = torch.full((64, h), SENT, dtype=F16, device=DEV)
     state = torch.zeros(16, dtype=torch.int32, device=DEV)
     saved = runner.k_cache[1].clone()
     if P > 65:
@@ -1266,28 +1265,32 @@ def test_draft_attention_phase_vs_float64(draft68m, P):
         for layer in (0, 1):
             for n0, n in rows:
                 got, ref, tol, _, _, kv_len = _draft_attn_run(runner, gm, bits, layer, n0, n, P, qkv, out, state)
-                what = f"draft attention P={P} layer={layer} n0={n0} n={n} kv_len={kv_len}"
+                what = f"draft attention h={h} P={P} layer={layer} n0={n0} n={n} kv_len={kv_len}"
                 worst = max(worst, _assert_within(got, ref, tol, what))
                 assert bool((out[n:] == SENT).all()), f"{what}: rows >= n were written"
                 kvs.add(kv_len)
     finally:
         runner.k_cache[1].copy_(saved)
-    cases.log_line("variant_sweep.log", f"draft attention P={P} layers=0,1 (n0,n)={rows} kv_len={min(kvs)}..{max(kvs)} "
+    cases.log_line("variant_sweep.log", f"draft attention h={h} P={P} layers=0,1 (n0,n)={rows} kv_len={min(kvs)}..{max(kvs)} "
                    f"boosted={'layer 1' if P > 65 else 'none'}: worst err/bound {worst:.3f}")
 
 
-def test_draft_attention_tolerance_sees_errors(draft68m):
-    """Negative controls for the draft attention bound on one of its cases (layer 1, P = 513, the last 64 tree rows)."""
-    runner = draft68m
+def test_draft_attention_tolerance_sees_errors():
+    """Negative controls for the draft attention bound on one of its cases (layer 1, P = 513, the last 64 tree rows), for
+    both draft shapes."""
     gm, _ = _draft_attn_rows()
     from sequoia_b200.tree import pack_tree_mask
     bits = pack_tree_mask(gm["mask"]).to(DEV)
-    g = torch.Generator(device=DEV).manual_seed(513)
-    qkv = torch.randn(64, 3 * 768, generator=g, device=DEV).to(F16)
-    out = torch.full((64, 768), SENT, dtype=F16, device=DEV)
-    state = torch.zeros(16, dtype=torch.int32, device=DEV)
     n0, n, P = 64, 64, 513
-    got, ref, tol, p, vis, kv_len = _draft_attn_run(runner, gm, bits, 1, n0, n, P, qkv, out, state)
-    _assert_within(got, ref, tol, "draft attention negative control (exact reference)")
-    _negative_controls(got, qkv[:n, :768].view(n, 12, 64), runner.k_cache[1, 0, :, :kv_len], runner.v_cache[1, 0, :, :kv_len],
-                       vis, 12, 12, 64, tol, p, "draft attention")
+    for shape in _DRAFT_SHAPES:
+        runner = _draft_runner(*shape)
+        h, H = runner.h, runner.H
+        g = torch.Generator(device=DEV).manual_seed(513)
+        qkv = torch.randn(64, 3 * h, generator=g, device=DEV).to(F16)
+        out = torch.full((64, h), SENT, dtype=F16, device=DEV)
+        state = torch.zeros(16, dtype=torch.int32, device=DEV)
+        got, ref, tol, p, vis, kv_len = _draft_attn_run(runner, gm, bits, 1, n0, n, P, qkv, out, state)
+        _assert_within(got, ref, tol, f"draft attention h={h} negative control (exact reference)")
+        _negative_controls(got, qkv[:n, :h].view(n, H, 64), runner.k_cache[1, 0, :, :kv_len],
+                           runner.v_cache[1, 0, :, :kv_len], vis, H, H, 64, tol, p, f"draft attention h={h}")
+        del runner
