@@ -16,7 +16,7 @@ from typing import Dict, List, Optional, Sequence
 import torch
 
 from . import _lib, ops
-from .tree import _Static
+from .tree import _Static, check_vocab
 
 F16 = torch.float16
 ST_P, ST_M, ST_FROZEN = 0, 8, 9
@@ -60,6 +60,7 @@ class BatchTree:
         self.st = st = _Static(grow_map, dev)
         S = self.S = st.S
         V = self.V = draft.engine.model_config.vocab_size
+        check_vocab(policy, V)
         M = max_length
         for p in prompts:
             if len(p) + S - 1 > M:

@@ -244,18 +244,25 @@ __global__ void accept_greedy_kernel(const int64_t* __restrict__ target_token, c
 
 using namespace sq;
 
+// SQ_ACCEPT_IMPL (read once): 1 = the cluster walk (default), 0 = the single-CTA cross-check walk
+static int accept_impl() {
+  static const int impl = [] { const char* e = getenv("SQ_ACCEPT_IMPL"); return e ? atoi(e) : 1; }();
+  return impl;
+}
+
 extern "C" int sq_accept_stochastic(const sq_half* target_logits, int64_t ld_t, const sq_half* draft_logits,
                                     int64_t ld_d, const sq_half* r, const sq_half* noise, const int32_t* succ_off,
                                     const int32_t* succ, const int32_t* depth, int S, int V, float T, int64_t* tokens,
                                     int64_t* position_ids, int32_t* accept_idx, int32_t* state, int max_target_seq,
                                     int policy, void* stream) {
-  SQ_CHECK_ARG(V % 8 == 0 && V > 0 && V <= ANT * ACH * 8, "sq_accept_stochastic: V=%d unsupported", V);
   SQ_CHECK_ARG(S >= 1 && S <= 1024, "sq_accept_stochastic: S=%d unsupported", S);
   SQ_CHECK_ARG((policy & ~3) == 0, "sq_accept_stochastic: unknown policy bits %d", policy);
-  static const int impl = [] { const char* e = getenv("SQ_ACCEPT_IMPL"); return e ? atoi(e) : 1; }();
-  if (impl == 1)   // product path: 8-CTA cluster kernel (sq_accept_cluster.cu); impl 0 = single-CTA cross-check
+  if (accept_impl() == 1)   // product path: 8-CTA cluster kernel (sq_accept_cluster.cu); impl 0 = single-CTA cross-check
     return sq::launch_accept_cluster(target_logits, ld_t, draft_logits, ld_d, r, noise, succ_off, succ, depth, S, V, T,
                                      tokens, position_ids, accept_idx, state, max_target_seq, policy, stream);
+  SQ_CHECK_ARG(V % 8 == 0 && V > 0 && V <= ANT * ACH * 8,
+               "sq_accept_stochastic: V=%d unsupported by the single-CTA walk (SQ_ACCEPT_IMPL=0): multiple of 8, <= 32768",
+               V);
   accept_stochastic_kernel<<<1, ANT, 0, (cudaStream_t)stream>>>(
       (const __half*)target_logits, ld_t, (const __half*)draft_logits, ld_d, (const __half*)r, (const __half*)noise,
       succ_off, succ, depth, S, V, 1.0f / T, tokens, position_ids, accept_idx, state, max_target_seq, policy);

@@ -3,7 +3,12 @@
 // partials are exchanged through distributed shared memory with ONE cluster barrier per tested child:
 // every CTA speculatively computes its share of the residual sum while the CTA owning the tested token evaluates the
 // accept rule, and both travel in the same exchange.  Per child: ~8 exp + 8 div per thread + 1 cluster.sync.
+// NCH = 16-byte chunks per thread (V <= CL*CNT*8*NCH): 1 up to V = 32768, up to 4 (V <= 131072) for large vocabularies.
+// CTA r owns chunks [r*cpb, (r+1)*cpb); thread t holds its CTA's chunks i*CNT + t.  With NCH > 1 the bonus keys carry
+// CTA-local indices (< 16384) and are merged in rank order, so equal maxima still resolve to the lowest index.
 #include <cooperative_groups.h>
+
+#include <type_traits>
 
 #include "sq_common.cuh"
 #include "sq_accept_common.cuh"
@@ -70,7 +75,7 @@ struct ClusterCtx {
 
 // BATCH: grid (CL, B), one cluster per sequence (see BatchArgs); a frozen sequence's cluster exits before its first
 // exchange (the whole cluster reads the same word).
-template <bool BATCH>
+template <bool BATCH, int NCH>
 __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(CNT) accept_stochastic_cluster_kernel(
     const __half* __restrict__ target_logits, int64_t ld_t, const __half* __restrict__ draft_logits, int64_t ld_d,
     const __half* __restrict__ r, const __half* __restrict__ noise, const int32_t* __restrict__ succ_off,
@@ -81,6 +86,7 @@ __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(CNT) accept_stochas
   __shared__ float red[CNW];
   __shared__ int32_t sh_acc[1024];
   __shared__ float sh_own[2];                    // owner thread -> block: {etok, flag bits as float}
+  if constexpr (NCH > 1) pdl_wait();
   const int b = seq_index<BATCH>(blockIdx.y);
   if (BATCH) {
     state += b * ST_WORDS;
@@ -96,26 +102,35 @@ __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(CNT) accept_stochas
   cx.rank = (int)cx.cluster.block_rank();
   const int P = state[ST_P];
   const int nvec = V / 8;
-  const int cpb = (nvec + CL - 1) / CL;          // chunks per CTA (<= CNT)
-  const int chunk = cx.rank * cpb + threadIdx.x;
-  const bool active = threadIdx.x < cpb && chunk < nvec;
+  const int cpb = (nvec + CL - 1) / CL;          // chunks per CTA (<= CNT * NCH)
+  int chunk[NCH];
+  bool active[NCH];
+#pragma unroll
+  for (int i = 0; i < NCH; ++i) {
+    chunk[i] = cx.rank * cpb + i * CNT + threadIdx.x;
+    active[i] = i * CNT + threadIdx.x < cpb && chunk[i] < nvec;
+  }
   const uint4 NEG_INF = make_uint4(0xFC00FC00u, 0xFC00FC00u, 0xFC00FC00u, 0xFC00FC00u);
-  Pack8 p, xd;
+  Pack8 p[NCH], xd[NCH];
   int cur = 0, n_new = 0;
   bool terminal = false;
   while (true) {
     const int c0 = succ_off[cur], c1 = succ_off[cur + 1];
     const bool leaf = (c0 == c1);
     // load + scale both rows; softmax statistics of both in two exchanges
-    p.u = active ? reinterpret_cast<const uint4*>(target_logits + cur * ld_t)[chunk] : NEG_INF;
-    xd.u = (active && !leaf) ? reinterpret_cast<const uint4*>(draft_logits + ba.row<BATCH>(cur, b) * ld_d)[chunk] : NEG_INF;
     float m1 = -INFINITY, m2 = -INFINITY;
 #pragma unroll
-    for (int e = 0; e < 8; ++e) {
-      p.h[e] = f2h(h2f(p.h[e]) * inv_T);
-      xd.h[e] = f2h(h2f(xd.h[e]) * inv_T);
-      m1 = fmaxf(m1, h2f(p.h[e]));
-      m2 = fmaxf(m2, h2f(xd.h[e]));
+    for (int i = 0; i < NCH; ++i) {
+      p[i].u = active[i] ? reinterpret_cast<const uint4*>(target_logits + cur * ld_t)[chunk[i]] : NEG_INF;
+      xd[i].u = (active[i] && !leaf) ? reinterpret_cast<const uint4*>(draft_logits + ba.row<BATCH>(cur, b) * ld_d)[chunk[i]]
+                                     : NEG_INF;
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        p[i].h[e] = f2h(h2f(p[i].h[e]) * inv_T);
+        xd[i].h[e] = f2h(h2f(xd[i].h[e]) * inv_T);
+        m1 = fmaxf(m1, h2f(p[i].h[e]));
+        m2 = fmaxf(m2, h2f(xd[i].h[e]));
+      }
     }
     m1 = block_max<CNW>(m1, red);
     m2 = block_max<CNW>(m2, red);
@@ -125,10 +140,12 @@ __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(CNT) accept_stochas
     cx.next();
     float s1 = 0.f, s2 = 0.f;
 #pragma unroll
-    for (int e = 0; e < 8; ++e) {
-      s1 += __expf(h2f(p.h[e]) - mxt);
-      s2 += __expf(h2f(xd.h[e]) - mxd);
-    }
+    for (int i = 0; i < NCH; ++i)
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        s1 += __expf(h2f(p[i].h[e]) - mxt);
+        s2 += __expf(h2f(xd[i].h[e]) - mxd);
+      }
     s1 = block_sum<CNW>(s1, red);
     s2 = block_sum<CNW>(s2, red);
     cx.exchange(s1, s2, 0.f, 0.f, 0u, 0u);
@@ -136,7 +153,9 @@ __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(CNT) accept_stochas
     float sumd = cx.fsum(1);
     cx.next();
 #pragma unroll
-    for (int e = 0; e < 8; ++e) p.h[e] = f2h(__fdividef(__expf(h2f(p.h[e]) - mxt), sumt));   // p = softmax(target/T)
+    for (int i = 0; i < NCH; ++i)
+#pragma unroll
+      for (int e = 0; e < 8; ++e) p[i].h[e] = f2h(__fdividef(__expf(h2f(p[i].h[e]) - mxt), sumt));   // p = softmax(target/T)
     if (leaf) break;                                         // residual = p   (SpecTree.py:143-144)
     int accepted = -1;
     for (int ci = c0; ci < c1; ++ci) {
@@ -144,29 +163,34 @@ __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(CNT) accept_stochas
       const int slot = P - 1 + child;
       const int tok = (int)tokens[slot];
       const int tc = tok >> 3, te = tok & 7;
-      const bool owner = (tc / cpb == cx.rank) && (threadIdx.x == tc % cpb);
+      // owner of the tested token: chunk own_i of this thread (-1: not this thread)
+      int own_i;
+      if constexpr (NCH == 1) own_i = ((tc / cpb == cx.rank) && (threadIdx.x == tc % cpb)) ? 0 : -1;
+      else own_i = ((tc / cpb == cx.rank) && ((tc % cpb) % CNT == threadIdx.x)) ? (tc % cpb) / CNT : -1;
       if (threadIdx.x == 0) { sh_own[0] = 0.f; sh_own[1] = 0.f; }
       __syncthreads();
       // speculative residual share: d = relu(fp16(p - q)), partial sum
-      Pack8 dtmp;
+      Pack8 dtmp[NCH];
       float s = 0.f;
 #pragma unroll
-      for (int e = 0; e < 8; ++e) {
-        const float q = h2f(f2h(__fdividef(__expf(h2f(xd.h[e]) - mxd), sumd)));
-        float d = rnd16(h2f(p.h[e]) - q);
-        d = (d < 0.f) ? 0.f : d;                             // relu_; NaN propagates like torch
-        dtmp.h[e] = f2h(d);
-        s += d;
-        if (owner && e == te) {
-          const float etok = __expf(h2f(xd.h[e]) - mxd);
-          const float thr = rnd16(h2f(r[slot]) * q);         // r * q[token] in fp16
-          const float pv = h2f(p.h[e]);
-          // strict > (SpecTree.py:152); the SpecInfer policy accepts on >= (SpecInferTree.py:158)
-          const int acc = ((policy & SQ_ACCEPT_GE) ? (pv >= thr) : (pv > thr)) ? 1 : 0;
-          sh_own[0] = etok;
-          sh_own[1] = (float)(acc | ((!(policy & SQ_ACCEPT_KEEP_Q) && h2f(xd.h[e]) >= mxd) ? 2 : 0));
+      for (int i = 0; i < NCH; ++i)
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+          const float q = h2f(f2h(__fdividef(__expf(h2f(xd[i].h[e]) - mxd), sumd)));
+          float d = rnd16(h2f(p[i].h[e]) - q);
+          d = (d < 0.f) ? 0.f : d;                           // relu_; NaN propagates like torch
+          dtmp[i].h[e] = f2h(d);
+          s += d;
+          if (own_i == i && e == te) {
+            const float etok = __expf(h2f(xd[i].h[e]) - mxd);
+            const float thr = rnd16(h2f(r[slot]) * q);       // r * q[token] in fp16
+            const float pv = h2f(p[i].h[e]);
+            // strict > (SpecTree.py:152); the SpecInfer policy accepts on >= (SpecInferTree.py:158)
+            const int acc = ((policy & SQ_ACCEPT_GE) ? (pv >= thr) : (pv > thr)) ? 1 : 0;
+            sh_own[0] = etok;
+            sh_own[1] = (float)(acc | ((!(policy & SQ_ACCEPT_KEEP_Q) && h2f(xd[i].h[e]) >= mxd) ? 2 : 0));
+          }
         }
-      }
       s = block_sum<CNW>(s, red);                            // (contains the barriers that publish sh_own)
       cx.exchange(s, sh_own[0], 0.f, 0.f, (uint32_t)sh_own[1], 0u);
       const float tot = rnd16(cx.fsum(0));
@@ -175,23 +199,29 @@ __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(CNT) accept_stochas
       cx.next();
       if (flag & 1u) { accepted = child; break; }
 #pragma unroll
-      for (int e = 0; e < 8; ++e) {
-        p.h[e] = f2h(h2f(dtmp.h[e]) / tot);                  // get_residual (utils.py:5-8)
-        if (owner && e == te && !(policy & SQ_ACCEPT_KEEP_Q))
-          xd.h[e] = __ushort_as_half((unsigned short)0xFC00u);   // draft_logits[token] = min (SpecTree.py:156)
-      }
+      for (int i = 0; i < NCH; ++i)
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+          p[i].h[e] = f2h(h2f(dtmp[i].h[e]) / tot);          // get_residual (utils.py:5-8)
+          if (own_i == i && e == te && !(policy & SQ_ACCEPT_KEEP_Q))
+            xd[i].h[e] = __ushort_as_half((unsigned short)0xFC00u);   // draft_logits[token] = min (SpecTree.py:156)
+        }
       if (policy & SQ_ACCEPT_KEEP_Q) continue;               // SpecInfer: q stays softmax(draft/T) for every child
       if (flag & 2u) {                                       // rare: the masked token held the max -> new statistics
         float m = -INFINITY;
 #pragma unroll
-        for (int e = 0; e < 8; ++e) m = fmaxf(m, h2f(xd.h[e]));
+        for (int i = 0; i < NCH; ++i)
+#pragma unroll
+          for (int e = 0; e < 8; ++e) m = fmaxf(m, h2f(xd[i].h[e]));
         m = block_max<CNW>(m, red);
         cx.exchange(m, 0.f, 0.f, 0.f, 0u, 0u);
         mxd = cx.fmax_(0);
         cx.next();
         float ss = 0.f;
 #pragma unroll
-        for (int e = 0; e < 8; ++e) ss += __expf(h2f(xd.h[e]) - mxd);
+        for (int i = 0; i < NCH; ++i)
+#pragma unroll
+          for (int e = 0; e < 8; ++e) ss += __expf(h2f(xd[i].h[e]) - mxd);
         ss = block_sum<CNW>(ss, red);
         cx.exchange(ss, 0.f, 0.f, 0.f, 0u, 0u);
         sumd = cx.fsum(0);
@@ -212,14 +242,19 @@ __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(CNT) accept_stochas
   int64_t bonus = -1;
   if (!terminal) {
     uint32_t has_nan = 0u, best = 0u;
-    if (active) {
-      Pack8 nz;
-      nz.u = reinterpret_cast<const uint4*>(noise)[chunk];
 #pragma unroll
-      for (int e = 0; e < 8; ++e) {
-        has_nan |= __hisnan(p.h[e]) ? 1u : 0u;
-        const __half v = f2h(h2f(p.h[e]) / h2f(nz.h[e]));    // multinomial(1) = argmax(residual / Exp(1))  (:222)
-        best = max(best, (c_ord16(v) << 16) | (0xFFFFu - (uint32_t)(chunk * 8 + e)));
+    for (int i = 0; i < NCH; ++i) {
+      if (active[i]) {
+        Pack8 nz;
+        nz.u = reinterpret_cast<const uint4*>(noise)[chunk[i]];
+        // key index field: the vocabulary index (NCH == 1), or the CTA-local one (< cpb * 8 <= 16384)
+        const uint32_t ib = NCH == 1 ? (uint32_t)chunk[i] * 8 : (uint32_t)(i * CNT + threadIdx.x) * 8;
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+          has_nan |= __hisnan(p[i].h[e]) ? 1u : 0u;
+          const __half v = f2h(h2f(p[i].h[e]) / h2f(nz.h[e]));   // multinomial(1) = argmax(residual / Exp(1))  (:222)
+          best = max(best, (c_ord16(v) << 16) | (0xFFFFu - (ib + e)));
+        }
       }
     }
     has_nan = __syncthreads_or((int)has_nan) ? 1u : 0u;
@@ -230,7 +265,17 @@ __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(CNT) accept_stochas
     best = __reduce_max_sync(0xffffffffu, (threadIdx.x & 31) < CNW ? redu[threadIdx.x & 31] : 0u);
     cx.exchange(0.f, 0.f, 0.f, 0.f, has_nan, best);
     nan_flag = cx.uor(0) != 0u;                              // torch.isnan(residual).any()  (:219)
-    bonus = (int64_t)(0xFFFFu - (cx.umax(1) & 0xFFFFu));
+    if constexpr (NCH == 1) {
+      bonus = (int64_t)(0xFFFFu - (cx.umax(1) & 0xFFFFu));
+    } else {                                                 // higher value, then the lower rank (strict >)
+      uint32_t bk = 0u;
+      int br = 0;
+      for (int rr = 0; rr < CL; ++rr) {
+        const uint32_t k = cx.x->u[cx.ph][rr][1];
+        if ((k >> 16) > (bk >> 16)) { bk = k; br = rr; }
+      }
+      bonus = (int64_t)br * cpb * 8 + (int64_t)(0xFFFFu - (bk & 0xFFFFu));
+    }
     cx.next();
     if (nan_flag) terminal = true;
   }
@@ -244,22 +289,40 @@ __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(CNT) accept_stochas
 
 using namespace sq;
 
-int sq::launch_accept_cluster(const sq_half* target_logits, int64_t ld_t, const sq_half* draft_logits, int64_t ld_d,
-                              const sq_half* r, const sq_half* noise, const int32_t* succ_off, const int32_t* succ,
-                              const int32_t* depth, int S, int V, float T, int64_t* tokens, int64_t* position_ids,
-                              int32_t* accept_idx, int32_t* state, int max_target_seq, int policy, void* stream,
-                              const BatchArgs* batch) {
-  SQ_CHECK_ARG(V % 8 == 0 && V > 0 && V <= CL * CNT * 8, "sq_accept_stochastic: V=%d unsupported", V);
+template <int NCH>
+static int launch_accept_nch(const sq_half* target_logits, int64_t ld_t, const sq_half* draft_logits, int64_t ld_d,
+                             const sq_half* r, const sq_half* noise, const int32_t* succ_off, const int32_t* succ,
+                             const int32_t* depth, int S, int V, float T, int64_t* tokens, int64_t* position_ids,
+                             int32_t* accept_idx, int32_t* state, int max_target_seq, int policy, void* stream,
+                             const BatchArgs* batch) {
   if (batch) {
-    accept_stochastic_cluster_kernel<true><<<dim3(CL, batch->B), CNT, 0, (cudaStream_t)stream>>>(
+    accept_stochastic_cluster_kernel<true, NCH><<<dim3(CL, batch->B), CNT, 0, (cudaStream_t)stream>>>(
         (const __half*)target_logits, ld_t, (const __half*)draft_logits, ld_d, (const __half*)r, (const __half*)noise,
         succ_off, succ, depth, S, V, 1.0f / T, tokens, position_ids, accept_idx, state, max_target_seq, policy, *batch);
     SQ_CHECK_LAUNCH("sq_accept_stochastic_batch");
     return SQ_OK;
   }
-  accept_stochastic_cluster_kernel<false><<<CL, CNT, 0, (cudaStream_t)stream>>>(
+  accept_stochastic_cluster_kernel<false, NCH><<<CL, CNT, 0, (cudaStream_t)stream>>>(
       (const __half*)target_logits, ld_t, (const __half*)draft_logits, ld_d, (const __half*)r, (const __half*)noise,
       succ_off, succ, depth, S, V, 1.0f / T, tokens, position_ids, accept_idx, state, max_target_seq, policy, BatchArgs{});
   SQ_CHECK_LAUNCH("sq_accept_stochastic(cluster)");
   return SQ_OK;
+}
+
+int sq::launch_accept_cluster(const sq_half* target_logits, int64_t ld_t, const sq_half* draft_logits, int64_t ld_d,
+                              const sq_half* r, const sq_half* noise, const int32_t* succ_off, const int32_t* succ,
+                              const int32_t* depth, int S, int V, float T, int64_t* tokens, int64_t* position_ids,
+                              int32_t* accept_idx, int32_t* state, int max_target_seq, int policy, void* stream,
+                              const BatchArgs* batch) {
+  SQ_CHECK_ARG(V % 8 == 0 && V > 0 && V <= CL * CNT * 8 * 4, "sq_accept_stochastic: V=%d unsupported (multiple of 8, "
+               "<= %d)", V, CL * CNT * 8 * 4);
+  const int nch = (V + CL * CNT * 8 - 1) / (CL * CNT * 8);
+  auto go = [&](auto kern_nch) {
+    return launch_accept_nch<decltype(kern_nch)::value>(target_logits, ld_t, draft_logits, ld_d, r, noise, succ_off, succ,
+                                                        depth, S, V, T, tokens, position_ids, accept_idx, state,
+                                                        max_target_seq, policy, stream, batch);
+  };
+  if (nch == 1) return go(std::integral_constant<int, 1>{});
+  if (nch == 2) return go(std::integral_constant<int, 2>{});
+  return go(std::integral_constant<int, 4>{});
 }

@@ -9,13 +9,72 @@
 //   sc = fp16(fp16(log(u)) / q)               rand.log() and the division are separate fp16 ops
 // exp uses ex2.approx (rel. error ~1e-6, far below the fp16 rounding that follows); log stays full precision
 // because log(u) for u close to 1 decides the top ranks.
+//
+// Large vocabularies (WIDE = true, 32768 < V <= 131072; all but softmax_T): one thread-block cluster of ceil(V / 32768) CTAs per row.  CTA r
+// owns the vocabulary slice [r*32768, (r+1)*32768) and runs the per-CTA code above on it (local indices, so keys keep
+// their 16-bit index field); the row max, the softmax sum, the top-p histograms and the top-k / argmax candidates cross
+// slices through distributed shared memory.  Every value is pushed into the slot of its source rank in the receiving
+// CTAs, then one cluster barrier; partials are combined in rank order, so results do not depend on timing.  Slices are in
+// index order, so candidates merged by (key, rank, local index) still resolve ties to the lower vocabulary index.
+// WIDE = false is the single-CTA kernel, unchanged.
+#include <cooperative_groups.h>
+
 #include "sq_common.cuh"
+
+namespace cg = cooperative_groups;
 
 namespace sq {
 
 constexpr int NT = 1024;
 constexpr int NW = NT / 32;
 constexpr int CH = 4;          // 16-byte chunks per thread: V <= NT*CH*8 = 32768
+constexpr int SLICE = NT * CH * 8;      // vocabulary entries per CTA
+constexpr int MAX_SLICES = 4;           // WIDE: V <= 131072
+constexpr int WIDE_KMAX = 256;          // WIDE top-k: k_max bound (candidate buffer of the merging CTA)
+
+// WIDE row geometry: the row (blockIdx.x / cluster size) and this CTA's slice.  The cluster rank and size are read from
+// their special registers where needed rather than held in registers across the kernel.
+struct Slice {
+  int row, base, V;
+  __device__ __forceinline__ int rank() const { return (int)cg::this_cluster().block_rank(); }
+  __device__ __forceinline__ int n() const { return (int)cg::this_cluster().num_blocks(); }
+};
+__device__ __forceinline__ Slice slice_of(int V) {
+  cg::cluster_group cl = cg::this_cluster();
+  const int r = (int)cl.block_rank(), n = (int)cl.num_blocks();
+  return Slice{(int)blockIdx.x / n, r * SLICE, min(SLICE, V - r * SLICE)};
+}
+
+// Block-uniform v -> slots[s.rank()] of every CTA of the cluster, then a cluster barrier (also a block barrier).  Each call
+// site owns its slots, so no slot is written twice and a CTA may leave after its last exchange.
+template <typename T>
+__device__ __forceinline__ void cl_publish(T v, T* slots, const Slice& s) {
+  cg::cluster_group cl = cg::this_cluster();
+  if ((int)threadIdx.x < s.n()) *cl.map_shared_rank(&slots[s.rank()], (int)threadIdx.x) = v;
+  cl.sync();
+}
+__device__ __forceinline__ float cl_max(float v, float* slots, const Slice& s) {
+  cl_publish(v, slots, s);
+  float m = -INFINITY;
+  for (int r = 0; r < s.n(); ++r) m = fmaxf(m, slots[r]);
+  return m;
+}
+__device__ __forceinline__ float cl_sum(float v, float* slots, const Slice& s) {
+  cl_publish(v, slots, s);
+  float t = 0.f;
+  for (int r = 0; r < s.n(); ++r) t += slots[r];
+  return t;
+}
+
+// slice-local key (ord16 << 16 | 0xFFFF - local index) of rank r -> row-wide key ordered by (value, lower rank, lower
+// index); 0 stays 0 (no candidate)
+__device__ __forceinline__ uint64_t wide_key(uint32_t key, int rank) {
+  return key ? ((uint64_t)(key >> 16) << 32) | ((uint64_t)(MAX_SLICES - 1 - rank) << 16) | (key & 0xFFFFu) : 0ull;
+}
+__device__ __forceinline__ int64_t wide_index(uint64_t k) {
+  const int rank = MAX_SLICES - 1 - (int)((k >> 16) & 0xFFFFu);
+  return (int64_t)rank * SLICE + (int64_t)(0xFFFFu - (uint32_t)(k & 0xFFFFu));
+}
 
 // fp16 bits -> uint16 whose unsigned order equals the float order (-inf lowest, +inf highest)
 __device__ __forceinline__ uint32_t ord16(__half h) {
@@ -62,6 +121,26 @@ __device__ __forceinline__ void scale_and_stats(Pack8 (&x)[CH], float inv_T, flo
   sum = block_sum<NW>(s, red);
 }
 
+// scale_and_stats over the whole row of a WIDE cluster (xs: two exchange slot sets)
+__device__ __forceinline__ void scale_and_stats_wide(Pack8 (&x)[CH], float inv_T, float* red, float (&xs)[2][MAX_SLICES],
+                                                     const Slice& sl, float& mx, float& sum) {
+  float m = -INFINITY;
+#pragma unroll
+  for (int i = 0; i < CH; ++i)
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      x[i].h[j] = f2h(h2f(x[i].h[j]) * inv_T);
+      m = fmaxf(m, h2f(x[i].h[j]));
+    }
+  mx = cl_max(block_max<NW>(m, red), xs[0], sl);
+  float s = 0.f;
+#pragma unroll
+  for (int i = 0; i < CH; ++i)
+#pragma unroll
+    for (int j = 0; j < 8; ++j) s += __expf(h2f(x[i].h[j]) - mx);
+  sum = cl_sum(block_sum<NW>(s, red), xs[1], sl);
+}
+
 __device__ __forceinline__ __half softmax_val(__half xt, float mx, float inv_sum_unused, float sum) {
   return f2h(__fdividef(__expf(h2f(xt) - mx), sum));
 }
@@ -88,9 +167,29 @@ __global__ void __launch_bounds__(NT) softmax_T_kernel(const __half* __restrict_
 }
 
 // ---------------------------------------------------------------------------------------------
+// WIDE top-k, after every CTA pushed its k_need best slice-local keys (0 = none) to gk[rank * k_need + i] of rank 0: the
+// merging CTA ranks the n * k_need candidates (rank = number of larger row-wide keys) and writes the first k_need.
+__device__ __forceinline__ void wide_topk_merge(const uint64_t* gk, int n, int k_need, int j, int k_max, int nb, int base,
+                                                int64_t* __restrict__ positions, int64_t* __restrict__ tokens) {
+  const int total = n * k_need;
+  for (int q = threadIdx.x; q < total; q += NT) {
+    const uint64_t mine = gk[q];
+    if (mine == 0ull) continue;
+    int rank = 0;
+    for (int i = 0; i < total; ++i) rank += (gk[i] > mine) ? 1 : 0;
+    if (rank < k_need) {
+      const int64_t idx = wide_index(mine);
+      if (positions) positions[(int64_t)j * k_max + rank] = idx;
+      if (tokens && rank < nb) tokens[base + rank] = idx;
+    }
+  }
+}
+
 // BATCH: grid (n_parents, B); sequence b reads the logits row drow_base[node] + b * drow_step[node] of parent node `node`,
 // its rand rows at rand + b * ld_rand_seq, writes tokens + b * ld_seq, and does nothing when frozen.
-template <bool BATCH>
+// WIDE: grid (n * n_parents, B), clusters of n = ceil(V / SLICE) CTAs; the whole cluster reads the same frozen word and
+// k_need, so it takes every exit together.
+template <bool BATCH, bool WIDE>
 __global__ void __launch_bounds__(NT) sample_level_kernel(
     const __half* __restrict__ logits, int64_t ld_logits, const __half* __restrict__ rand, int64_t ld_rand,
     const int32_t* __restrict__ parent_rows, const int32_t* __restrict__ child_first,
@@ -99,7 +198,12 @@ __global__ void __launch_bounds__(NT) sample_level_kernel(
     const int32_t* __restrict__ drow_step, int64_t ld_rand_seq, int64_t ld_seq) {
   __shared__ float red[NW];
   __shared__ uint32_t redu[NW];
-  const int j = blockIdx.x;
+  Slice sl{};
+  if constexpr (WIDE) {
+    pdl_wait();
+    sl = slice_of(V);
+  }
+  const int j = WIDE ? sl.row : blockIdx.x;
   const int b = seq_index<BATCH>(blockIdx.y);
   if (BATCH) {
     state += b * ST_WORDS;
@@ -112,6 +216,11 @@ __global__ void __launch_bounds__(NT) sample_level_kernel(
   const int prow = parent_rows ? parent_rows[j] : j;
   const int64_t lrow = BATCH ? (int64_t)drow_base[prow] + (int64_t)b * drow_step[prow] : prow;
   if (BATCH && rand) rand += b * ld_rand_seq;
+  if constexpr (WIDE) {                  // from here on: this CTA's slice, slice-local indices
+    logits += sl.base;
+    if (rand) rand += sl.base;
+    V = sl.V;
+  }
   const int nvec = V / 8;
   uint32_t key[CH * 8];
   {
@@ -119,7 +228,12 @@ __global__ void __launch_bounds__(NT) sample_level_kernel(
     load_row(logits + lrow * ld_logits, V, x);
     if (mode == 0) {
       float mx, sum;
-      scale_and_stats(x, inv_T, red, mx, sum);
+      if constexpr (WIDE) {
+        __shared__ float xs[2][MAX_SLICES];
+        scale_and_stats_wide(x, inv_T, red, xs, sl, mx, sum);
+      } else {
+        scale_and_stats(x, inv_T, red, mx, sum);
+      }
 #pragma unroll
       for (int i = 0; i < CH; ++i) {
         const int c = i * NT + threadIdx.x;
@@ -149,6 +263,13 @@ __global__ void __launch_bounds__(NT) sample_level_kernel(
 #pragma unroll
   for (int e = 0; e < CH * 8; ++e) best = max(best, key[e]);
   const int base = tokens ? row_base(state, child_first[j]) : 0;
+  // WIDE: the k_need best keys of this slice go to the merging CTA (rank 0) instead of the outputs
+  uint64_t* gk = nullptr;
+  if constexpr (WIDE) {
+    __shared__ uint64_t gk_buf[MAX_SLICES * WIDE_KMAX];
+    gk = gk_buf;
+  }
+  cg::cluster_group cl = cg::this_cluster();
   // Fast path (k <= 32): the k-th largest of the 32 warp maxima is a lower bound of the k-th largest key (at least k keys
   // reach it), and usually only a few more do: collect the keys >= that threshold in shared memory and rank them directly
   // (rank = number of larger candidates) -- three block barriers instead of two per selected child.
@@ -182,10 +303,19 @@ __global__ void __launch_bounds__(NT) sample_level_kernel(
         int rank = 0;
         for (int i = 0; i < C; ++i) rank += (cand[i] > mine) ? 1 : 0;
         if (rank < k_need) {
-          const int64_t idx = (int64_t)(0xFFFFu - (mine & 0xFFFFu));
-          if (positions) positions[(int64_t)j * k_max + rank] = idx;
-          if (tokens && rank < nb) tokens[base + rank] = idx;
+          if constexpr (WIDE) {
+            *cl.map_shared_rank(&gk[sl.rank() * k_need + rank], 0) = wide_key(mine, sl.rank());
+          } else {
+            const int64_t idx = (int64_t)(0xFFFFu - (mine & 0xFFFFu));
+            if (positions) positions[(int64_t)j * k_max + rank] = idx;
+            if (tokens && rank < nb) tokens[base + rank] = idx;
+          }
         }
+      }
+      if constexpr (WIDE) {
+        for (int q = C + threadIdx.x; q < k_need; q += NT) *cl.map_shared_rank(&gk[sl.rank() * k_need + q], 0) = 0ull;
+        cl.sync();
+        if (sl.rank() == 0) wide_topk_merge(gk, sl.n(), k_need, j, k_max, nb, base, positions, tokens);
       }
       return;
     }
@@ -193,10 +323,20 @@ __global__ void __launch_bounds__(NT) sample_level_kernel(
   }
   for (int rnd = 0; rnd < k_need; ++rnd) {
     const uint32_t top = block_max_u32(best, redu);
+    if constexpr (WIDE) {                 // a short last slice may run out of keys: push 0 (no candidate)
+      if (top == 0u) {
+        if (threadIdx.x == 0) *cl.map_shared_rank(&gk[sl.rank() * k_need + rnd], 0) = 0ull;
+        continue;
+      }
+    }
     if (best == top) {                    // unique owner (keys embed the index)
-      const int64_t idx = (int64_t)(0xFFFFu - (top & 0xFFFFu));
-      if (positions) positions[(int64_t)j * k_max + rnd] = idx;
-      if (tokens && rnd < nb) tokens[base + rnd] = idx;
+      if constexpr (WIDE) {
+        *cl.map_shared_rank(&gk[sl.rank() * k_need + rnd], 0) = wide_key(top, sl.rank());
+      } else {
+        const int64_t idx = (int64_t)(0xFFFFu - (top & 0xFFFFu));
+        if (positions) positions[(int64_t)j * k_max + rnd] = idx;
+        if (tokens && rnd < nb) tokens[base + rnd] = idx;
+      }
       best = 0u;
 #pragma unroll
       for (int e = 0; e < CH * 8; ++e) {
@@ -204,6 +344,10 @@ __global__ void __launch_bounds__(NT) sample_level_kernel(
         best = max(best, key[e]);
       }
     }
+  }
+  if constexpr (WIDE) {
+    cl.sync();
+    if (sl.rank() == 0) wide_topk_merge(gk, sl.n(), k_need, j, k_max, nb, base, positions, tokens);
   }
 }
 
@@ -293,9 +437,19 @@ __global__ void __launch_bounds__(NT) sample_replace_kernel(
 }
 
 // ---------------------------------------------------------------------------------------------
+template <bool WIDE>
 __global__ void __launch_bounds__(NT) residual_kernel(const __half* __restrict__ p, const __half* __restrict__ q,
                                                        __half* __restrict__ out, int V) {
   __shared__ float red[NW];
+  Slice sl{};
+  if constexpr (WIDE) {                  // grid = one cluster over the row
+    pdl_wait();
+    sl = slice_of(V);
+    p += sl.base;
+    q += sl.base;
+    out += sl.base;
+    V = sl.V;
+  }
   Pack8 a[CH], b[CH];
   load_row(p, V, a);
   load_row(q, V, b);
@@ -312,7 +466,13 @@ __global__ void __launch_bounds__(NT) residual_kernel(const __half* __restrict__
         s += d;
       }
     }
-  const float tot = rnd16(block_sum<NW>(s, red));                  // .sum() of an fp16 tensor -> fp16
+  float tot;
+  if constexpr (WIDE) {
+    __shared__ float xs[MAX_SLICES];
+    tot = rnd16(cl_sum(block_sum<NW>(s, red), xs, sl));
+  } else {
+    tot = rnd16(block_sum<NW>(s, red));                            // .sum() of an fp16 tensor -> fp16
+  }
 #pragma unroll
   for (int i = 0; i < CH; ++i) {
     const int c = i * NT + threadIdx.x;
@@ -326,11 +486,20 @@ __global__ void __launch_bounds__(NT) residual_kernel(const __half* __restrict__
 }
 
 // ---------------------------------------------------------------------------------------------
+template <bool WIDE>
 __global__ void __launch_bounds__(NT) argmax_rows_kernel(const __half* __restrict__ logits, int64_t ld, int V,
                                                           int64_t* __restrict__ out) {
   __shared__ uint32_t redu[NW];
+  Slice sl{};
   Pack8 x[CH];
-  load_row(logits + blockIdx.x * ld, V, x);
+  if constexpr (WIDE) {
+    pdl_wait();
+    sl = slice_of(V);
+    V = sl.V;
+    load_row(logits + sl.row * ld + sl.base, V, x);
+  } else {
+    load_row(logits + blockIdx.x * ld, V, x);
+  }
   const int nvec = V / 8;
   uint32_t best = 0u;
 #pragma unroll
@@ -342,7 +511,17 @@ __global__ void __launch_bounds__(NT) argmax_rows_kernel(const __half* __restric
     }
   }
   const uint32_t top = block_max_u32(best, redu);
-  if (threadIdx.x == 0) out[blockIdx.x] = (int64_t)(0xFFFFu - (top & 0xFFFFu));
+  if constexpr (WIDE) {                  // equal maxima in several slices: the lowest rank, i.e. the lowest index, wins
+    __shared__ uint64_t gk[MAX_SLICES];
+    cl_publish(wide_key(top, sl.rank()), gk, sl);
+    if (sl.rank() == 0 && threadIdx.x == 0) {
+      uint64_t m = 0ull;
+      for (int r = 0; r < sl.n(); ++r) m = max(m, gk[r]);
+      out[sl.row] = wide_index(m);
+    }
+  } else {
+    if (threadIdx.x == 0) out[blockIdx.x] = (int64_t)(0xFFFFu - (top & 0xFFFFu));
+  }
 }
 
 
@@ -359,6 +538,9 @@ __global__ void __launch_bounds__(NT) argmax_rows_kernel(const __half* __restric
 // below the fp16 rounding of the comparison.)
 __device__ __forceinline__ bool topp_pred(uint32_t S, float tp) { return h2f(f2h((float)S * (1.0f / 16777216.f))) > tp; }
 
+// WIDE: the histograms are summed over the cluster (every CTA then selects the same boundary bins, so all take the same
+// exits), and the boundary tie group is ranked across slices by an exclusive prefix of the per-slice counts in rank order.
+template <bool WIDE>
 __global__ void __launch_bounds__(NT) top_p_filter_kernel(__half* __restrict__ logits, int64_t ld, int V, float inv_T,
                                                            float tp) {
   __shared__ float red[NW];
@@ -366,13 +548,27 @@ __global__ void __launch_bounds__(NT) top_p_filter_kernel(__half* __restrict__ l
   __shared__ uint32_t hist[256];
   __shared__ int sel[2];            // boundary bin, mass ranked before it
   __shared__ uint32_t wtot[CH][NW];
-  __half* row = logits + blockIdx.x * ld;
+  Slice sl{};
+  __half* row;
+  if constexpr (WIDE) {
+    pdl_wait();
+    sl = slice_of(V);
+    row = logits + sl.row * ld + sl.base;
+    V = sl.V;
+  } else {
+    row = logits + blockIdx.x * ld;
+  }
   const int nvec = V / 8;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   Pack8 xt[CH];
   load_row(row, V, xt);
   float mx, sum;
-  scale_and_stats(xt, inv_T, red, mx, sum);
+  if constexpr (WIDE) {
+    __shared__ float xs[2][MAX_SLICES];
+    scale_and_stats_wide(xt, inv_T, red, xs, sl, mx, sum);
+  } else {
+    scale_and_stats(xt, inv_T, red, mx, sum);
+  }
   uint32_t before = 0u;             // mass ranked before the current boundary bin
   int hi = -1, key_b = -1;
   for (int level = 0; level < 2; ++level) {
@@ -387,11 +583,28 @@ __global__ void __launch_bounds__(NT) top_p_filter_kernel(__half* __restrict__ l
         if (w != 0u && (level == 0 || (int)(k >> 8) == hi)) atomicAdd(&whist[warp][level == 0 ? (k >> 8) : (k & 255u)], w);
       }
     __syncthreads();
-    if (threadIdx.x < 256) {
-      uint32_t t = 0u;
+    if constexpr (WIDE) {
+      __shared__ uint32_t ghist[2][MAX_SLICES][256];
+      cg::cluster_group cl = cg::this_cluster();
+      if (threadIdx.x < 256) {
+        uint32_t t = 0u;
 #pragma unroll 8
-      for (int w = 0; w < NW; ++w) t += whist[w][threadIdx.x];
-      hist[threadIdx.x] = t;
+        for (int w = 0; w < NW; ++w) t += whist[w][threadIdx.x];
+        for (int r = 0; r < sl.n(); ++r) *cl.map_shared_rank(&ghist[level][sl.rank()][threadIdx.x], r) = t;
+      }
+      cl.sync();
+      if (threadIdx.x < 256) {
+        uint32_t t = 0u;
+        for (int r = 0; r < sl.n(); ++r) t += ghist[level][r][threadIdx.x];
+        hist[threadIdx.x] = t;
+      }
+    } else {
+      if (threadIdx.x < 256) {
+        uint32_t t = 0u;
+#pragma unroll 8
+        for (int w = 0; w < NW; ++w) t += whist[w][threadIdx.x];
+        hist[threadIdx.x] = t;
+      }
     }
     if (threadIdx.x == 0) sel[0] = -1;
     __syncthreads();
@@ -462,6 +675,24 @@ __global__ void __launch_bounds__(NT) top_p_filter_kernel(__half* __restrict__ l
     excl[i] = total + (warp ? prev : 0) + inc[i] - cs[i];
     total += __shfl_sync(0xffffffffu, v, 31);
   }
+  if constexpr (WIDE) {             // tie members in lower slices rank first; w_b from a slice that holds the key
+    __shared__ uint32_t gcnt[MAX_SLICES], gw[MAX_SLICES];
+    cg::cluster_group cl = cg::this_cluster();
+    if ((int)threadIdx.x < sl.n()) {
+      *cl.map_shared_rank(&gcnt[sl.rank()], (int)threadIdx.x) = (uint32_t)total;
+      *cl.map_shared_rank(&gw[sl.rank()], (int)threadIdx.x) = w_b;
+    }
+    cl.sync();
+    int below = 0;
+    total = 0;
+    for (int r = 0; r < sl.n(); ++r) {
+      if (r < sl.rank()) below += (int)gcnt[r];
+      total += (int)gcnt[r];
+      w_b = max(w_b, gw[r]);
+    }
+#pragma unroll
+    for (int i = 0; i < CH; ++i) excl[i] += below;
+  }
   // smallest t with pred(before + t * w_b): tie ranks >= t are removed (pred(before) is false, pred at t = total true)
   int lo = 0, hi_t = total;
   while (lo < hi_t) {
@@ -500,7 +731,39 @@ using namespace sq;
 
 #define SQ_CHECK_V(V) \
   SQ_CHECK_ARG((V) % 8 == 0 && (V) > 0 && (V) <= NT * CH * 8, "V=%d must be a multiple of 8, <= 32768", (V))
+#define SQ_CHECK_V_WIDE(V)                                                                                         \
+  SQ_CHECK_ARG((V) % 8 == 0 && (V) > 0 && (V) <= SLICE * MAX_SLICES, "V=%d must be a multiple of 8, <= %d", (V), \
+               SLICE * MAX_SLICES)
 
+// V > SLICE: `rows` clusters of ceil(V / SLICE) CTAs along x (times grid_y)
+template <typename... KArgs, typename... Args>
+static cudaError_t launch_wide(void (*kern)(KArgs...), int rows, int grid_y, int V, cudaStream_t st, Args&&... args) {
+  const unsigned n = (unsigned)((V + SLICE - 1) / SLICE);
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(rows * n, grid_y);
+  cfg.blockDim = dim3(NT);
+  cfg.stream = st;
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeClusterDimension;
+  at[0].val.clusterDim.x = n;
+  at[0].val.clusterDim.y = 1;
+  at[0].val.clusterDim.z = 1;
+  cfg.attrs = at;
+  cfg.numAttrs = 1;
+  return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
+}
+
+#define SQ_CHECK_WIDE_LAUNCH(call, name)                                                   \
+  do {                                                                                     \
+    cudaError_t e_ = (call);                                                               \
+    if (e_ != cudaSuccess) {                                                               \
+      sq::set_error("%s: launch failed: %s", name, cudaGetErrorString(e_));                \
+      return SQ_ERR_CUDA;                                                                  \
+    }                                                                                      \
+    SQ_CHECK_LAUNCH(name);                                                                 \
+  } while (0)
+
+// (a test and tooling entry point; the decode path has no softmax_T launch, so it keeps the single-CTA bound)
 extern "C" int sq_softmax_T(const sq_half* logits, int64_t ld_in, sq_half* out, int64_t ld_out, int n, int V, float T,
                             void* stream) {
   SQ_CHECK_V(V);
@@ -514,12 +777,21 @@ extern "C" int sq_sample_level(const sq_half* logits, int64_t ld_logits, const s
                                const int32_t* parent_rows, const int32_t* child_first, const int32_t* n_branch,
                                int n_parents, int k_max, int V, float T, int mode, int64_t* positions, int64_t* tokens,
                                const int32_t* state, void* stream) {
-  SQ_CHECK_V(V);
+  SQ_CHECK_V_WIDE(V);
   if (n_parents == 0 || k_max == 0) return SQ_OK;
   SQ_CHECK_ARG(mode == 1 || rand != nullptr, "sq_sample_level: rand required for mode 0");
   SQ_CHECK_ARG(tokens == nullptr || (child_first && n_branch), "sq_sample_level: tokens needs child_first/n_branch");
   SQ_CHECK_ARG(k_max <= V, "sq_sample_level: k_max > V");
-  sample_level_kernel<false><<<n_parents, NT, 0, (cudaStream_t)stream>>>(
+  if (V > SLICE) {
+    SQ_CHECK_ARG(k_max <= WIDE_KMAX, "sq_sample_level: k_max=%d > %d with V > %d", k_max, WIDE_KMAX, SLICE);
+    SQ_CHECK_WIDE_LAUNCH(launch_wide(sample_level_kernel<false, true>, n_parents, 1, V, (cudaStream_t)stream,
+                                     (const __half*)logits, ld_logits, (const __half*)rand, ld_rand, parent_rows,
+                                     child_first, n_branch, k_max, V, 1.0f / T, mode, positions, tokens, state,
+                                     (const int32_t*)nullptr, (const int32_t*)nullptr, (int64_t)0, (int64_t)0),
+                         "sq_sample_level");
+    return SQ_OK;
+  }
+  sample_level_kernel<false, false><<<n_parents, NT, 0, (cudaStream_t)stream>>>(
       (const __half*)logits, ld_logits, (const __half*)rand, ld_rand, parent_rows, child_first, n_branch, k_max, V, 1.0f / T,
       mode, positions, tokens, state, nullptr, nullptr, 0, 0);
   SQ_CHECK_LAUNCH("sq_sample_level");
@@ -531,25 +803,37 @@ extern "C" int sq_sample_level_batch(const sq_half* logits, int64_t ld_logits, c
                                      const int32_t* parent_rows, const int32_t* child_first, const int32_t* n_branch,
                                      int n_parents, int k_max, int V, float T, int mode, int64_t* tokens, int64_t ld_seq,
                                      const int32_t* state, int B, void* stream) {
-  SQ_CHECK_V(V);
+  SQ_CHECK_V_WIDE(V);
   SQ_CHECK_ARG(B >= 1 && B <= SQ_MAX_BATCH, "sq_sample_level_batch: B=%d (1..%d)", B, SQ_MAX_BATCH);
   if (n_parents == 0 || k_max == 0) return SQ_OK;
   SQ_CHECK_ARG(mode == 1 || rand != nullptr, "sq_sample_level_batch: rand required for mode 0");
   SQ_CHECK_ARG(tokens && child_first && n_branch && parent_rows && state && row_base && row_step,
                "sq_sample_level_batch: null table or buffer");
   SQ_CHECK_ARG(k_max <= V, "sq_sample_level_batch: k_max > V");
-  sample_level_kernel<true><<<dim3(n_parents, B), NT, 0, (cudaStream_t)stream>>>(
+  if (V > SLICE) {
+    SQ_CHECK_ARG(k_max <= WIDE_KMAX, "sq_sample_level_batch: k_max=%d > %d with V > %d", k_max, WIDE_KMAX, SLICE);
+    SQ_CHECK_WIDE_LAUNCH(launch_wide(sample_level_kernel<true, true>, n_parents, B, V, (cudaStream_t)stream,
+                                     (const __half*)logits, ld_logits, (const __half*)rand, ld_rand, parent_rows,
+                                     child_first, n_branch, k_max, V, 1.0f / T, mode, (int64_t*)nullptr, tokens, state,
+                                     row_base, row_step, ld_rand_seq, ld_seq),
+                         "sq_sample_level_batch");
+    return SQ_OK;
+  }
+  sample_level_kernel<true, false><<<dim3(n_parents, B), NT, 0, (cudaStream_t)stream>>>(
       (const __half*)logits, ld_logits, (const __half*)rand, ld_rand, parent_rows, child_first, n_branch, k_max, V, 1.0f / T,
       mode, nullptr, tokens, state, row_base, row_step, ld_rand_seq, ld_seq);
   SQ_CHECK_LAUNCH("sq_sample_level_batch");
   return SQ_OK;
 }
 
+// Sampling with replacement (the SpecInfer policy) has no large-vocabulary instance: V <= 32768 only.
 extern "C" int sq_sample_replace(const sq_half* logits, int64_t ld_logits, const int64_t* words,
                                  const int32_t* parent_rows, const int32_t* child_first, const int32_t* n_branch,
                                  int n_parents, int k_max, int V, float T, int64_t* positions, int64_t* tokens,
                                  const int32_t* state, void* stream) {
-  SQ_CHECK_V(V);
+  SQ_CHECK_ARG(V % 8 == 0 && V > 0 && V <= SLICE,
+               "sq_sample_replace: V=%d must be a multiple of 8, <= 32768 (sampling with replacement has no "
+               "large-vocabulary kernel)", V);
   if (n_parents == 0 || k_max == 0) return SQ_OK;
   SQ_CHECK_ARG(words != nullptr, "sq_sample_replace: words required");
   SQ_CHECK_ARG(tokens == nullptr || (child_first && n_branch), "sq_sample_replace: tokens needs child_first/n_branch");
@@ -562,25 +846,40 @@ extern "C" int sq_sample_replace(const sq_half* logits, int64_t ld_logits, const
 }
 
 extern "C" int sq_residual(const sq_half* p, const sq_half* q, sq_half* out, int V, void* stream) {
-  SQ_CHECK_V(V);
-  residual_kernel<<<1, NT, 0, (cudaStream_t)stream>>>((const __half*)p, (const __half*)q, (__half*)out, V);
+  SQ_CHECK_V_WIDE(V);
+  if (V > SLICE) {
+    SQ_CHECK_WIDE_LAUNCH(launch_wide(residual_kernel<true>, 1, 1, V, (cudaStream_t)stream, (const __half*)p,
+                                     (const __half*)q, (__half*)out, V), "sq_residual");
+    return SQ_OK;
+  }
+  residual_kernel<false><<<1, NT, 0, (cudaStream_t)stream>>>((const __half*)p, (const __half*)q, (__half*)out, V);
   SQ_CHECK_LAUNCH("sq_residual");
   return SQ_OK;
 }
 
 extern "C" int sq_argmax_rows(const sq_half* logits, int64_t ld, int n, int V, int64_t* out, void* stream) {
-  SQ_CHECK_V(V);
+  SQ_CHECK_V_WIDE(V);
   if (n == 0) return SQ_OK;
-  argmax_rows_kernel<<<n, NT, 0, (cudaStream_t)stream>>>((const __half*)logits, ld, V, out);
+  if (V > SLICE) {
+    SQ_CHECK_WIDE_LAUNCH(launch_wide(argmax_rows_kernel<true>, n, 1, V, (cudaStream_t)stream, (const __half*)logits, ld, V,
+                                     out), "sq_argmax_rows");
+    return SQ_OK;
+  }
+  argmax_rows_kernel<false><<<n, NT, 0, (cudaStream_t)stream>>>((const __half*)logits, ld, V, out);
   SQ_CHECK_LAUNCH("sq_argmax_rows");
   return SQ_OK;
 }
 
 extern "C" int sq_top_p_filter(sq_half* logits, int64_t ld, int n, int V, float top_p, float T, void* stream) {
-  SQ_CHECK_V(V);
+  SQ_CHECK_V_WIDE(V);
   if (n == 0 || top_p >= 1.0f) return SQ_OK;                       // utils.py:68: only when top_p < 1
   const float tp = __half2float(__float2half_rn(top_p));           // torch compares in the tensor's dtype (fp16)
-  top_p_filter_kernel<<<n, NT, 0, (cudaStream_t)stream>>>((__half*)logits, ld, V, 1.0f / T, tp);
+  if (V > SLICE) {
+    SQ_CHECK_WIDE_LAUNCH(launch_wide(top_p_filter_kernel<true>, n, 1, V, (cudaStream_t)stream, (__half*)logits, ld, V,
+                                     1.0f / T, tp), "sq_top_p_filter");
+    return SQ_OK;
+  }
+  top_p_filter_kernel<false><<<n, NT, 0, (cudaStream_t)stream>>>((__half*)logits, ld, V, 1.0f / T, tp);
   SQ_CHECK_LAUNCH("sq_top_p_filter");
   return SQ_OK;
 }

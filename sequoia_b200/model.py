@@ -38,6 +38,7 @@ class LlamaConfigLite:
     rms_norm_eps: float = 1e-6
     rope_theta: float = 10000.0
     max_position_embeddings: int = 2048
+    rope_scaling: Optional[dict] = None    # None, or parse_rope_scaling()'s llama3 dict
 
     @property
     def head_dim(self):
@@ -54,20 +55,60 @@ NAMED_CONFIGS = {
     # the first 8 layers' worth of a 70B-shaped model: TP parity checks at the real head / FFN shapes where the
     # unsharded 138 GB model cannot sit next to a shard (bench.py tp_parity, tests/test_gpu_tp.py)
     "llama-2-70b-8l": LlamaConfigLite(8192, 28672, 8, 64, 8, rms_norm_eps=1e-5, max_position_embeddings=4096),
+    # Llama 3 draft / target pair (128256-token vocabulary, llama3 RoPE scaling)
+    "llama-3.2-1b": LlamaConfigLite(2048, 8192, 16, 32, 8, vocab_size=128256, rms_norm_eps=1e-5, rope_theta=500000.0,
+                                    max_position_embeddings=131072,
+                                    rope_scaling=dict(rope_type="llama3", factor=32.0, low_freq_factor=1.0,
+                                                      high_freq_factor=4.0, original_max_position_embeddings=8192)),
+    "llama-3.1-8b": LlamaConfigLite(4096, 14336, 32, 32, 8, vocab_size=128256, rms_norm_eps=1e-5, rope_theta=500000.0,
+                                    max_position_embeddings=131072,
+                                    rope_scaling=dict(rope_type="llama3", factor=8.0, low_freq_factor=1.0,
+                                                      high_freq_factor=4.0, original_max_position_embeddings=8192)),
 }
+
+
+def parse_rope_scaling(rs) -> Optional[dict]:
+    """config.json's `rope_scaling` -> None (no scaling) or the llama3 parameters.  Any other type raises: decoding with
+    unscaled frequencies would silently give wrong results."""
+    if rs is None:
+        return None
+    kind = rs.get("rope_type", rs.get("type"))
+    if kind in (None, "default"):          # transformers >= 5 writes {"rope_type": "default", "rope_theta": ...}
+        return None
+    if kind != "llama3":
+        raise ValueError(f"rope_scaling type {kind!r} is not supported (supported: None, 'llama3')")
+    return dict(rope_type="llama3", factor=float(rs["factor"]), low_freq_factor=float(rs["low_freq_factor"]),
+                high_freq_factor=float(rs["high_freq_factor"]),
+                original_max_position_embeddings=int(rs["original_max_position_embeddings"]))
+
+
+def llama3_inv_freq(inv_freq: torch.Tensor, rs: dict) -> torch.Tensor:
+    """The Llama 3 inverse-frequency transform: wavelengths longer than original_max / low_freq_factor are divided by
+    `factor`, shorter than original_max / high_freq_factor kept, and the band between interpolated smoothly."""
+    factor, lo, hi = rs["factor"], rs["low_freq_factor"], rs["high_freq_factor"]
+    old = rs["original_max_position_embeddings"]
+    wavelen = 2 * math.pi / inv_freq
+    out = torch.where(wavelen > old / lo, inv_freq / factor, inv_freq)
+    smooth = (old / wavelen - lo) / (hi - lo)
+    smoothed = (1 - smooth) * out / factor + smooth * out
+    medium = ~(wavelen < old / hi) & ~(wavelen > old / lo)
+    return torch.where(medium, smoothed, out)
 
 
 def config_from(obj) -> LlamaConfigLite:
     if isinstance(obj, LlamaConfigLite):
         return obj
     g = (lambda k, d=None: obj.get(k, d)) if isinstance(obj, dict) else (lambda k, d=None: getattr(obj, k, d))
-    theta = g("rope_theta", None)
+    # transformers >= 5 keeps theta and the scaling under `rope_parameters`; older configs use the two top-level keys
+    rp = g("rope_parameters", None) or {}
+    theta = g("rope_theta", None) or rp.get("rope_theta")
+    rs = g("rope_scaling", None) or (rp or None)
     return LlamaConfigLite(
         hidden_size=g("hidden_size"), intermediate_size=g("intermediate_size"),
         num_hidden_layers=g("num_hidden_layers"), num_attention_heads=g("num_attention_heads"),
         num_key_value_heads=g("num_key_value_heads") or g("num_attention_heads"), vocab_size=g("vocab_size", 32000),
         rms_norm_eps=g("rms_norm_eps", 1e-6), rope_theta=float(theta) if theta else 10000.0,
-        max_position_embeddings=g("max_position_embeddings", 2048))
+        max_position_embeddings=g("max_position_embeddings", 2048), rope_scaling=parse_rope_scaling(rs))
 
 
 def _load_state_dict_dir(path: str) -> Dict[str, torch.Tensor]:
@@ -143,6 +184,8 @@ def rope_cache(cfg: LlamaConfigLite, max_length: int, device):
     """LlamaRotaryEmbedding_FI (Engine/Llama_modules.py:16-45): fp32 tables, sliced [:max_length], cast to fp16."""
     d = cfg.head_dim
     inv_freq = 1.0 / (cfg.rope_theta ** (torch.arange(0, d, 2, dtype=torch.float32) / d))
+    if cfg.rope_scaling is not None:
+        inv_freq = llama3_inv_freq(inv_freq, parse_rope_scaling(cfg.rope_scaling))
     # the reference builds max_position_embeddings rows and slices [:max_length]; rows beyond that table would be an
     # out-of-bounds read in the RoPE kernel, so the table always covers max_length (identical values where both exist)
     t = torch.arange(max(cfg.max_position_embeddings, max_length), dtype=torch.float32)

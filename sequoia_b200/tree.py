@@ -13,6 +13,7 @@ own n=1 algorithm (SpecTree.py:222).
 """
 from __future__ import annotations
 
+import os
 import time
 from typing import Dict, List, Optional
 
@@ -298,6 +299,24 @@ class _Runtime:
 _RUNTIMES: Dict[tuple, _Runtime] = {}
 
 
+SMALL_VOCAB = 32768       # largest vocabulary of the single-CTA kernels (sampling with replacement, SQ_ACCEPT_IMPL=0)
+MAX_VOCAB = 131072        # largest vocabulary of the cluster kernels (the default decode path)
+
+
+def check_vocab(policy: str, V: int):
+    """Refuse, before any buffer is allocated, a vocabulary the policy's kernels cannot take."""
+    if V > MAX_VOCAB or V % 8:
+        raise ValueError(f"vocabulary {V}: the kernels take multiples of 8 up to {MAX_VOCAB}")
+    if V <= SMALL_VOCAB:
+        return
+    if policy == "specinfer":
+        raise ValueError(f"SpecInferTree supports vocabularies up to {SMALL_VOCAB} (sampling with replacement has no "
+                         f"large-vocabulary kernel); this model has {V}")
+    if policy in ("spec", "spec_test", "specinfer") and os.environ.get("SQ_ACCEPT_IMPL", "1") == "0":
+        raise ValueError(f"SQ_ACCEPT_IMPL=0 (the single-CTA verification walk) supports vocabularies up to {SMALL_VOCAB}; "
+                         f"this model has {V}")
+
+
 def get_runtime(draft, target, grow_map, policy, T, top_p, M, max_target_seq, V, device) -> _Runtime:
     key = (id(draft), id(target), id(grow_map), policy, float(T), float(top_p), M, max_target_seq, V)
     rt = _RUNTIMES.get(key)
@@ -334,12 +353,17 @@ class _TreeBase(Tree):
         self.sampling_callables = sampling_callables
         self.sample_gather_indices = sample_gather_indices
         self.grow_map = grow_map
+        # the buffers are sized by the engines' vocabulary (`vocab_size` is the reference's signature; 32000 = not given)
+        V = draft_model_engine.engine.model_config.vocab_size
+        if vocab_size not in (32000, V):
+            raise ValueError(f"vocab_size={vocab_size} does not match the engines' vocabulary ({V})")
+        check_vocab(self.POLICY, V)
         self.draft_step = len(grow_map["roots"])
         self.Successors = grow_map["Successors"]
         self.tree_size = grow_map["size"]
         self.initialize(attn_mask, sequence, new_tokens_buffer, parents_buffer, position_ids, None)
         rt = get_runtime(draft_model_engine, target_model_engine, grow_map, self.POLICY, temperature, top_p,
-                         max_length, max_target_seq, vocab_size, device)
+                         max_length, max_target_seq, V, device)
         self.rt = rt
         S, M = self.tree_size, max_length
         P = len(prefix)

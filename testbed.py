@@ -82,8 +82,25 @@ def _tree_class(name: str):
     return cls
 
 
+def stop_tokens(model_name_or_path) -> frozenset:
+    """Token ids that end a generation: `eos_token_id` (an int or a list) of the model directory's config.json when it has
+    one, else 2 and 0 (the Llama-2 eos and pad ids, what the reference stops on)."""
+    path = os.path.join(str(model_name_or_path), "config.json")
+    if os.path.isfile(path):
+        with open(path) as f:
+            eos = json.load(f).get("eos_token_id")
+        if isinstance(eos, int):
+            return frozenset([eos])
+        if isinstance(eos, (list, tuple)) and eos:
+            return frozenset(int(t) for t in eos)
+    return DEFAULT_STOP
+
+
+DEFAULT_STOP = frozenset([0, 2])
+
+
 @torch.inference_mode()
-def simulation(target, draft, prompts, grow_map, tree_cls, T, top_p, M, benchmark: bool):
+def simulation(target, draft, prompts, grow_map, tree_cls, T, top_p, M, benchmark: bool, stop=DEFAULT_STOP):
     """simulation_fast / simulation_benchmark."""
     bufs = _buffers(M)
     steps = decoded = 0
@@ -114,10 +131,10 @@ def simulation(target, draft, prompts, grow_map, tree_cls, T, top_p, M, benchmar
                 valid, _, _, terminate = tree.verify()
             input_ids = valid.unsqueeze(0)
             last = int(input_ids[0, -1])
-            if last == 2 or last == 0:
+            if last in stop:
                 terminate = True
             if benchmark:
-                if bool(((input_ids[0] == 2) | (input_ids[0] == 0)).any()) or input_ids.shape[1] >= MAX_NEW_LEN:
+                if any(int(t) in stop for t in input_ids[0].tolist()) or input_ids.shape[1] >= MAX_NEW_LEN:
                     terminate = True
                 if terminate:                          # the reference drops the last step from the phase averages
                     continue
@@ -143,7 +160,7 @@ def simulation(target, draft, prompts, grow_map, tree_cls, T, top_p, M, benchmar
 
 
 @torch.inference_mode()          # engine outputs are inference tensors; the nucleus filter edits them in place
-def simulation_baseline(target, prompts, T, top_p, M, new_tokens: int = 32):
+def simulation_baseline(target, prompts, T, top_p, M, new_tokens: int = 32, stop=DEFAULT_STOP):
     """Autoregressive sampling from the target alone (tests/testbed.py:98-137)."""
     from utils import _make_causal_mask, get_sampling_logits
     position_ids = torch.arange(M, device=DEV).unsqueeze(0)
@@ -162,7 +179,7 @@ def simulation_baseline(target, prompts, T, top_p, M, new_tokens: int = 32):
             logits = get_sampling_logits(logits=logits, top_p=top_p, T=T)
             ids = torch.softmax(logits / T, dim=-1).multinomial(num_samples=1).unsqueeze(0)
             decoded += 1
-            if int(ids[0, -1]) == 2:
+            if int(ids[0, -1]) in stop - {0}:      # (the baseline loop only ever stopped on eos)
                 break
         torch.cuda.synchronize()
         total_time += time.time() - t1
@@ -172,7 +189,7 @@ def simulation_baseline(target, prompts, T, top_p, M, new_tokens: int = 32):
 
 
 @torch.inference_mode()
-def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: int):
+def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: int, stop=DEFAULT_STOP):
     """--batch B: the same metric loop with B prompts decoded together (sequoia_b200.batch.BatchTree)."""
     from sequoia_b200.batch import BatchTree
     steps = decoded = 0                          # steps: target steps summed over sequences (per-sequence tokens / step)
@@ -194,7 +211,7 @@ def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: i
                 steps += 1
                 length[b] = valid.shape[0]
                 last = int(valid[-1]) if valid.shape[0] else 0
-                if terminate or last in (0, 2) or length[b] >= MAX_NEW_LEN:
+                if terminate or last in stop or length[b] >= MAX_NEW_LEN:
                     done.add(b)
                     if not tree.frozen[b]:
                         tree.freeze(b)
@@ -238,6 +255,7 @@ def main(argv=None):
     from Engine.offload_engine import OffloadEngine
     prompts = load_prompts(args.dataset, args.start, args.end, args.seed)
     tcls = OffloadEngine if args.offloading else GraphInferenceEngineTG
+    stop = stop_tokens(args.target)
     if args.batch != 1:
         if args.Mode != "greedy" or args.tree not in ("spec", "greedy") or args.offloading:
             raise SystemExit("--batch runs --Mode greedy with --tree spec or greedy, without --offloading")
@@ -250,19 +268,20 @@ def main(argv=None):
         path = args.growmap if os.path.isabs(args.growmap) or os.path.exists(args.growmap) else os.path.join(ROOT, args.growmap)
         grow_map = torch.load(path)
         assert args.M >= MAX_NEW_LEN + grow_map["size"], "--M must hold 256 tokens + the tree (README.md:47 of the reference)"
-        res = simulation_batch(target, draft, prompts, grow_map, args.tree, args.T, args.P, args.M, args.batch)
+        res = simulation_batch(target, draft, prompts, grow_map, args.tree, args.T, args.P, args.M, args.batch,
+                               stop=stop)
         print(json.dumps({k: (round(v, 5) if isinstance(v, float) else v) for k, v in res.items()}))
         return res
     target = tcls(max_length=args.M, model_name_or_path=args.target, dtype=torch.float16, device=DEV)
     if args.Mode == "baseline":
-        res = simulation_baseline(target, prompts, args.T, args.P, args.M)
+        res = simulation_baseline(target, prompts, args.T, args.P, args.M, stop=stop)
     else:
         draft = GraphInferenceEngine(max_length=args.M, model_name_or_path=args.model, dtype=torch.float16, device=DEV)
         path = args.growmap if os.path.isabs(args.growmap) or os.path.exists(args.growmap) else os.path.join(ROOT, args.growmap)
         grow_map = torch.load(path)
         assert args.M >= MAX_NEW_LEN + grow_map["size"], "--M must hold 256 tokens + the tree (README.md:47 of the reference)"
         res = simulation(target, draft, prompts, grow_map, _tree_class(args.tree), args.T, args.P, args.M,
-                         benchmark=(args.Mode == "benchmark"))
+                         benchmark=(args.Mode == "benchmark"), stop=stop)
     print(json.dumps({k: (round(v, 5) if isinstance(v, float) else v) for k, v in res.items()}))
     return res
 
