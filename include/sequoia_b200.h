@@ -226,6 +226,27 @@ int sq_gemm_run(sq_gemm_plan* plan, int n, void* stream);
  * own output buffer, rows [a_row0, a_row0 + n). */
 int sq_gemm_run_at(sq_gemm_plan* plan, int n, int a_row0, sq_half* c, int ldc, void* stream);
 
+/* ---- FP8 (E4M3) weight-streaming GEMM: the target's layer projections on quantized weights (csrc/sq_gemm_fp8.cu) ---- */
+
+/* C[n, N] = A[n, K] * W'[N, K]^T with W'[j, k] = fp16(fp16(q[j, k]) * w_scale[j]): q e4m3 (one byte per weight), one fp16
+ * scale per output channel; fp16 activations, fp32 accumulation, fp16 out.  q is stored pre-tiled by
+ * sq_gemm_fp8_tile_weights (its only producer).  N % 64 == 0, K % 64 == 0, lda and ldc multiples of 8.  err_flag: optional
+ * device word set by the pipeline watchdog.  n > 128 runs one launch per 128-row tile.  SQ_GEMM_FP8_FORCE="nwg,split"
+ * (nwg 2 or 3 weight tiles of 64 rows per CTA, split 1-4 K splits over a cluster), read at plan creation, forces the
+ * instance; sq_gemm_fp8_plan_info reports the one chosen (stages: ring depth of the 128-row instance). */
+typedef struct sq_gemm_fp8_plan sq_gemm_fp8_plan;
+/* (N, K) row-major e4m3 q -> the kernel's pre-tiled copy (N * K bytes): block (t, kb) of 4096 bytes per 64-row tile t
+ * and 64-wide K block kb, at (t * K/64 + kb) * 4096; byte h * 2048 + u * 16 + 8 (k % 2) + 2 r + e (h = k / 2) of a
+ * block holds register r, half e of the wgmma m64k16 A fragment of k16 step k of consumer thread u (0-127). */
+int sq_gemm_fp8_tile_weights(const uint8_t* q, uint8_t* q_tiled, int N, int K, void* stream);
+int sq_gemm_fp8_plan_create(sq_gemm_fp8_plan** plan, const sq_half* a, int lda, int n_max, const uint8_t* w_q,
+                            const sq_half* w_scale, int N, int K, sq_half* c, int ldc, int* err_flag);
+int sq_gemm_fp8_plan_info(sq_gemm_fp8_plan* plan, int* nwg, int* split, int* stages);
+int sq_gemm_fp8_plan_destroy(sq_gemm_fp8_plan* plan);
+/* Rows [a_row0, a_row0 + n) of the plan's activation buffer -> rows [0, n) of `c` (pitch ldc halfs); c == NULL: the plan's
+ * own output buffer, rows [a_row0, a_row0 + n). */
+int sq_gemm_fp8_run_at(sq_gemm_fp8_plan* plan, int n, int a_row0, sq_half* c, int ldc, void* stream);
+
 /* ---- target tensor parallelism: fused one-shot all-reduce over NVLink peer memory (no reference counterpart) ---- */
 
 /* Peer-mappable device buffers (cudaMalloc + CUDA IPC).  handle64: 64-byte cudaIpcMemHandle_t. */

@@ -56,6 +56,11 @@ _SIGNATURES = {
     "sq_gemm_plan_info": (i32, [vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32)]),
     "sq_gemm_run": (i32, [vp, i32, vp]),
     "sq_gemm_run_at": (i32, [vp, i32, i32, vp, i32, vp]),
+    "sq_gemm_fp8_tile_weights": (i32, [vp, vp, i32, i32, vp]),
+    "sq_gemm_fp8_plan_create": (i32, [C.POINTER(vp), vp, i32, i32, vp, vp, i32, i32, vp, i32, vp]),
+    "sq_gemm_fp8_plan_info": (i32, [vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32)]),
+    "sq_gemm_fp8_plan_destroy": (i32, [vp]),
+    "sq_gemm_fp8_run_at": (i32, [vp, i32, i32, vp, i32, vp]),
     "sq_tp_alloc": (i32, [C.POINTER(vp), i64]),
     "sq_tp_free": (i32, [vp]),
     "sq_tp_ipc_export": (i32, [vp, vp]),

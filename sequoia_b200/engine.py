@@ -47,7 +47,7 @@ class InferenceEngine:
     _TG = False
 
     def __init__(self, max_length: int, model_name_or_path, dtype=torch.float16, device="cuda:0", tp_group=None,
-                 batch_size: int = 1):
+                 batch_size: int = 1, weight_format: str = "fp16"):
         _check_batch(batch_size, tp_group)
         if dtype != torch.float16:
             raise NotImplementedError("sequoia_b200 engines are fp16 (reference default)")
@@ -55,7 +55,8 @@ class InferenceEngine:
         self.dtype = dtype
         self.max_length = max_length
         self.batch_size = batch_size
-        self.runner = LlamaRunner(model_name_or_path, max_length, device=device, tp_group=tp_group, batch_size=batch_size)
+        self.runner = LlamaRunner(model_name_or_path, max_length, device=device, tp_group=tp_group, batch_size=batch_size,
+                                  weight_format=weight_format)
         self.model = self.runner                      # reference attribute name
         self.model_config = self.runner.cfg
         self.kv_cache = KV_Cache(config=self.model_config, batch_size=batch_size, max_length=max_length, device=device,
@@ -114,9 +115,9 @@ class InferenceEngineTG(InferenceEngine):
     _TG = True
 
     def __init__(self, max_length: int, model_name_or_path, dtype=torch.float16, device="cuda:0", offloading=False,
-                 tp_group=None, batch_size: int = 1):
+                 tp_group=None, batch_size: int = 1, weight_format: str = "fp16"):
         super().__init__(max_length, model_name_or_path, dtype=dtype, device=device, tp_group=tp_group,
-                         batch_size=batch_size)
+                         batch_size=batch_size, weight_format=weight_format)
         self.offloading = offloading
 
     def set_kv_len(self, kv_len: int):
@@ -159,13 +160,13 @@ class GraphInferenceEngine:
     """Engine/Engine.py:168-244."""
 
     def __init__(self, max_length: int, model_name_or_path, dtype=torch.float16, device="cuda:0", tp_group=None,
-                 batch_size: int = 1):
+                 batch_size: int = 1, weight_format: str = "fp16"):
         _check_batch(batch_size, tp_group)
         self.device = device
         self.dtype = dtype
         self.max_length = max_length
         self.engine = InferenceEngine(max_length=max_length, model_name_or_path=model_name_or_path, dtype=dtype,
-                                      device=device, tp_group=tp_group, batch_size=batch_size)
+                                      device=device, tp_group=tp_group, batch_size=batch_size, weight_format=weight_format)
         self.callables = {}
         self.mempool = None
 
@@ -218,13 +219,14 @@ class GraphInferenceEngineTG:
     """Engine/Engine.py:247-289."""
 
     def __init__(self, max_length: int, model_name_or_path, dtype=torch.float16, device="cuda:0", offloading=False,
-                 tp_group=None, batch_size: int = 1):
+                 tp_group=None, batch_size: int = 1, weight_format: str = "fp16"):
         _check_batch(batch_size, tp_group)
         self.device = device
         self.dtype = dtype
         self.max_length = max_length
         self.engine = InferenceEngineTG(max_length=max_length, model_name_or_path=model_name_or_path, dtype=dtype,
-                                        device=device, offloading=offloading, tp_group=tp_group, batch_size=batch_size)
+                                        device=device, offloading=offloading, tp_group=tp_group, batch_size=batch_size,
+                                        weight_format=weight_format)
 
     def clear_kv(self):
         drv = getattr(self, "_tp_driver", None)

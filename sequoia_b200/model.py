@@ -259,8 +259,17 @@ def load_sharded_weights(cfg: LlamaConfigLite, src, rank: int, tp: int) -> dict:
 class LlamaRunner:
     """Weights + preallocated activations + attention plan of one engine."""
 
+    PROJECTIONS = ("wqkv", "wo", "wgu", "wd")
+
     def __init__(self, model_name_or_path, max_length: int, device="cuda:0", tp_group=None, n_max: Optional[int] = None,
-                 batch_size: int = 1):
+                 batch_size: int = 1, weight_format: str = "fp16"):
+        """weight_format "fp8": the four layer projections are quantized to E4M3 with one fp16 scale per output channel
+        at load (ops.quantize_fp8) and run on the FP8 GEMM at every row count; embedding, norms and lm_head stay fp16."""
+        if weight_format not in ("fp16", "fp8"):
+            raise ValueError(f"weight_format must be 'fp16' or 'fp8', got {weight_format!r}")
+        if weight_format == "fp8" and tp_group is not None:
+            raise NotImplementedError("FP8 target weights run on one GPU: tensor parallelism needs weight_format='fp16'")
+        self.weight_format = weight_format
         self.device = torch.device(device)
         self.B = batch_size
         self.cfg, src = resolve_model(model_name_or_path, self.device)
@@ -274,6 +283,10 @@ class LlamaRunner:
         self.I = cfg.intermediate_size // tp
         h, D, V = cfg.hidden_size, self.D, cfg.vocab_size
         self.h, self.V, self.L = h, V, cfg.num_hidden_layers
+        if weight_format == "fp8":
+            shapes = (((self.H + 2 * self.Hkv) * D, h), (h, self.H * D), (2 * self.I, h), (h, self.I))
+            if any(n % 64 or k % 64 for n, k in shapes):
+                raise ValueError(f"weight_format='fp8' needs every layer projection (N, K) to be multiples of 64, got {shapes}")
         wts = load_sharded_weights(cfg, src, r, tp)
         self.embed, self.layers, self.norm, self.lm_head = wts["embed"], wts["layers"], wts["norm"], wts["lm_head"]
         self.cos, self.sin = rope_cache(cfg, max_length, self.device)
@@ -295,6 +308,16 @@ class LlamaRunner:
         # down_proj stay on cuBLASLt (torch.mm), which is faster at those shapes.
         self.gemm_err = torch.zeros(4, dtype=torch.int32, device=dev)
         self.lm_plan = None
+        if weight_format == "fp8":
+            # each fp16 projection is dropped as soon as its plan holds the quantized, pre-tiled copy
+            io = dict(wqkv=(self.normed, self.qkv), wo=(self.attn_out, self.proj), wgu=(self.normed, self.gate_up),
+                      wd=(self.act, self.proj))
+            for ly in self.layers:
+                for k in self.PROJECTIONS:
+                    q, s = ops.quantize_fp8(ly.pop(k))
+                    ly[k + "_fp8"] = ops.GemmFp8Plan(io[k][0], q, s, io[k][1], self.gemm_err)
+                    del q
+            torch.cuda.empty_cache()
         stream_sized = h >= 2048
         # (a fused-epilogue plan cannot split K, so a narrow shard -- TP-4/8 of a 7B -- would leave most SMs idle: those
         # stay on cuBLASLt + sq_silu_mul).  The plans serve forwards of <= 128 rows; larger ones (prefill, the 768-row verify
@@ -303,7 +326,7 @@ class LlamaRunner:
         gu_bn, gu_split, _ = ops.gemm_pick_tiles(2 * self.I, h, ops.GEMM_SWIGLU) if self.I % 16 == 0 and h % 64 == 0 else (0, 1, 1)
         gu_ctas = (-(-2 * self.I // gu_bn)) * gu_split if gu_bn else 0
         self.gu_interleaved = False
-        if stream_sized and gu_ctas >= 120:
+        if stream_sized and gu_ctas >= 120 and weight_format == "fp16":
             self.gu_interleaved = True
             for ly in self.layers:
                 ly["wgu"] = ops.interleave_gate_up(ly["wgu"][:self.I], ly["wgu"][self.I:])
@@ -329,14 +352,24 @@ class LlamaRunner:
         if plan is not None and 96 < n <= 128:
             plan.run(n)
             return
-        torch.mm(self.normed[:n], ly["wgu"].t(), out=self.gate_up[:n])
+        self._project(ly, "wgu", self.normed, n, self.gate_up)
         ops.silu_mul(self.gate_up, self.act, n, interleaved=self.gu_interleaved)
 
+    def _project(self, ly, k: str, a: torch.Tensor, n: int, out: torch.Tensor):
+        """out[:n] = a[:n] @ W_k.T: torch.mm on an fp16 weight, the FP8 plan (bound to a / out) on a quantized one"""
+        plan = ly.get(k + "_fp8")
+        if plan is not None:
+            plan.run(n)
+        else:
+            torch.mm(a[:n], ly[k].t(), out=out[:n])
+
     def weight_bytes(self) -> int:
-        b = self.embed.numel() + self.lm_head.numel() + self.norm.numel()
+        """bytes of the weights resident on the device (an FP8 projection: its e4m3 bytes and fp16 scales)"""
+        b = 2 * (self.embed.numel() + self.lm_head.numel() + self.norm.numel())
         for ly in self.layers:
-            b += sum(ly[k].numel() for k in ("wqkv", "wo", "wgu", "wd", "ln1", "ln2"))
-        return 2 * b
+            b += 2 * (ly["ln1"].numel() + ly["ln2"].numel())
+            b += sum(ly[k + "_fp8"].weight_bytes() if k + "_fp8" in ly else 2 * ly[k].numel() for k in self.PROJECTIONS)
+        return b
 
     @torch.no_grad()
     def forward(self, n: int, tokens: torch.Tensor, position_ids: torch.Tensor, storage_ids: torch.Tensor, *,
@@ -365,7 +398,7 @@ class LlamaRunner:
         n_seq, n = n, N                                # from here on n counts the rows of all sequences
         ops.rmsnorm(self.hidden, self.layers[0]["ln1"], self.normed, n, self.eps)
         for l, ly in enumerate(self.layers):
-            torch.mm(self.normed[:n], ly["wqkv"].t(), out=self.qkv[:n])
+            self._project(ly, "wqkv", self.normed, n, self.qkv)
             if batch:
                 ops.rope_kv_append_batch(self.qkv, H, Hkv, D, self.cos, self.sin, position_ids, storage_ids, n_seq,
                                          self.k_cache[l], self.v_cache[l], M, state, n0=n0)
@@ -389,11 +422,11 @@ class LlamaRunner:
                 torch.mm(self.act[:n], ly["wd"].t(), out=self.peer.buf[1][:n])
                 self.peer.allreduce_add_rmsnorm(1, self.hidden, nxt, self.normed, n, self.eps)
                 continue
-            torch.mm(self.attn_out[:n], ly["wo"].t(), out=self.proj[:n])
+            self._project(ly, "wo", self.attn_out, n, self.proj)
             self.tp.all_reduce(self.proj[:n])
             ops.add_rmsnorm(self.hidden, self.proj, ly["ln2"], self.normed, n, self.eps)
             self._gate_up_act(ly, n)
-            torch.mm(self.act[:n], ly["wd"].t(), out=self.proj[:n])
+            self._project(ly, "wd", self.act, n, self.proj)
             self.tp.all_reduce(self.proj[:n])
             ops.add_rmsnorm(self.hidden, self.proj, nxt, self.normed, n, self.eps)
         if skip_lm_head:                               # TP follower ranks: only rank 0 consumes logits

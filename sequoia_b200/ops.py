@@ -261,6 +261,91 @@ class GemmPlan:
             pass
 
 
+# ---- FP8 (E4M3) weights (csrc/sq_gemm_fp8.cu) --------------------------------------------------------------------------------
+FP8_MAX = 448.0                          # largest finite e4m3 magnitude
+F8 = torch.float8_e4m3fn
+
+
+def quantize_fp8(w: torch.Tensor, rows_per_chunk: int = 4096):
+    """(N, K) fp16 weight -> (q (N, K) float8_e4m3fn, s (N) fp16), on w's device:
+    s[j] = fp16(max|W[j,:]| / 448) (1 for an all-zero row, the smallest positive fp16 where that rounds to 0) and
+    q = e4m3(clamp(W / s, -448, 448)), rounded to nearest even.  Works through `rows_per_chunk` rows at a time, so the
+    fp32 temporaries stay small next to the weight."""
+    if w.dtype != F16 or w.dim() != 2:
+        raise TypeError(f"quantize_fp8: expected a 2-D float16 tensor, got {w.dtype} {tuple(w.shape)}")
+    N, K = w.shape
+    q = torch.empty(N, K, dtype=F8, device=w.device)
+    s = torch.empty(N, dtype=F16, device=w.device)
+    tiny = torch.finfo(F16).smallest_normal * 2.0 ** -10          # 2^-24, the smallest positive (subnormal) fp16
+    for r0 in range(0, N, rows_per_chunk):
+        blk = w[r0:r0 + rows_per_chunk].float()
+        amax = blk.abs().amax(dim=1)
+        sc = (amax / FP8_MAX).to(F16)
+        sc = torch.where(amax == 0, torch.ones_like(sc), torch.where(sc == 0, torch.full_like(sc, tiny), sc))
+        q[r0:r0 + rows_per_chunk] = (blk / sc.float()[:, None]).clamp_(-FP8_MAX, FP8_MAX).to(F8)
+        s[r0:r0 + rows_per_chunk] = sc
+    return q, s
+
+
+def dequantize_fp8(q: torch.Tensor, s: torch.Tensor) -> torch.Tensor:
+    """W'[j, k] = fp16(fp16(q[j, k]) * s[j]): the fp16 matrix the FP8 GEMM multiplies by (exact e4m3 -> fp16, one
+    rounding of the product)."""
+    return q.to(F16) * s.to(F16)[:, None]
+
+
+def fp8_tile_weights(q: torch.Tensor) -> torch.Tensor:
+    """(N, K) float8_e4m3fn row-major -> the FP8 GEMM's pre-tiled copy (N * K bytes, layout in include/sequoia_b200.h)."""
+    if q.dtype != F8 or not q.is_cuda or not q.is_contiguous():
+        raise TypeError("fp8_tile_weights: expected a contiguous CUDA float8_e4m3fn tensor")
+    N, K = q.shape
+    out = torch.empty(N * K, dtype=torch.uint8, device=q.device)
+    check(_lib.load().sq_gemm_fp8_tile_weights(ptr(q), ptr(out), N, K, stream_ptr(q.device)), "sq_gemm_fp8_tile_weights")
+    return out
+
+
+class GemmFp8Plan:
+    """C[:n] = A[:n] @ W'.T on the FP8 weight-streaming kernel, W' = dequantize_fp8(q, s).  The plan keeps the pre-tiled
+    copy of q and the scales (the only resident form of the weight); n > 128 runs one launch per 128 rows."""
+
+    def __init__(self, a: torch.Tensor, q: torch.Tensor, s: torch.Tensor, c: torch.Tensor,
+                 err_flag: Optional[torch.Tensor] = None):
+        assert a.dtype == F16 and c.dtype == F16 and s.dtype == F16 and q.dtype == F8
+        assert a.stride(-1) == 1 and c.stride(-1) == 1 and a.shape[1] == q.shape[1] and c.shape[1] >= q.shape[0]
+        assert s.shape == (q.shape[0],) and s.is_contiguous()
+        self.N, self.K = q.shape
+        self.w_tiled = fp8_tile_weights(q)
+        self.scale = s
+        self.handle = C.c_void_p()
+        self._keep = (a, c, err_flag)
+        check(_lib.load().sq_gemm_fp8_plan_create(C.byref(self.handle), ptr(a), a.stride(0), a.shape[0], ptr(self.w_tiled),
+                                                  ptr(s), self.N, self.K, ptr(c), c.stride(0), ptr(err_flag)),
+              "sq_gemm_fp8_plan_create")
+
+    def info(self):
+        """(64-row weight tiles per CTA, K splits, ring stages of the 128-row instance)"""
+        w, sp, st = C.c_int(), C.c_int(), C.c_int()
+        check(_lib.load().sq_gemm_fp8_plan_info(self.handle, C.byref(w), C.byref(sp), C.byref(st)), "sq_gemm_fp8_plan_info")
+        return w.value, sp.value, st.value
+
+    def weight_bytes(self) -> int:
+        return self.w_tiled.numel() + 2 * self.scale.numel()
+
+    def run(self, n: int, a_row0: int = 0, out: Optional[torch.Tensor] = None):
+        """rows [a_row0, a_row0+n) of the activation buffer -> `out[:n]` (default: the plan's output buffer, same rows)."""
+        if out is not None:
+            assert out.dtype == F16 and out.stride(-1) == 1 and out.shape[0] >= n
+        check(_lib.load().sq_gemm_fp8_run_at(self.handle, n, a_row0, ptr(out), out.stride(0) if out is not None else 0,
+                                             stream_ptr()), "sq_gemm_fp8_run_at")
+
+    def __del__(self):
+        try:
+            if self.handle:
+                _lib.load().sq_gemm_fp8_plan_destroy(self.handle)
+                self.handle = None
+        except Exception:
+            pass
+
+
 # ---- draft attention (csrc/sq_draft.cu) -----------------------------------------------------------------------------------
 def draft_supported(hidden, n_heads, n_kv_heads, head_dim, max_length) -> bool:
     return bool(_lib.load().sq_draft_supported(hidden, n_heads, n_kv_heads, head_dim, max_length))

@@ -244,6 +244,8 @@ def build_parser():
     ap.add_argument("--offloading", action="store_true", help="use OffloadEngine for the target (weights stay resident)")
     ap.add_argument("--batch", type=int, default=1,
                     help="decode this many prompts together (--Mode greedy, --tree spec|greedy; the prompt count must divide)")
+    ap.add_argument("--target-weights", type=str, default="fp16", choices=["fp16", "fp8"],
+                    help="fp8: the target's layer projections quantized to E4M3 with per-channel scales at load")
     return ap
 
 
@@ -256,13 +258,15 @@ def main(argv=None):
     prompts = load_prompts(args.dataset, args.start, args.end, args.seed)
     tcls = OffloadEngine if args.offloading else GraphInferenceEngineTG
     stop = stop_tokens(args.target)
+    if args.target_weights != "fp16" and args.offloading:
+        raise SystemExit("--target-weights fp8 runs without --offloading")
     if args.batch != 1:
         if args.Mode != "greedy" or args.tree not in ("spec", "greedy") or args.offloading:
             raise SystemExit("--batch runs --Mode greedy with --tree spec or greedy, without --offloading")
         if len(prompts) % args.batch:
             raise SystemExit(f"--batch {args.batch} must divide the {len(prompts)} prompts")
         target = GraphInferenceEngineTG(max_length=args.M, model_name_or_path=args.target, dtype=torch.float16,
-                                        device=DEV, batch_size=args.batch)
+                                        device=DEV, batch_size=args.batch, weight_format=args.target_weights)
         draft = GraphInferenceEngine(max_length=args.M, model_name_or_path=args.model, dtype=torch.float16, device=DEV,
                                      batch_size=args.batch)
         path = args.growmap if os.path.isabs(args.growmap) or os.path.exists(args.growmap) else os.path.join(ROOT, args.growmap)
@@ -272,7 +276,10 @@ def main(argv=None):
                                stop=stop)
         print(json.dumps({k: (round(v, 5) if isinstance(v, float) else v) for k, v in res.items()}))
         return res
-    target = tcls(max_length=args.M, model_name_or_path=args.target, dtype=torch.float16, device=DEV)
+    target = (tcls(max_length=args.M, model_name_or_path=args.target, dtype=torch.float16, device=DEV)
+              if args.offloading else
+              tcls(max_length=args.M, model_name_or_path=args.target, dtype=torch.float16, device=DEV,
+                   weight_format=args.target_weights))
     if args.Mode == "baseline":
         res = simulation_baseline(target, prompts, args.T, args.P, args.M, stop=stop)
     else:
