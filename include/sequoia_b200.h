@@ -359,6 +359,26 @@ int sq_accept_stochastic_batch(const sq_half* target_logits, int64_t ld_t, const
                                int64_t ld_noise, const int32_t* succ_off, const int32_t* succ, const int32_t* depth, int S,
                                int V, float T, int64_t* tokens, int64_t* position_ids, int64_t ld_seq, int32_t* accept_idx,
                                int64_t ld_acc, int32_t* state, int B, int max_target_seq, int policy, void* stream);
+/* Per-sequence sampling parameters: as sq_sample_level_batch / sq_accept_stochastic_batch / sq_top_p_filter, with the
+ * temperature (and top_p) of sequence b read from (B,) fp32 device arrays T[b] / top_p[b] instead of one scalar, so a
+ * captured graph serves sequences with any settings.  With all-equal arrays each computes bit for bit what the scalar
+ * call computes.  sq_sample_level_batch_per_seq: mode 0 uses T[b], mode 1 ignores it.  sq_top_p_filter_per_seq: row r of
+ * the n rows belongs to sequence r / rows_per_seq (rows_per_seq must divide n); a row whose sequence has top_p >= 1 is left
+ * untouched.  Null arrays are refused with SQ_ERR_INVALID_ARG. */
+int sq_sample_level_batch_per_seq(const sq_half* logits, int64_t ld_logits, const int32_t* row_base,
+                                  const int32_t* row_step, const sq_half* rand, int64_t ld_rand, int64_t ld_rand_seq,
+                                  const int32_t* parent_rows, const int32_t* child_first, const int32_t* n_branch,
+                                  int n_parents, int k_max, int V, const float* T, int mode, int64_t* tokens,
+                                  int64_t ld_seq, const int32_t* state, int B, void* stream);
+int sq_accept_stochastic_batch_per_seq(const sq_half* target_logits, int64_t ld_t, const sq_half* draft_logits,
+                                       int64_t ld_d, const int32_t* row_base, const int32_t* row_step, const sq_half* r,
+                                       const sq_half* noise, int64_t ld_noise, const int32_t* succ_off,
+                                       const int32_t* succ, const int32_t* depth, int S, int V, const float* T,
+                                       int64_t* tokens, int64_t* position_ids, int64_t ld_seq, int32_t* accept_idx,
+                                       int64_t ld_acc, int32_t* state, int B, int max_target_seq, int policy,
+                                       void* stream);
+int sq_top_p_filter_per_seq(sq_half* logits, int64_t ld, int n, int V, const float* top_p, const float* T,
+                            int rows_per_seq, void* stream);
 /* target_token (B*S) int64 */
 int sq_accept_greedy_batch(const int64_t* target_token, const int32_t* succ_off, const int32_t* succ, const int32_t* depth,
                            int S, int64_t* tokens, int64_t* position_ids, int64_t ld_seq, int32_t* accept_idx,

@@ -86,6 +86,11 @@ _SIGNATURES = {
     "sq_accept_stochastic_batch": (i32, [vp, i64, vp, i64, vp, vp, vp, vp, i64, vp, vp, vp, i32, i32, f32, vp, vp, i64, vp,
                                          i64, vp, i32, i32, i32, vp]),
     "sq_accept_greedy_batch": (i32, [vp, vp, vp, vp, i32, vp, vp, i64, vp, i64, vp, i32, i32, vp]),
+    "sq_sample_level_batch_per_seq": (i32, [vp, i64, vp, vp, vp, i64, i64, vp, vp, vp, i32, i32, i32, vp, i32, vp, i64,
+                                            vp, i32, vp]),
+    "sq_accept_stochastic_batch_per_seq": (i32, [vp, i64, vp, i64, vp, vp, vp, vp, i64, vp, vp, vp, i32, i32, vp, vp, vp,
+                                                 i64, vp, i64, vp, i32, i32, i32, vp]),
+    "sq_top_p_filter_per_seq": (i32, [vp, i64, i32, i32, vp, vp, i32, vp]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

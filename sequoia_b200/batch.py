@@ -1,17 +1,21 @@
-"""Several prompts per decode step: B sequences that share the engines, the growmap, T and top_p (DESIGN.md §3a).
+"""Several prompts per decode step: B sequences that share the engines and the growmap (DESIGN.md §3a).
 
 A steady step is the same two graph replays and one host sync as a single-sequence tree (sequoia_b200.tree), for all B
 sequences together: every per-sequence kernel is one launch for the batch, the row-wise kernels and the GEMMs see B*n
 rows.  Sequence b's device data: row b of state (B, 16), tokens / position_ids / storage_ids / r (B, M), rand (B, S, V),
-noise (B, V), accept_idx (B, S); rows b*S .. b*S+S-1 of the target logits (B*S, V); the draft logits of node k at
-row_base[k] + b*row_step[k] (each tree level of all sequences is one block, written by one lm_head GEMM).
+noise (B, V), accept_idx (B, S), its temperature and top_p (B,); rows b*S .. b*S+S-1 of the target logits (B*S, V); the
+draft logits of node k at row_base[k] + b*row_step[k] (each tree level of all sequences is one block, written by one
+lm_head GEMM).
 
 A sequence that is terminal, or has no room for another tree in max_length, is frozen: its state word SQ_ST_FROZEN is
-set and every batched kernel leaves its tokens, state and KV rows alone until the batch ends.
+set and every batched kernel leaves its tokens, state and KV rows alone.  A frozen slot can take a new prompt with
+admit(); the other sequences keep decoding.
 """
 from __future__ import annotations
 
-from typing import Dict, List, Optional, Sequence
+import math
+import numbers
+from typing import Dict, List, Optional, Sequence, Union
 
 import torch
 
@@ -33,17 +37,45 @@ def draw_random(prompts: Sequence[torch.Tensor], M: int, S: int, V: int):
     return torch.stack(rs), torch.stack(rands)
 
 
+def _h2d(t: torch.Tensor) -> torch.Tensor:
+    """A copy source that does not block the host: device tensors as they are, host tensors pinned (the caching host
+    allocator keeps the pinned block until the copy has run)."""
+    return t if t.is_cuda else t.pin_memory()
+
+
+def check_sampling(temperature: float, top_p: float):
+    """Refuse a temperature that is not a finite T > 0 and a top_p outside (0, 1]."""
+    if not (math.isfinite(temperature) and temperature > 0):
+        raise ValueError(f"temperature must be finite and > 0, got {temperature}")
+    if not (math.isfinite(top_p) and 0 < top_p <= 1):
+        raise ValueError(f"top_p must be in (0, 1], got {top_p}")
+
+
+def _per_seq(value, B: int, name: str) -> List[float]:
+    """One value (a Python, numpy or 0-d tensor scalar) for all B sequences, or a sequence of B values."""
+    if isinstance(value, numbers.Real) or (isinstance(value, torch.Tensor) and value.dim() == 0):
+        return [float(value)] * B
+    vals = [float(v) for v in value]
+    if len(vals) != B:
+        raise ValueError(f"{name}: {len(vals)} values for {B} sequences")
+    return vals
+
+
 class BatchTree:
     """Batched SpecTree ("spec") / GreedyTree ("greedy") over `len(prompts)` sequences.  The engines must have been built
-    with batch_size == len(prompts).  verify() returns one (valid_tokens, accept_length, terminal) per sequence."""
+    with batch_size == len(prompts).  verify() returns one (valid_tokens, accept_length, terminal) per sequence.
+    temperature and top_p: one value for all sequences, or one per sequence; "greedy" ignores both."""
 
     def __init__(self, draft, target, prompts: Sequence[torch.Tensor], grow_map: dict, policy: str = "spec",
-                 temperature: float = 0.6, top_p: float = 1.0, max_length: int = 256,
-                 max_target_seq: Optional[int] = None):
+                 temperature: Union[float, Sequence[float]] = 0.6, top_p: Union[float, Sequence[float]] = 1.0,
+                 max_length: int = 256, max_target_seq: Optional[int] = None):
         if policy not in POLICIES:
             raise ValueError(f"BatchTree policy {policy!r} is not supported (only {POLICIES}); greedys, specinfer and the "
                              "*TreeTest policies run one sequence at a time")
         B = len(prompts)
+        temps, top_ps = _per_seq(temperature, B, "temperature"), _per_seq(top_p, B, "top_p")
+        for t, p in zip(temps, top_ps):
+            check_sampling(t, p)
         for name, eng in (("draft", draft), ("target", target)):
             if eng.engine.batch_size != B:
                 raise ValueError(f"{name} engine holds {eng.engine.batch_size} sequences, got {B} prompts")
@@ -54,7 +86,7 @@ class BatchTree:
             raise RuntimeError("sequoia_b200 trees run on a CUDA device only (there is no CPU path)")
         self.draft, self.target = draft, target
         self.policy, self.greedy = policy, policy == "greedy"
-        self.T, self.top_p = float(temperature), float(top_p)
+        self.temps, self.top_ps = temps, top_ps
         self.B, self.M = B, max_length
         self.max_target_seq = max_target_seq or max_length
         self.st = st = _Static(grow_map, dev)
@@ -66,6 +98,11 @@ class BatchTree:
             if len(p) + S - 1 > M:
                 raise ValueError(f"max_length={M} must hold the prompt ({len(p)}) + tree ({S}) - 1")
         self.device = dev
+        # sampling parameters live on the device, so the captured graphs serve any values an admission brings; the top-p
+        # filter joins the steady / post graphs only once a sequence has had top_p < 1 (one recapture, see admit)
+        self.T_dev = torch.tensor(temps, dtype=torch.float32, device=dev)
+        self.top_p_dev = torch.tensor(top_ps, dtype=torch.float32, device=dev)
+        self.use_top_p = not self.greedy and any(p < 1.0 for p in top_ps)
         i64 = dict(dtype=torch.int64, device=dev)
         self.tokens = torch.zeros(B, M, **i64)
         self.position_ids = torch.zeros(B, M, **i64)
@@ -83,6 +120,8 @@ class BatchTree:
         self.graphs: Dict[str, torch.cuda.CUDAGraph] = {}
         self.graph_launches: Dict[str, int] = {}
         self.replays: Dict[str, int] = {}
+        self.captures: Dict[str, int] = {}
+        self.replayed_launches = 0
         self.use_graphs = True
         self.iter = 0
         self.frozen = [False] * B
@@ -94,28 +133,36 @@ class BatchTree:
             self.r, self.rand = r.to(dev), rand.to(dev)
         else:
             self.r = self.rand = None
-        st0 = torch.zeros(B, 16, dtype=torch.int32)
-        pos = torch.zeros(B, M, dtype=torch.int64)
         for b, p in enumerate(prompts):
-            P = len(p)
-            self.tokens[b, :P] = p.to(dev)
-            pos[b, :P] = torch.arange(P)
-            pos[b, P:P + S - 1] = st.depth_cpu[1:] + P - 1
-            st0[b, ST_P], st0[b, ST_M] = P, M
-        self.position_ids.copy_(pos)
-        self.state.copy_(st0)
-        # draft prefill (SpecTree.py:67-80), one sequence at a time: rows [0, P) causal, the last row's logits -> node 0
+            self._load_prompt(b, p)
         with torch.inference_mode():
             for b in range(B):
-                P = self.ground_truth_len[b]
-                self._alone(b, lambda: draft.engine.runner.forward(
-                    P, self.tokens, self.position_ids, self.storage_ids, state=self.state, n0=1 - P, kv_end=1,
-                    batch=True, logits_from=b * P + P - 1, logits_to=b * P + P, logits_out=self.draft_logits[b:b + 1],
-                    **self._mask_kw()))
+                self._prefill(b)
 
     # ---- helpers ---------------------------------------------------------------------------------------------------------
     def _mask_kw(self):
         return dict(tree_bits=self.st.tree_bits, tree_words=self.st.tree_words, tree_size=self.S)
+
+    def _load_prompt(self, b: int, prompt: torch.Tensor):
+        """Row b of tokens, position ids, state and accept_idx for a new prompt: nothing of an earlier occupant stays."""
+        P, S, M = len(prompt), self.S, self.M
+        pos = torch.zeros(M, dtype=torch.int64)
+        pos[:P] = torch.arange(P)
+        pos[P:P + S - 1] = self.st.depth_cpu[1:] + P - 1
+        st0 = torch.zeros(16, dtype=torch.int32)
+        st0[ST_P], st0[ST_M] = P, M
+        self.tokens[b].zero_()
+        self.tokens[b, :P].copy_(_h2d(prompt), non_blocking=True)
+        self.position_ids[b].copy_(_h2d(pos), non_blocking=True)
+        self.state[b].copy_(_h2d(st0), non_blocking=True)
+        self.accept_idx[b].zero_()
+
+    def _prefill(self, b: int):
+        """Draft prefill of sequence b (SpecTree.py:67-80): rows [0, P) causal, the last row's logits -> node 0."""
+        P = self.ground_truth_len[b]
+        self._alone(b, lambda: self.draft.engine.runner.forward(
+            P, self.tokens, self.position_ids, self.storage_ids, state=self.state, n0=1 - P, kv_end=1, batch=True,
+            logits_from=b * P + P - 1, logits_to=b * P + P, logits_out=self.draft_logits[b:b + 1], **self._mask_kw()))
 
     def _alone(self, b: int, fn):
         """Run a batched op sequence for sequence b only (prefill and first verify, whose row count depends on the
@@ -130,16 +177,49 @@ class BatchTree:
         self.state.copy_(saved)
 
     def freeze(self, b: int):
-        """Stop sequence b (the caller's length limit); it stays frozen until the batch ends."""
+        """Stop sequence b (the caller's length limit); it stays frozen until admit() gives the slot a new prompt."""
         self.frozen[b] = True
         self.state[b, ST_FROZEN] = 1
+
+    @torch.inference_mode()
+    def admit(self, b: int, prompt: torch.Tensor, temperature: Optional[float] = None, top_p: Optional[float] = None):
+        """Start `prompt` in the frozen slot b (finished, out of room, or stopped with freeze), at its own temperature and
+        top_p (default: the slot's previous values).  The next verify() runs its first verify next to the steady
+        sequences.  The slot draws r and rand as a lone SpecTree on the prompt would, and runs its draft prefill now."""
+        if not 0 <= b < self.B:
+            raise IndexError(f"slot {b} out of range for a batch of {self.B}")
+        if not self.frozen[b]:
+            raise ValueError(f"slot {b} is still decoding; admit takes a finished or frozen slot")
+        P = len(prompt)
+        if P < 1 or P + self.S - 1 > self.M:
+            raise ValueError(f"max_length={self.M} must hold the prompt ({P}) + tree ({self.S}) - 1")
+        T = self.temps[b] if temperature is None else float(temperature)
+        tp = self.top_ps[b] if top_p is None else float(top_p)
+        check_sampling(T, tp)
+        self.temps[b], self.top_ps[b] = T, tp
+        self.T_dev[b] = T
+        self.top_p_dev[b] = tp
+        if tp < 1.0 and not self.greedy and not self.use_top_p:
+            self.use_top_p = True                  # the filter enters op_accept: capture steady and post once more
+            for name in ("steady", "post"):
+                self.graphs.pop(name, None)
+        self._load_prompt(b, prompt)
+        self.frozen[b] = False
+        self.last[b] = None
+        self.ground_truth_len[b] = P
+        self.target_kv_len[b] = 0
+        if not self.greedy:
+            r, rand = draw_random([prompt], self.M, self.S, self.V)
+            self.r[b].copy_(_h2d(r[0]), non_blocking=True)
+            self.rand[b].copy_(_h2d(rand[0]), non_blocking=True)
+        self._prefill(b)
 
     # ---- the op sequences ------------------------------------------------------------------------------------------------
     def op_sample(self, i: int):
         lv = self.st.levels[i]
-        ops.sample_level_batch(self.draft_logits, self.row_base, self.row_step, self.rand, lv["n_parents"], lv["k"],
-                               self.T, 1 if self.greedy else 0, parent_rows=lv["parents"], child_first=lv["first"],
-                               n_branch=lv["nb"], tokens=self.tokens, state=self.state)
+        ops.sample_level_batch_per_seq(self.draft_logits, self.row_base, self.row_step, self.rand, lv["n_parents"],
+                                       lv["k"], self.T_dev, 1 if self.greedy else 0, parent_rows=lv["parents"],
+                                       child_first=lv["first"], n_branch=lv["nb"], tokens=self.tokens, state=self.state)
 
     def op_draft_level(self, i: int):
         lv = self.st.levels[i]
@@ -169,13 +249,13 @@ class BatchTree:
             ops.accept_greedy_batch(self.target_token, st.succ_off, st.succ, st.depth, self.S, self.tokens,
                                     self.position_ids, self.accept_idx, self.state, self.max_target_seq)
             return
-        if self.top_p < 1.0:
-            ops.top_p_filter_(self.target_logits, self.top_p, self.T)
+        if self.use_top_p:
+            ops.top_p_filter_per_seq_(self.target_logits, self.top_p_dev, self.T_dev, self.S)
         if self.external_noise is None:
             self.noise.exponential_(1.0)
-        ops.accept_stochastic_batch(self.target_logits, self.draft_logits, self.row_base, self.row_step, self.r,
-                                    self.noise, st.succ_off, st.succ, st.depth, self.S, self.T, self.tokens,
-                                    self.position_ids, self.accept_idx, self.state, self.max_target_seq)
+        ops.accept_stochastic_batch_per_seq(self.target_logits, self.draft_logits, self.row_base, self.row_step, self.r,
+                                            self.noise, st.succ_off, st.succ, st.depth, self.S, self.T_dev, self.tokens,
+                                            self.position_ids, self.accept_idx, self.state, self.max_target_seq)
 
     def op_kv_gather(self):
         md = max(self.st.max_depth, 1)
@@ -224,8 +304,10 @@ class BatchTree:
             self.graph_launches[name] = _lib.launch_count() - c0
             self._restore(snap)
             self.graphs[name] = g
+            self.captures[name] = self.captures.get(name, 0) + 1
         g.replay()
         self.replays[name] = self.replays.get(name, 0) + 1
+        self.replayed_launches += self.graph_launches[name]      # per replay: a recapture changes the count
 
     def _caches(self):
         return [t for e in (self.draft, self.target) for t in (e.engine.kv_cache.k_cache, e.engine.kv_cache.v_cache)]
@@ -244,7 +326,8 @@ class BatchTree:
         torch.cuda.set_rng_state(s["rng"], self.device)
 
     def kernel_launches(self) -> int:
-        return sum(self.graph_launches.get(k, 0) * v for k, v in self.replays.items())
+        """Kernels launched by graph replays so far, each replay counted with the launches of the graph it replayed."""
+        return self.replayed_launches
 
     # ---- the reference-style steps ---------------------------------------------------------------------------------------
     @torch.inference_mode()
@@ -258,7 +341,15 @@ class BatchTree:
             self.noise.copy_(self.external_noise[self.iter])
         first = [b for b in range(self.B) if not self.frozen[b] and self.target_kv_len[b] != self.ground_truth_len[b] - 1]
         if first:
-            # prefill + tree rows of each sequence eagerly (their row counts differ); the walk and the rest batched
+            if len(first) + sum(self.frozen) < self.B:
+                # steady sequences share the step with admitted ones: their tree rows first, the admitted slots frozen
+                saved = self.state.clone()
+                for b in first:
+                    self.state[b, ST_FROZEN] = 1
+                self.op_target_steady()
+                self.state.copy_(saved)
+            # prefill + tree rows of each first-verify sequence eagerly (their row counts differ); the walk and the rest
+            # batched
             for b in first:
                 self.op_target_first(b)
             self.run("post", self.seq_post)

@@ -294,6 +294,24 @@ extern "C" int sq_accept_greedy_batch(const int64_t* target_token, const int32_t
   return SQ_OK;
 }
 
+// sq_accept_stochastic_batch (T_seq == nullptr) and its per-sequence form
+static int accept_stochastic_batch(const char* name, const sq_half* target_logits, int64_t ld_t,
+                                   const sq_half* draft_logits, int64_t ld_d, const int32_t* row_base,
+                                   const int32_t* row_step, const sq_half* r, const sq_half* noise, int64_t ld_noise,
+                                   const int32_t* succ_off, const int32_t* succ, const int32_t* depth, int S, int V,
+                                   float T, const float* T_seq, int64_t* tokens, int64_t* position_ids, int64_t ld_seq,
+                                   int32_t* accept_idx, int64_t ld_acc, int32_t* state, int B, int max_target_seq,
+                                   int policy, void* stream) {
+  SQ_CHECK_ARG(S >= 1 && S <= 1024, "%s: S=%d unsupported", name, S);
+  SQ_CHECK_ARG(B >= 1 && B <= SQ_MAX_BATCH, "%s: B=%d (1..%d)", name, B, SQ_MAX_BATCH);
+  SQ_CHECK_ARG((policy & ~3) == 0, "%s: unknown policy bits %d", name, policy);
+  SQ_CHECK_ARG(row_base && row_step, "%s: null draft-row table", name);
+  SQ_CHECK_ARG(ld_acc >= S && ld_noise >= V, "%s: accept_idx / noise rows too short", name);
+  BatchArgs ba{B, ld_seq, ld_noise, ld_acc, row_base, row_step};
+  return sq::launch_accept_cluster(target_logits, ld_t, draft_logits, ld_d, r, noise, succ_off, succ, depth, S, V, T, tokens,
+                                   position_ids, accept_idx, state, max_target_seq, policy, stream, &ba, T_seq);
+}
+
 extern "C" int sq_accept_stochastic_batch(const sq_half* target_logits, int64_t ld_t, const sq_half* draft_logits,
                                           int64_t ld_d, const int32_t* row_base, const int32_t* row_step, const sq_half* r,
                                           const sq_half* noise, int64_t ld_noise, const int32_t* succ_off,
@@ -301,12 +319,20 @@ extern "C" int sq_accept_stochastic_batch(const sq_half* target_logits, int64_t 
                                           int64_t* tokens, int64_t* position_ids, int64_t ld_seq, int32_t* accept_idx,
                                           int64_t ld_acc, int32_t* state, int B, int max_target_seq, int policy,
                                           void* stream) {
-  SQ_CHECK_ARG(S >= 1 && S <= 1024, "sq_accept_stochastic_batch: S=%d unsupported", S);
-  SQ_CHECK_ARG(B >= 1 && B <= SQ_MAX_BATCH, "sq_accept_stochastic_batch: B=%d (1..%d)", B, SQ_MAX_BATCH);
-  SQ_CHECK_ARG((policy & ~3) == 0, "sq_accept_stochastic_batch: unknown policy bits %d", policy);
-  SQ_CHECK_ARG(row_base && row_step, "sq_accept_stochastic_batch: null draft-row table");
-  SQ_CHECK_ARG(ld_acc >= S && ld_noise >= V, "sq_accept_stochastic_batch: accept_idx / noise rows too short");
-  BatchArgs ba{B, ld_seq, ld_noise, ld_acc, row_base, row_step};
-  return sq::launch_accept_cluster(target_logits, ld_t, draft_logits, ld_d, r, noise, succ_off, succ, depth, S, V, T, tokens,
-                                   position_ids, accept_idx, state, max_target_seq, policy, stream, &ba);
+  return accept_stochastic_batch("sq_accept_stochastic_batch", target_logits, ld_t, draft_logits, ld_d, row_base, row_step,
+                                 r, noise, ld_noise, succ_off, succ, depth, S, V, T, nullptr, tokens, position_ids, ld_seq,
+                                 accept_idx, ld_acc, state, B, max_target_seq, policy, stream);
+}
+
+extern "C" int sq_accept_stochastic_batch_per_seq(const sq_half* target_logits, int64_t ld_t, const sq_half* draft_logits,
+                                                  int64_t ld_d, const int32_t* row_base, const int32_t* row_step,
+                                                  const sq_half* r, const sq_half* noise, int64_t ld_noise,
+                                                  const int32_t* succ_off, const int32_t* succ, const int32_t* depth, int S,
+                                                  int V, const float* T, int64_t* tokens, int64_t* position_ids,
+                                                  int64_t ld_seq, int32_t* accept_idx, int64_t ld_acc, int32_t* state,
+                                                  int B, int max_target_seq, int policy, void* stream) {
+  SQ_CHECK_ARG(T != nullptr, "sq_accept_stochastic_batch_per_seq: null temperature array");
+  return accept_stochastic_batch("sq_accept_stochastic_batch_per_seq", target_logits, ld_t, draft_logits, ld_d, row_base,
+                                 row_step, r, noise, ld_noise, succ_off, succ, depth, S, V, 1.0f, T, tokens, position_ids,
+                                 ld_seq, accept_idx, ld_acc, state, B, max_target_seq, policy, stream);
 }

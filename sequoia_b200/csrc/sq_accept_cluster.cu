@@ -75,13 +75,16 @@ struct ClusterCtx {
 
 // BATCH: grid (CL, B), one cluster per sequence (see BatchArgs); a frozen sequence's cluster exits before its first
 // exchange (the whole cluster reads the same word).
-template <bool BATCH, int NCH>
+// PER_SEQ (BATCH only): `temp` is the (B,) temperature array and the walk of sequence b scales both the target and the
+// draft rows by 1/T[b]; otherwise `temp` is the scalar 1/T.
+template <bool BATCH, int NCH, bool PER_SEQ = false>
 __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(CNT) accept_stochastic_cluster_kernel(
     const __half* __restrict__ target_logits, int64_t ld_t, const __half* __restrict__ draft_logits, int64_t ld_d,
     const __half* __restrict__ r, const __half* __restrict__ noise, const int32_t* __restrict__ succ_off,
-    const int32_t* __restrict__ succ, const int32_t* __restrict__ depth, int S, int V, float inv_T,
+    const int32_t* __restrict__ succ, const int32_t* __restrict__ depth, int S, int V, SeqParam<PER_SEQ> temp,
     int64_t* __restrict__ tokens, int64_t* __restrict__ position_ids, int32_t* __restrict__ accept_idx,
     int32_t* __restrict__ state, int max_target_seq, int policy, BatchArgs ba) {
+  static_assert(BATCH || !PER_SEQ, "per-sequence parameters need the batched kernel");
   __shared__ Xch xch;
   __shared__ float red[CNW];
   __shared__ int32_t sh_acc[1024];
@@ -98,6 +101,7 @@ __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(CNT) accept_stochas
     position_ids += b * ba.ld_seq;
     accept_idx += b * ba.ld_acc;
   }
+  const float inv_T = inv_temp(temp, b);
   ClusterCtx cx{cg::this_cluster(), &xch, 0, 0};
   cx.rank = (int)cx.cluster.block_rank();
   const int P = state[ST_P];
@@ -294,7 +298,14 @@ static int launch_accept_nch(const sq_half* target_logits, int64_t ld_t, const s
                              const sq_half* r, const sq_half* noise, const int32_t* succ_off, const int32_t* succ,
                              const int32_t* depth, int S, int V, float T, int64_t* tokens, int64_t* position_ids,
                              int32_t* accept_idx, int32_t* state, int max_target_seq, int policy, void* stream,
-                             const BatchArgs* batch) {
+                             const BatchArgs* batch, const float* T_seq) {
+  if (batch && T_seq) {
+    accept_stochastic_cluster_kernel<true, NCH, true><<<dim3(CL, batch->B), CNT, 0, (cudaStream_t)stream>>>(
+        (const __half*)target_logits, ld_t, (const __half*)draft_logits, ld_d, (const __half*)r, (const __half*)noise,
+        succ_off, succ, depth, S, V, T_seq, tokens, position_ids, accept_idx, state, max_target_seq, policy, *batch);
+    SQ_CHECK_LAUNCH("sq_accept_stochastic_batch_per_seq");
+    return SQ_OK;
+  }
   if (batch) {
     accept_stochastic_cluster_kernel<true, NCH><<<dim3(CL, batch->B), CNT, 0, (cudaStream_t)stream>>>(
         (const __half*)target_logits, ld_t, (const __half*)draft_logits, ld_d, (const __half*)r, (const __half*)noise,
@@ -313,14 +324,14 @@ int sq::launch_accept_cluster(const sq_half* target_logits, int64_t ld_t, const 
                               const sq_half* r, const sq_half* noise, const int32_t* succ_off, const int32_t* succ,
                               const int32_t* depth, int S, int V, float T, int64_t* tokens, int64_t* position_ids,
                               int32_t* accept_idx, int32_t* state, int max_target_seq, int policy, void* stream,
-                              const BatchArgs* batch) {
+                              const BatchArgs* batch, const float* T_seq) {
   SQ_CHECK_ARG(V % 8 == 0 && V > 0 && V <= CL * CNT * 8 * 4, "sq_accept_stochastic: V=%d unsupported (multiple of 8, "
                "<= %d)", V, CL * CNT * 8 * 4);
   const int nch = (V + CL * CNT * 8 - 1) / (CL * CNT * 8);
   auto go = [&](auto kern_nch) {
     return launch_accept_nch<decltype(kern_nch)::value>(target_logits, ld_t, draft_logits, ld_d, r, noise, succ_off, succ,
                                                         depth, S, V, T, tokens, position_ids, accept_idx, state,
-                                                        max_target_seq, policy, stream, batch);
+                                                        max_target_seq, policy, stream, batch, T_seq);
   };
   if (nch == 1) return go(std::integral_constant<int, 1>{});
   if (nch == 2) return go(std::integral_constant<int, 2>{});

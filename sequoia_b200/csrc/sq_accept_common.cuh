@@ -18,12 +18,12 @@ struct BatchArgs {
   }
 };
 
-// batch == nullptr: the single-sequence kernel
+// batch == nullptr: the single-sequence kernel.  T_seq (batches only): the (B,) temperature array, used instead of T.
 int launch_accept_cluster(const sq_half* target_logits, int64_t ld_t, const sq_half* draft_logits, int64_t ld_d,
                           const sq_half* r, const sq_half* noise, const int32_t* succ_off, const int32_t* succ,
                           const int32_t* depth, int S, int V, float T, int64_t* tokens, int64_t* position_ids,
                           int32_t* accept_idx, int32_t* state, int max_target_seq, int policy, void* stream,
-                          const BatchArgs* batch = nullptr);
+                          const BatchArgs* batch = nullptr, const float* T_seq = nullptr);
 
 // policy bits: SQ_ACCEPT_GE / SQ_ACCEPT_KEEP_Q from include/sequoia_b200.h
 

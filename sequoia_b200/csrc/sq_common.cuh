@@ -4,6 +4,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 #include "../../include/sequoia_b200.h"
 
 namespace sq {
@@ -70,6 +72,15 @@ enum StateWord : int {
 // Batched entry points: sequence b is the grid's batch index.  BATCH = false compiles the single-sequence kernel unchanged.
 template <bool BATCH>
 __device__ __forceinline__ int seq_index(unsigned grid_coord) { return BATCH ? (int)grid_coord : 0; }
+
+// Per-sequence sampling parameters (PER_SEQ = true): the kernel argument is a (B,) fp32 device array read at the
+// sequence's index; PER_SEQ = false keeps the scalar argument, so those instances compile as before.
+template <bool PER_SEQ>
+using SeqParam = typename std::conditional<PER_SEQ, const float*, float>::type;
+// temperature argument -> 1/T of sequence b: the scalar form already carries the host's fp32 1/T; the per-sequence form
+// divides on the device, which rounds the same (IEEE division, no fast-math)
+__device__ __forceinline__ float inv_temp(float inv_T, int) { return inv_T; }
+__device__ __forceinline__ float inv_temp(const float* T, int b) { return 1.0f / T[b]; }
 
 __device__ __forceinline__ int row_base(const int32_t* P_ptr, int n0) {
   return (P_ptr ? (P_ptr[ST_P] - 1) : 0) + n0;

@@ -189,13 +189,15 @@ __device__ __forceinline__ void wide_topk_merge(const uint64_t* gk, int n, int k
 // its rand rows at rand + b * ld_rand_seq, writes tokens + b * ld_seq, and does nothing when frozen.
 // WIDE: grid (n * n_parents, B), clusters of n = ceil(V / SLICE) CTAs; the whole cluster reads the same frozen word and
 // k_need, so it takes every exit together.
-template <bool BATCH, bool WIDE>
+// PER_SEQ (BATCH only): `temp` is the (B,) temperature array and mode 0 uses T[b]; otherwise `temp` is the scalar 1/T.
+template <bool BATCH, bool WIDE, bool PER_SEQ = false>
 __global__ void __launch_bounds__(NT) sample_level_kernel(
     const __half* __restrict__ logits, int64_t ld_logits, const __half* __restrict__ rand, int64_t ld_rand,
     const int32_t* __restrict__ parent_rows, const int32_t* __restrict__ child_first,
-    const int32_t* __restrict__ n_branch, int k_max, int V, float inv_T, int mode, int64_t* __restrict__ positions,
-    int64_t* __restrict__ tokens, const int32_t* __restrict__ state, const int32_t* __restrict__ drow_base,
-    const int32_t* __restrict__ drow_step, int64_t ld_rand_seq, int64_t ld_seq) {
+    const int32_t* __restrict__ n_branch, int k_max, int V, SeqParam<PER_SEQ> temp, int mode,
+    int64_t* __restrict__ positions, int64_t* __restrict__ tokens, const int32_t* __restrict__ state,
+    const int32_t* __restrict__ drow_base, const int32_t* __restrict__ drow_step, int64_t ld_rand_seq, int64_t ld_seq) {
+  static_assert(BATCH || !PER_SEQ, "per-sequence parameters need the batched kernel");
   __shared__ float red[NW];
   __shared__ uint32_t redu[NW];
   Slice sl{};
@@ -227,6 +229,7 @@ __global__ void __launch_bounds__(NT) sample_level_kernel(
     Pack8 x[CH];
     load_row(logits + lrow * ld_logits, V, x);
     if (mode == 0) {
+      const float inv_T = inv_temp(temp, b);
       float mx, sum;
       if constexpr (WIDE) {
         __shared__ float xs[2][MAX_SLICES];
@@ -540,9 +543,12 @@ __device__ __forceinline__ bool topp_pred(uint32_t S, float tp) { return h2f(f2h
 
 // WIDE: the histograms are summed over the cluster (every CTA then selects the same boundary bins, so all take the same
 // exits), and the boundary tie group is ranked across slices by an exclusive prefix of the per-slice counts in rank order.
-template <bool WIDE>
-__global__ void __launch_bounds__(NT) top_p_filter_kernel(__half* __restrict__ logits, int64_t ld, int V, float inv_T,
-                                                           float tp) {
+// PER_SEQ: `temp` / `top_p` are (B,) arrays and row r belongs to sequence r / rows_per_seq; a row whose top_p >= 1 is left
+// untouched (the whole cluster reads the same value).  Otherwise `temp` is the scalar 1/T and `top_p` fp16(top_p) < 1.
+template <bool WIDE, bool PER_SEQ = false>
+__global__ void __launch_bounds__(NT) top_p_filter_kernel(__half* __restrict__ logits, int64_t ld, int V,
+                                                           SeqParam<PER_SEQ> temp, SeqParam<PER_SEQ> top_p,
+                                                           int rows_per_seq) {
   __shared__ float red[NW];
   __shared__ uint32_t whist[NW][256];
   __shared__ uint32_t hist[256];
@@ -550,13 +556,23 @@ __global__ void __launch_bounds__(NT) top_p_filter_kernel(__half* __restrict__ l
   __shared__ uint32_t wtot[CH][NW];
   Slice sl{};
   __half* row;
+  if constexpr (WIDE || PER_SEQ) pdl_wait();
   if constexpr (WIDE) {
-    pdl_wait();
     sl = slice_of(V);
     row = logits + sl.row * ld + sl.base;
     V = sl.V;
   } else {
     row = logits + blockIdx.x * ld;
+  }
+  float inv_T, tp;
+  if constexpr (PER_SEQ) {
+    const int seq = (WIDE ? sl.row : (int)blockIdx.x) / rows_per_seq;
+    if (top_p[seq] >= 1.0f) return;                  // utils.py:68: only when top_p < 1
+    inv_T = inv_temp(temp, seq);
+    tp = rnd16(top_p[seq]);                          // torch compares in the tensor's dtype (fp16)
+  } else {
+    inv_T = temp;
+    tp = top_p;
   }
   const int nvec = V / 8;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -798,32 +814,56 @@ extern "C" int sq_sample_level(const sq_half* logits, int64_t ld_logits, const s
   return SQ_OK;
 }
 
+// sq_sample_level_batch and its per-sequence form: `temp` is 1/T (PER_SEQ = false) or the (B,) T array
+template <bool PER_SEQ>
+static int sample_level_batch(const char* name, const sq_half* logits, int64_t ld_logits, const int32_t* row_base,
+                              const int32_t* row_step, const sq_half* rand, int64_t ld_rand, int64_t ld_rand_seq,
+                              const int32_t* parent_rows, const int32_t* child_first, const int32_t* n_branch,
+                              int n_parents, int k_max, int V, SeqParam<PER_SEQ> temp, int mode, int64_t* tokens,
+                              int64_t ld_seq, const int32_t* state, int B, void* stream) {
+  SQ_CHECK_V_WIDE(V);
+  SQ_CHECK_ARG(B >= 1 && B <= SQ_MAX_BATCH, "%s: B=%d (1..%d)", name, B, SQ_MAX_BATCH);
+  if (n_parents == 0 || k_max == 0) return SQ_OK;
+  SQ_CHECK_ARG(mode == 1 || rand != nullptr, "%s: rand required for mode 0", name);
+  SQ_CHECK_ARG(tokens && child_first && n_branch && parent_rows && state && row_base && row_step,
+               "%s: null table or buffer", name);
+  SQ_CHECK_ARG(k_max <= V, "%s: k_max > V", name);
+  if (V > SLICE) {
+    SQ_CHECK_ARG(k_max <= WIDE_KMAX, "%s: k_max=%d > %d with V > %d", name, k_max, WIDE_KMAX, SLICE);
+    SQ_CHECK_WIDE_LAUNCH(launch_wide(sample_level_kernel<true, true, PER_SEQ>, n_parents, B, V, (cudaStream_t)stream,
+                                     (const __half*)logits, ld_logits, (const __half*)rand, ld_rand, parent_rows,
+                                     child_first, n_branch, k_max, V, temp, mode, (int64_t*)nullptr, tokens, state,
+                                     row_base, row_step, ld_rand_seq, ld_seq),
+                         name);
+    return SQ_OK;
+  }
+  sample_level_kernel<true, false, PER_SEQ><<<dim3(n_parents, B), NT, 0, (cudaStream_t)stream>>>(
+      (const __half*)logits, ld_logits, (const __half*)rand, ld_rand, parent_rows, child_first, n_branch, k_max, V, temp,
+      mode, nullptr, tokens, state, row_base, row_step, ld_rand_seq, ld_seq);
+  SQ_CHECK_LAUNCH(name);
+  return SQ_OK;
+}
+
 extern "C" int sq_sample_level_batch(const sq_half* logits, int64_t ld_logits, const int32_t* row_base,
                                      const int32_t* row_step, const sq_half* rand, int64_t ld_rand, int64_t ld_rand_seq,
                                      const int32_t* parent_rows, const int32_t* child_first, const int32_t* n_branch,
                                      int n_parents, int k_max, int V, float T, int mode, int64_t* tokens, int64_t ld_seq,
                                      const int32_t* state, int B, void* stream) {
-  SQ_CHECK_V_WIDE(V);
-  SQ_CHECK_ARG(B >= 1 && B <= SQ_MAX_BATCH, "sq_sample_level_batch: B=%d (1..%d)", B, SQ_MAX_BATCH);
-  if (n_parents == 0 || k_max == 0) return SQ_OK;
-  SQ_CHECK_ARG(mode == 1 || rand != nullptr, "sq_sample_level_batch: rand required for mode 0");
-  SQ_CHECK_ARG(tokens && child_first && n_branch && parent_rows && state && row_base && row_step,
-               "sq_sample_level_batch: null table or buffer");
-  SQ_CHECK_ARG(k_max <= V, "sq_sample_level_batch: k_max > V");
-  if (V > SLICE) {
-    SQ_CHECK_ARG(k_max <= WIDE_KMAX, "sq_sample_level_batch: k_max=%d > %d with V > %d", k_max, WIDE_KMAX, SLICE);
-    SQ_CHECK_WIDE_LAUNCH(launch_wide(sample_level_kernel<true, true>, n_parents, B, V, (cudaStream_t)stream,
-                                     (const __half*)logits, ld_logits, (const __half*)rand, ld_rand, parent_rows,
-                                     child_first, n_branch, k_max, V, 1.0f / T, mode, (int64_t*)nullptr, tokens, state,
-                                     row_base, row_step, ld_rand_seq, ld_seq),
-                         "sq_sample_level_batch");
-    return SQ_OK;
-  }
-  sample_level_kernel<true, false><<<dim3(n_parents, B), NT, 0, (cudaStream_t)stream>>>(
-      (const __half*)logits, ld_logits, (const __half*)rand, ld_rand, parent_rows, child_first, n_branch, k_max, V, 1.0f / T,
-      mode, nullptr, tokens, state, row_base, row_step, ld_rand_seq, ld_seq);
-  SQ_CHECK_LAUNCH("sq_sample_level_batch");
-  return SQ_OK;
+  return sample_level_batch<false>("sq_sample_level_batch", logits, ld_logits, row_base, row_step, rand, ld_rand,
+                                   ld_rand_seq, parent_rows, child_first, n_branch, n_parents, k_max, V, 1.0f / T, mode,
+                                   tokens, ld_seq, state, B, stream);
+}
+
+extern "C" int sq_sample_level_batch_per_seq(const sq_half* logits, int64_t ld_logits, const int32_t* row_base,
+                                             const int32_t* row_step, const sq_half* rand, int64_t ld_rand,
+                                             int64_t ld_rand_seq, const int32_t* parent_rows, const int32_t* child_first,
+                                             const int32_t* n_branch, int n_parents, int k_max, int V, const float* T,
+                                             int mode, int64_t* tokens, int64_t ld_seq, const int32_t* state, int B,
+                                             void* stream) {
+  SQ_CHECK_ARG(T != nullptr, "sq_sample_level_batch_per_seq: null temperature array");
+  return sample_level_batch<true>("sq_sample_level_batch_per_seq", logits, ld_logits, row_base, row_step, rand, ld_rand,
+                                  ld_rand_seq, parent_rows, child_first, n_branch, n_parents, k_max, V, T, mode, tokens,
+                                  ld_seq, state, B, stream);
 }
 
 // Sampling with replacement (the SpecInfer policy) has no large-vocabulary instance: V <= 32768 only.
@@ -876,10 +916,27 @@ extern "C" int sq_top_p_filter(sq_half* logits, int64_t ld, int n, int V, float 
   const float tp = __half2float(__float2half_rn(top_p));           // torch compares in the tensor's dtype (fp16)
   if (V > SLICE) {
     SQ_CHECK_WIDE_LAUNCH(launch_wide(top_p_filter_kernel<true>, n, 1, V, (cudaStream_t)stream, (__half*)logits, ld, V,
-                                     1.0f / T, tp), "sq_top_p_filter");
+                                     1.0f / T, tp, 0), "sq_top_p_filter");
     return SQ_OK;
   }
-  top_p_filter_kernel<false><<<n, NT, 0, (cudaStream_t)stream>>>((__half*)logits, ld, V, 1.0f / T, tp);
+  top_p_filter_kernel<false><<<n, NT, 0, (cudaStream_t)stream>>>((__half*)logits, ld, V, 1.0f / T, tp, 0);
   SQ_CHECK_LAUNCH("sq_top_p_filter");
+  return SQ_OK;
+}
+
+extern "C" int sq_top_p_filter_per_seq(sq_half* logits, int64_t ld, int n, int V, const float* top_p, const float* T,
+                                       int rows_per_seq, void* stream) {
+  SQ_CHECK_V_WIDE(V);
+  SQ_CHECK_ARG(top_p != nullptr && T != nullptr, "sq_top_p_filter_per_seq: null top_p or temperature array");
+  SQ_CHECK_ARG(rows_per_seq >= 1 && n >= 0 && n % rows_per_seq == 0,
+               "sq_top_p_filter_per_seq: rows_per_seq=%d does not divide n=%d", rows_per_seq, n);
+  if (n == 0) return SQ_OK;
+  if (V > SLICE) {
+    SQ_CHECK_WIDE_LAUNCH(launch_wide(top_p_filter_kernel<true, true>, n, 1, V, (cudaStream_t)stream, (__half*)logits, ld,
+                                     V, T, top_p, rows_per_seq), "sq_top_p_filter_per_seq");
+    return SQ_OK;
+  }
+  top_p_filter_kernel<false, true><<<n, NT, 0, (cudaStream_t)stream>>>((__half*)logits, ld, V, T, top_p, rows_per_seq);
+  SQ_CHECK_LAUNCH("sq_top_p_filter_per_seq");
   return SQ_OK;
 }

@@ -452,6 +452,51 @@ def accept_stochastic_batch(target_logits, draft_logits, row_base, row_step, r, 
         max_target_seq, policy, stream_ptr()), "sq_accept_stochastic_batch")
 
 
+def _seq_params(name, B, **arrays):
+    for k, t in arrays.items():
+        if t is None or t.dtype != torch.float32 or not t.is_cuda or t.dim() != 1 or t.shape[0] < B or t.stride(0) != 1:
+            raise TypeError(f"{name}: {k} must be a contiguous ({B},) float32 CUDA tensor")
+
+
+def sample_level_batch_per_seq(logits, row_base, row_step, rand, n_parents, k_max, T, mode, *, parent_rows, child_first,
+                               n_branch, tokens, state):
+    """sample_level_batch with the temperature of sequence b read from T[b] ((B,) float32 on the device)."""
+    _seq_params("sample_level_batch_per_seq", state.shape[0], T=T)
+    if rand is not None:
+        assert rand.dim() == 3 and rand.stride(-1) == 1
+    check(_lib.load().sq_sample_level_batch_per_seq(
+        ptr(logits), logits.stride(0), ptr(row_base), ptr(row_step), ptr(rand), rand.stride(1) if rand is not None else 0,
+        rand.stride(0) if rand is not None else 0, ptr(parent_rows), ptr(child_first), ptr(n_branch), n_parents, k_max,
+        logits.shape[-1], ptr(T), mode, ptr(tokens), _rows(tokens, "tokens"), ptr(state), state.shape[0], stream_ptr()),
+        "sq_sample_level_batch_per_seq")
+
+
+def accept_stochastic_batch_per_seq(target_logits, draft_logits, row_base, row_step, r, noise, succ_off, succ, depth, S, T,
+                                    tokens, position_ids, accept_idx, state, max_target_seq, policy=0):
+    """accept_stochastic_batch with the temperature of sequence b read from T[b] ((B,) float32 on the device)."""
+    _seq_params("accept_stochastic_batch_per_seq", state.shape[0], T=T)
+    V = target_logits.shape[-1]
+    ld = _rows(tokens, "tokens")
+    assert _rows(position_ids, "position_ids") == ld and _rows(r, "r") == ld
+    check(_lib.load().sq_accept_stochastic_batch_per_seq(
+        ptr(target_logits), target_logits.stride(0), ptr(draft_logits), draft_logits.stride(0), ptr(row_base),
+        ptr(row_step), ptr(r), ptr(noise), _rows(noise, "noise"), ptr(succ_off), ptr(succ), ptr(depth), S, V, ptr(T),
+        ptr(tokens), ptr(position_ids), ld, ptr(accept_idx), _rows(accept_idx, "accept_idx"), ptr(state), state.shape[0],
+        max_target_seq, policy, stream_ptr()), "sq_accept_stochastic_batch_per_seq")
+
+
+def top_p_filter_per_seq_(logits, top_p, T, rows_per_seq: int):
+    """top_p_filter_ in place on (n, V) fp16 logits whose row r belongs to sequence r // rows_per_seq, at that sequence's
+    top_p[b] and T[b] ((B,) float32 on the device); rows of a sequence with top_p >= 1 are left untouched."""
+    _need(logits, F16, "top_p_filter_per_seq_")
+    n, V = logits.shape
+    B = n // rows_per_seq if rows_per_seq > 0 else 0
+    _seq_params("top_p_filter_per_seq_", B, top_p=top_p, T=T)
+    check(_lib.load().sq_top_p_filter_per_seq(ptr(logits), logits.stride(0), n, V, ptr(top_p), ptr(T), rows_per_seq,
+                                              stream_ptr()), "sq_top_p_filter_per_seq")
+    return logits
+
+
 def accept_greedy_batch(target_token, succ_off, succ, depth, S, tokens, position_ids, accept_idx, state, max_target_seq):
     """target_token (B*S) int64."""
     ld = _rows(tokens, "tokens")

@@ -188,33 +188,95 @@ def simulation_baseline(target, prompts, T, top_p, M, new_tokens: int = 32, stop
     return dict(decoded_tokens=decoded, seconds=total_time, latency=total_time / max(decoded, 1))
 
 
+def decode_refill(tree, prompts, limits, stop=DEFAULT_STOP, step_times=None):
+    """Decode every prompt of a queue on a BatchTree whose B slots start with prompts[:B]: each slot that finishes (a stop
+    token, its length limit `limits[i]`, or out of room) takes the next prompt, until the queue is empty.
+    -> (outputs, decoded tokens, per-sequence target steps, admission order); outputs[i] = prompt i's committed tokens.
+    step_times: a list that receives ("steady" | "admission", seconds) per step; an admission step is timed from the
+    first admit() of the step to the end of its verify."""
+    B = len(tree.frozen)
+    slot = list(range(B))                        # prompt index decoding in each slot (None: the queue ran out)
+    length = [len(p) for p in prompts[:B]]
+    order, pending, nxt = list(range(B)), [], B
+    outputs = [None] * len(prompts)
+    decoded = steps = 0
+    while any(i is not None for i in slot):
+        t0 = time.perf_counter()
+        for b in pending:
+            tree.admit(b, prompts[slot[b]])
+        kind = "admission" if pending else "steady"
+        pending = []
+        tree.construct_grow_map()
+        res = tree.verify()
+        if step_times is not None:
+            step_times.append((kind, time.perf_counter() - t0))
+        for b, (valid, _, terminate) in enumerate(res):
+            i = slot[b]
+            if i is None:
+                continue
+            decoded += valid.shape[0] - length[b]
+            steps += 1
+            length[b] = valid.shape[0]
+            last = int(valid[-1]) if valid.shape[0] else 0
+            # tree.frozen[b] without `terminate`: the tree stopped the slot itself (no room for another tree)
+            if terminate or tree.frozen[b] or last in stop or length[b] >= limits[i]:
+                outputs[i] = valid.clone()           # the slot's token row is reused by the next prompt
+                if not tree.frozen[b]:
+                    tree.freeze(b)
+                if nxt < len(prompts):
+                    slot[b], length[b] = nxt, len(prompts[nxt])
+                    order.append(nxt)
+                    pending.append(b)
+                    nxt += 1
+                else:
+                    slot[b] = None
+    return outputs, decoded, steps, order
+
+
+def decode_chunk(tree, chunk, limits, stop=DEFAULT_STOP):
+    """Decode a BatchTree built on `chunk` until every sequence has finished.  -> (decoded tokens, per-sequence steps)"""
+    length = [len(p) for p in chunk]
+    done = set()
+    decoded = steps = 0
+    while not all(tree.frozen):
+        tree.construct_grow_map()
+        for b, (valid, _, terminate) in enumerate(tree.verify()):
+            if b in done:
+                continue
+            decoded += valid.shape[0] - length[b]
+            steps += 1
+            length[b] = valid.shape[0]
+            last = int(valid[-1]) if valid.shape[0] else 0
+            if terminate or tree.frozen[b] or last in stop or length[b] >= limits[b]:
+                done.add(b)
+                if not tree.frozen[b]:
+                    tree.freeze(b)
+    return decoded, steps
+
+
 @torch.inference_mode()
-def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: int, stop=DEFAULT_STOP):
-    """--batch B: the same metric loop with B prompts decoded together (sequoia_b200.batch.BatchTree)."""
+def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: int, stop=DEFAULT_STOP,
+                     refill: bool = False):
+    """--batch B: the same metric loop with B prompts decoded together (sequoia_b200.batch.BatchTree).  Chunked: B
+    prompts at a time, each chunk until its last sequence stops.  refill: one batch whose finished slots take the next
+    prompt (BatchTree.admit)."""
     from sequoia_b200.batch import BatchTree
     steps = decoded = 0                          # steps: target steps summed over sequences (per-sequence tokens / step)
     total_time = 0.0
-    for i in range(0, len(prompts), B):
-        chunk = [p.to(DEV) for p in prompts[i:i + B]]
+    limits = [MAX_NEW_LEN] * len(prompts)
+    prompts = [p.to(DEV) for p in prompts]
+    chunks = [prompts[:B]] if refill else [prompts[i:i + B] for i in range(0, len(prompts), B)]
+    for chunk in chunks:
         tree = BatchTree(draft, target, chunk, grow_map, policy=policy, temperature=T, top_p=top_p, max_length=M,
                          max_target_seq=M)
-        length = [len(p) for p in chunk]
-        done = set()
         torch.cuda.synchronize()
         t1 = time.time()
-        while not all(tree.frozen):
-            tree.construct_grow_map()
-            for b, (valid, _, terminate) in enumerate(tree.verify()):
-                if b in done:
-                    continue
-                decoded += valid.shape[0] - length[b]
-                steps += 1
-                length[b] = valid.shape[0]
-                last = int(valid[-1]) if valid.shape[0] else 0
-                if terminate or last in stop or length[b] >= MAX_NEW_LEN:
-                    done.add(b)
-                    if not tree.frozen[b]:
-                        tree.freeze(b)
+        if refill:
+            _, d, s, _ = decode_refill(tree, prompts, limits, stop)
+        else:
+            d, s = decode_chunk(tree, chunk, limits[:len(chunk)], stop)
+        decoded += d
+        steps += s
         torch.cuda.synchronize()
         total_time += time.time() - t1
         draft.clear_kv()
@@ -222,9 +284,10 @@ def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: i
     steps = max(steps, 1)
     print("total time :{:.5f}s, latency :{:.5f}s, decoding step: {}, large model step: {}, {}".format(
         total_time, total_time / max(decoded, 1), decoded, steps, decoded / steps))
-    print("batch {}: aggregate {:.2f} tokens/s".format(B, decoded / total_time if total_time > 0 else 0.0))
+    print("batch {}{}: aggregate {:.2f} tokens/s".format(B, " (refill)" if refill else "",
+                                                         decoded / total_time if total_time > 0 else 0.0))
     return dict(decoded_tokens=decoded, target_steps=steps, tokens_per_step=decoded / steps, seconds=total_time,
-                tokens_per_second=decoded / total_time if total_time > 0 else 0.0, batch=B)
+                tokens_per_second=decoded / total_time if total_time > 0 else 0.0, batch=B, refill=refill)
 
 
 def build_parser():
@@ -243,10 +306,26 @@ def build_parser():
     ap.add_argument("--tree", type=str, default="spec", choices=["spec", "greedy", "specinfer", "greedys"])
     ap.add_argument("--offloading", action="store_true", help="use OffloadEngine for the target (weights stay resident)")
     ap.add_argument("--batch", type=int, default=1,
-                    help="decode this many prompts together (--Mode greedy, --tree spec|greedy; the prompt count must divide)")
+                    help="decode this many prompts together (--Mode greedy, --tree spec|greedy; without --refill the "
+                         "prompt count must divide)")
+    ap.add_argument("--refill", action="store_true",
+                    help="with --batch: keep the batch full, each finished slot takes the next prompt of the queue")
     ap.add_argument("--target-weights", type=str, default="fp16", choices=["fp16", "fp8"],
                     help="fp8: the target's layer projections quantized to E4M3 with per-channel scales at load")
     return ap
+
+
+def check_batch_args(args, n_prompts: int) -> int:
+    """Refuse --batch / --refill combinations the batched path does not run; -> the engines' batch size."""
+    if args.Mode != "greedy" or args.tree not in ("spec", "greedy") or args.offloading:
+        raise SystemExit("--batch runs --Mode greedy with --tree spec or greedy, without --offloading")
+    if args.batch < 1 or n_prompts < 1:
+        raise SystemExit(f"--batch {args.batch} with {n_prompts} prompts")
+    if args.refill:
+        return min(args.batch, n_prompts)
+    if n_prompts % args.batch:
+        raise SystemExit(f"--batch {args.batch} must divide the {n_prompts} prompts (or use --refill)")
+    return args.batch
 
 
 def main(argv=None):
@@ -260,20 +339,17 @@ def main(argv=None):
     stop = stop_tokens(args.target)
     if args.target_weights != "fp16" and args.offloading:
         raise SystemExit("--target-weights fp8 runs without --offloading")
-    if args.batch != 1:
-        if args.Mode != "greedy" or args.tree not in ("spec", "greedy") or args.offloading:
-            raise SystemExit("--batch runs --Mode greedy with --tree spec or greedy, without --offloading")
-        if len(prompts) % args.batch:
-            raise SystemExit(f"--batch {args.batch} must divide the {len(prompts)} prompts")
+    if args.batch != 1 or args.refill:
+        B = check_batch_args(args, len(prompts))
         target = GraphInferenceEngineTG(max_length=args.M, model_name_or_path=args.target, dtype=torch.float16,
-                                        device=DEV, batch_size=args.batch, weight_format=args.target_weights)
+                                        device=DEV, batch_size=B, weight_format=args.target_weights)
         draft = GraphInferenceEngine(max_length=args.M, model_name_or_path=args.model, dtype=torch.float16, device=DEV,
-                                     batch_size=args.batch)
+                                     batch_size=B)
         path = args.growmap if os.path.isabs(args.growmap) or os.path.exists(args.growmap) else os.path.join(ROOT, args.growmap)
         grow_map = torch.load(path)
         assert args.M >= MAX_NEW_LEN + grow_map["size"], "--M must hold 256 tokens + the tree (README.md:47 of the reference)"
-        res = simulation_batch(target, draft, prompts, grow_map, args.tree, args.T, args.P, args.M, args.batch,
-                               stop=stop)
+        res = simulation_batch(target, draft, prompts, grow_map, args.tree, args.T, args.P, args.M, B, stop=stop,
+                               refill=args.refill)
         print(json.dumps({k: (round(v, 5) if isinstance(v, float) else v) for k, v in res.items()}))
         return res
     target = (tcls(max_length=args.M, model_name_or_path=args.target, dtype=torch.float16, device=DEV)
