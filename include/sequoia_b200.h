@@ -384,6 +384,37 @@ int sq_accept_greedy_batch(const int64_t* target_token, const int32_t* succ_off,
                            int S, int64_t* tokens, int64_t* position_ids, int64_t ld_seq, int32_t* accept_idx,
                            int64_t ld_acc, int32_t* state, int B, int max_target_seq, void* stream);
 
+/* ---- ragged batches: a forward over a chosen set of the B sequences, each with its own row count ----
+ * A part list names the sequences to run.  Part j is n rows of sequence seq in that sequence's tree-relative addressing:
+ * rows base + n0 + r (r < n), base = state[seq][SQ_ST_P] - 1, attending slots [0, base + kv_end) under the structured tree
+ * mask.  Activation rows are packed in list order: part j starts at row row0_j = sum of n over the parts before it.
+ * parts is a HOST array; each call copies it into its kernel arguments (no device table, no host-to-device copy) and is
+ * one launch for all parts.  Refused with SQ_ERR_INVALID_ARG before any launch: n_parts outside 1..B, a seq outside
+ * [0, B) or listed twice, n < 1, more rows in all than n_max (the activation buffer's rows, or the plan's), and
+ * tree_words > 32.  The list is the selection: SQ_ST_FROZEN is not read, and nothing of an unlisted sequence (tokens,
+ * state, KV bytes) is read or written by embed / RoPE + KV append; attention reads only the listed sequences' cache
+ * planes.  A single part at B = 1 computes bit for bit what the corresponding _batch call computes. */
+typedef struct {
+  int32_t seq, n, n0, kv_end;
+} sq_ragged_part;
+/* the packed layout of a part list: row0[j] / tile0[j] (host arrays of n_parts + 1 entries, either may be NULL) = rows /
+ * q tiles of rows_per_tile rows before part j; the same checks as the calls below */
+int sq_ragged_layout(const sq_ragged_part* parts, int n_parts, int B, int n_max, int rows_per_tile, int32_t* row0,
+                     int32_t* tile0);
+/* out: n_max rows of hidden halfs */
+int sq_embed_rows_ragged(const sq_half* table, const int64_t* tokens, int64_t ld_seq, const int32_t* state,
+                         const sq_ragged_part* parts, int n_parts, int B, int n_max, int hidden, sq_half* out,
+                         void* stream);
+/* qkv: n_max rows; k_layer / v_layer: (B, Hkv, M, D) of this layer */
+int sq_rope_kv_append_ragged(sq_half* qkv, int ld, int H, int Hkv, int D, const sq_half* cos, const sq_half* sin,
+                             const int64_t* position_ids, const int64_t* storage_ids, int64_t ld_seq,
+                             const int32_t* state, const sq_ragged_part* parts, int n_parts, int B, int n_max,
+                             sq_half* k_layer, sq_half* v_layer, int M, void* stream);
+/* on a plan made by sq_attn_plan_create_batch (its B and n_max); the KV split count is chosen once for the launch from all
+ * parts' q tiles (SQ_ATTN_SPLITS forces it, sq_attn_plan_info reports it) */
+int sq_tree_attn_ragged(sq_attn_plan* plan, int layer, const sq_ragged_part* parts, int n_parts, const int32_t* state,
+                        const uint32_t* tree_bits, int tree_words, int tree_size, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -136,8 +136,7 @@ class BatchTree:
         for b, p in enumerate(prompts):
             self._load_prompt(b, p)
         with torch.inference_mode():
-            for b in range(B):
-                self._prefill(b)
+            self.op_draft_prefill(range(B))
 
     # ---- helpers ---------------------------------------------------------------------------------------------------------
     def _mask_kw(self):
@@ -157,24 +156,12 @@ class BatchTree:
         self.state[b].copy_(_h2d(st0), non_blocking=True)
         self.accept_idx[b].zero_()
 
-    def _prefill(self, b: int):
-        """Draft prefill of sequence b (SpecTree.py:67-80): rows [0, P) causal, the last row's logits -> node 0."""
-        P = self.ground_truth_len[b]
-        self._alone(b, lambda: self.draft.engine.runner.forward(
-            P, self.tokens, self.position_ids, self.storage_ids, state=self.state, n0=1 - P, kv_end=1, batch=True,
-            logits_from=b * P + P - 1, logits_to=b * P + P, logits_out=self.draft_logits[b:b + 1], **self._mask_kw()))
-
-    def _alone(self, b: int, fn):
-        """Run a batched op sequence for sequence b only (prefill and first verify, whose row count depends on the
-        prompt): every other sequence gets a frozen copy of b's state row, so its kernels write nothing of it and read
-        exactly the cache range b reads; the state rows are restored afterwards."""
-        saved = self.state.clone()
-        tmp = saved[b:b + 1].repeat(self.B, 1)
-        tmp[:, ST_FROZEN] = 1
-        tmp[b] = saved[b]
-        self.state.copy_(tmp)
-        fn()
-        self.state.copy_(saved)
+    def op_draft_prefill(self, seqs):
+        """Draft prefill of the sequences `seqs` (SpecTree.py:67-80) as one ragged forward: each one's rows [0, P) causal,
+        its last row's logits -> its node 0."""
+        self.draft.engine.runner.forward_ragged(
+            [(b, self.ground_truth_len[b], 1 - self.ground_truth_len[b], 1, 1, self.draft_logits[b:b + 1]) for b in seqs],
+            self.tokens, self.position_ids, self.storage_ids, state=self.state, **self._mask_kw())
 
     def freeze(self, b: int):
         """Stop sequence b (the caller's length limit); it stays frozen until admit() gives the slot a new prompt."""
@@ -212,7 +199,7 @@ class BatchTree:
             r, rand = draw_random([prompt], self.M, self.S, self.V)
             self.r[b].copy_(_h2d(r[0]), non_blocking=True)
             self.rand[b].copy_(_h2d(rand[0]), non_blocking=True)
-        self._prefill(b)
+        self.op_draft_prefill([b])
 
     # ---- the op sequences ------------------------------------------------------------------------------------------------
     def op_sample(self, i: int):
@@ -233,14 +220,13 @@ class BatchTree:
                                           n0=0, kv_end=self.S, batch=True, logits_out=self.target_logits,
                                           **self._mask_kw())
 
-    def op_target_first(self, b: int):
-        """First verify of sequence b (SpecTree.py:164-176): rows [0, P+S-1), logits of the S tree rows."""
-        P, S = self.ground_truth_len[b], self.S
-        n = P + S - 1
-        self._alone(b, lambda: self.target.engine.runner.forward(
-            n, self.tokens, self.position_ids, self.storage_ids, state=self.state, n0=1 - P, kv_end=S, batch=True,
-            logits_from=b * n + n - S, logits_to=b * n + n, logits_out=self.target_logits[b * S:(b + 1) * S],
-            **self._mask_kw()))
+    def op_target_first(self, seqs):
+        """First verify of the sequences `seqs` (SpecTree.py:164-176) as one ragged forward: each one's rows [0, P+S-1),
+        the logits of its S tree rows."""
+        S = self.S
+        self.target.engine.runner.forward_ragged(
+            [(b, self.ground_truth_len[b] + S - 1, 1 - self.ground_truth_len[b], S, S,
+              self.target_logits[b * S:(b + 1) * S]) for b in seqs], self.tokens, self.position_ids, self.storage_ids, state=self.state, **self._mask_kw())
 
     def op_accept(self):
         st = self.st
@@ -348,10 +334,9 @@ class BatchTree:
                     self.state[b, ST_FROZEN] = 1
                 self.op_target_steady()
                 self.state.copy_(saved)
-            # prefill + tree rows of each first-verify sequence eagerly (their row counts differ); the walk and the rest
-            # batched
-            for b in first:
-                self.op_target_first(b)
+            # prefill + tree rows of every first-verify sequence in one ragged forward (their row counts differ); the walk
+            # and the rest batched
+            self.op_target_first(first)
             self.run("post", self.seq_post)
         else:
             self.run("steady", self.seq_steady)

@@ -185,20 +185,31 @@ constexpr float RESCALE_THRESHOLD = 8.0f;   // log2 units: P stays <= 2^8 under 
 // 64-column chunk the columns 8 j + 2 (lane % 4) + {0, 1}: element [4 j + 2 h + e] is (row r0 + 8 h, column 8 j + 2 q + e).
 // BATCH (structured mask only): grid.y = B * q tiles, sequence b = blockIdx.y / q tiles reads its own state row, its Q rows
 // and writes its output rows at offset b*n, and reads cache heads (layer*B + b)*Hkv + h.
-template <int D, bool DENSE, bool BATCH>
+// RAGGED (structured mask only): grid.y = the q tiles of all parts; the CTA's part j is found from the q-tile prefix
+// sums, n / n0 / kv_end are part j's, its Q rows and output rows start at row0_j, and it reads cache heads
+// (layer*B + seq)*Hkv + h.
+// The Q box of a part's last tile may cover the next part's rows: those rows are never written.
+template <int D, bool DENSE, bool BATCH, bool RAGGED = false>
 __global__ void __launch_bounds__(256, 1)
     tree_attn_tc_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_k,
-                        const __grid_constant__ CUtensorMap tm_v, AttnArgs a) {
+                        const __grid_constant__ CUtensorMap tm_v, AttnArgs a,
+                        const __grid_constant__ RaggedArg<RAGGED> rp) {
   using SM = TcSmem<D>;
   constexpr int DC = D / 64;                     // 64-column chunks of O
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // dynamic smem base is only guaranteed 16 B aligned: re-align to 1024 B for SWIZZLE_128B (same offset in every CTA)
   uint8_t* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
+  constexpr bool SEQ = BATCH || RAGGED;          // per-sequence state row and cache planes
+  const RaggedParts* R = ragged_ptr(rp);
+  const int pj = RAGGED ? ragged_part(R->tile0, R->n_parts, blockIdx.y) : 0;   // RAGGED: this CTA's part
+#define SQ_PART(f) (RAGGED ? R->f[pj] : a.f)
   const int q_tiles = BATCH ? (int)gridDim.y / a.B : (int)gridDim.y;
-  const int b = BATCH ? (int)blockIdx.y / q_tiles : 0;
-  const int grp = blockIdx.x, qt = BATCH ? (int)blockIdx.y % q_tiles : (int)blockIdx.y, split = blockIdx.z, Z = gridDim.z;
-  const int32_t* state = BATCH ? a.state + b * ST_WORDS : a.state;
-  __half* out = BATCH ? a.out + (int64_t)b * a.n * (a.H * D) : a.out;
+  const int b = RAGGED ? R->seq[pj] : BATCH ? (int)blockIdx.y / q_tiles : 0;
+  const int grp = blockIdx.x, split = blockIdx.z, Z = gridDim.z;
+  const int qt = RAGGED ? (int)blockIdx.y - R->tile0[pj] : BATCH ? (int)blockIdx.y % q_tiles : (int)blockIdx.y;
+  const int32_t* state = SEQ ? a.state + b * ST_WORDS : a.state;
+  __half* out = RAGGED  ? a.out + (int64_t)R->row0[pj] * (a.H * D)
+                : BATCH ? a.out + (int64_t)b * a.n * (a.H * D) : a.out;
   const int GP = a.GP, RPT = TILE_Q / GP;        // heads per tile, query rows per tile
   const int hkv = (grp * GP) / (a.H / a.Hkv);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -230,11 +241,12 @@ __global__ void __launch_bounds__(256, 1)
   if (tid == 0) {
     ptx::mbar_expect_tx(bar_q, SM::TILE_BYTES);
 #pragma unroll
-    for (int hh = 0; hh < SM::HALVES; ++hh) ptx::tma_load_3d(sQ + hh * 16384, &tm_q, bar_q, hh * 64, grp * GP, b * a.n + q0);
+    for (int hh = 0; hh < SM::HALVES; ++hh)
+      ptx::tma_load_3d(sQ + hh * 16384, &tm_q, bar_q, hh * 64, grp * GP, RAGGED ? R->row0[pj] + q0 : b * a.n + q0);
   }
   uint32_t* sbits = reinterpret_cast<uint32_t*>(smem + SM::OFF_MASK);
   if (!DENSE && a.tree_words > 0 && tid < RPT) {
-    const int node = state ? (a.n0 + q0 + tid) : (a.n0 + q0 + tid - (a.prefix_len_host - 1));
+    const int node = state ? (SQ_PART(n0) + q0 + tid) : (a.n0 + q0 + tid - (a.prefix_len_host - 1));
     const bool has = node >= 1 && node < a.tree_size;
 #pragma unroll 4
     for (int w = 0; w < a.tree_words; ++w)
@@ -242,11 +254,11 @@ __global__ void __launch_bounds__(256, 1)
   }
   const int P = state ? state[ST_P] : a.prefix_len_host;
   const int base = state ? (P - 1) : 0;
-  const int kv_len = base + a.kv_end;
+  const int kv_len = base + SQ_PART(kv_end);
   // active KV tiles of this q tile (tiles wholly beyond what its last row may see are never touched), split in chunks
   int T;
   {
-    const int last_slot = base + a.n0 + min(q0 + RPT, a.n) - 1;
+    const int last_slot = base + SQ_PART(n0) + min(q0 + RPT, SQ_PART(n)) - 1;
     const int max_vis = DENSE ? (kv_len - 1) : ((last_slot >= P) ? (kv_len - 1) : min(last_slot, P - 1));
     T = min((kv_len + TILE_KV - 1) / TILE_KV, max_vis / TILE_KV + 1);
   }
@@ -254,7 +266,7 @@ __global__ void __launch_bounds__(256, 1)
   const int nsplit = (T + tps - 1) / tps;        // splits that own at least one tile
   const int t_begin = split * tps;
   const int NT = max(0, min(T, t_begin + tps) - t_begin);
-  const int kvrow = (BATCH ? a.layer * a.B + b : a.layer) * a.Hkv + hkv;
+  const int kvrow = (SEQ ? a.layer * a.B + b : a.layer) * a.Hkv + hkv;
   SQ_STAMP(0);
 
   if (NT > 0) {
@@ -276,9 +288,9 @@ __global__ void __launch_bounds__(256, 1)
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int qr = (r0 + 8 * h) / GP;          // query row inside the tile
-      rm[h] = row_mask(base + a.n0 + q0 + qr, P);
+      rm[h] = row_mask(base + SQ_PART(n0) + q0 + qr, P);
       my_bits[h] = sbits + qr * a.tree_words;
-      row_ok[h] = (q0 + qr) < a.n;
+      row_ok[h] = (q0 + qr) < SQ_PART(n);
     }
     __syncthreads();                             // ancestor bits staged, barriers initialised
     SQ_STAMP(1);
@@ -427,7 +439,7 @@ __global__ void __launch_bounds__(256, 1)
 #pragma unroll 4
       for (int rr = warp * RPW + sub; rr < TILE_Q; rr += 8 * RPW) {
         const int qrow = q0 + rr / GP;
-        if (qrow < a.n)
+        if (qrow < SQ_PART(n))
           *reinterpret_cast<uint4*>(out + (int64_t)qrow * (a.H * D) + (grp * GP + rr % GP) * D + cc * 8) =
               *reinterpret_cast<const uint4*>(sO + rr * SM::O_STRIDE + cc * 8);
       }
@@ -490,7 +502,7 @@ __global__ void __launch_bounds__(256, 1)
       const int lr = i / CPR, cc = i % CPR;
       const int rr = lr * Z + split;             // tile row owned by this CTA
       const int qrow = q0 + rr / GP;
-      if (rr >= TILE_Q || qrow >= a.n) continue;
+      if (rr >= TILE_Q || qrow >= SQ_PART(n)) continue;
       const float4 w0 = *reinterpret_cast<const float4*>(wts + lr * 8), w1 = *reinterpret_cast<const float4*>(wts + lr * 8 + 4);
       const float w[8] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
       Pack8 o[8];
@@ -510,6 +522,7 @@ __global__ void __launch_bounds__(256, 1)
     }
   }
   SQ_STAMP(8);
+#undef SQ_PART
 }
 
 }  // namespace sq
@@ -632,15 +645,17 @@ extern "C" int sq_attn_plan_error(sq_attn_plan* plan) {
   return v;
 }
 
-template <int D, bool BATCH>
-static int launch_attn(sq_attn_plan* p, AttnArgs& a, int impl, cudaStream_t st) {
+template <int D, bool BATCH, bool RAGGED = false>
+static int launch_attn(sq_attn_plan* p, AttnArgs& a, int impl, cudaStream_t st, const RaggedArg<RAGGED>& rp = {}) {
   if (impl == 1) {
     tree_attn_simt_kernel<D><<<dim3(a.n, a.H), 128, 0, st>>>(a);
     SQ_CHECK_LAUNCH("sq_tree_attn(simt)");
     return SQ_OK;
   }
   constexpr int smem = TcSmem<D>::TOTAL + 1024;
-  auto kern = BATCH ? tree_attn_tc_kernel<D, false, true>
+  decltype(&tree_attn_tc_kernel<D, false, false, RAGGED>) kern;
+  if constexpr (RAGGED) kern = tree_attn_tc_kernel<D, false, false, true>;
+  else kern = BATCH ? tree_attn_tc_kernel<D, false, true>
                     : (a.dense_mask ? tree_attn_tc_kernel<D, true, false> : tree_attn_tc_kernel<D, false, false>);
   static bool attr_set[2] = {false, false};    // (a process drives one device: bench / tests / torchrun ranks)
   if (!attr_set[a.dense_mask ? 1 : 0]) {
@@ -649,7 +664,10 @@ static int launch_attn(sq_attn_plan* p, AttnArgs& a, int impl, cudaStream_t st) 
     attr_set[a.dense_mask ? 1 : 0] = true;
   }
   const int RPT = TILE_Q / p->GP;
-  const int q_tiles = (a.n + RPT - 1) / RPT;
+  // a ragged launch has one y block per q tile of every part; the others q_tiles per sequence, B sequences
+  int q_tiles;
+  if constexpr (RAGGED) q_tiles = rp.tile0[rp.n_parts];
+  else q_tiles = (a.n + RPT - 1) / RPT;
   const int groups = a.H / p->GP;
   // KV splits per cluster: as many as it takes to put a CTA on every SM, never more than the KV tiles the cache can hold
   // (graph-static launches read the length from the device) or that this call touches (host-known kv_end)
@@ -659,13 +677,14 @@ static int launch_attn(sq_attn_plan* p, AttnArgs& a, int impl, cudaStream_t st) 
     cudaGetDevice(&dev);
     if (cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n_sm <= 0) n_sm = 132;
   }
-  int Z = p->splits_force > 0 ? p->splits_force : n_sm / std::max(1, groups * q_tiles * a.B);
+  const int seqs = RAGGED ? 1 : a.B;
+  int Z = p->splits_force > 0 ? p->splits_force : n_sm / std::max(1, groups * q_tiles * seqs);
   Z = std::max(1, std::min(8, Z));
   Z = std::min(Z, p->splits_max);
   if (a.state == nullptr) Z = std::max(1, std::min(Z, (a.kv_end + TILE_KV - 1) / TILE_KV));
   p->last_splits = Z;
   cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(groups, q_tiles * a.B, Z);
+  cfg.gridDim = dim3(groups, q_tiles * seqs, Z);
   cfg.blockDim = dim3(256);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = st;
@@ -681,7 +700,7 @@ static int launch_attn(sq_attn_plan* p, AttnArgs& a, int impl, cudaStream_t st) 
     attr[1].val.programmaticStreamSerializationAllowed = 1;
     cfg.numAttrs = 2;
   }
-  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, p->tm_q, p->tm_k, p->tm_v, a);
+  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, p->tm_q, p->tm_k, p->tm_v, a, rp);
   if (e != cudaSuccess) { set_error("sq_tree_attn(tc): launch failed: %s", cudaGetErrorString(e)); return SQ_ERR_CUDA; }
   SQ_CHECK_LAUNCH("sq_tree_attn(tc)");
   return SQ_OK;
@@ -734,4 +753,27 @@ extern "C" int sq_tree_attn_batch(sq_attn_plan* plan, int layer, int n, int B, c
   cudaStream_t st = (cudaStream_t)stream;
   if (plan->D == 64) return launch_attn<64, true>(plan, a, 0, st);
   return launch_attn<128, true>(plan, a, 0, st);
+}
+
+extern "C" int sq_tree_attn_ragged(sq_attn_plan* plan, int layer, const sq_ragged_part* parts, int n_parts,
+                                   const int32_t* state, const uint32_t* tree_bits, int tree_words, int tree_size,
+                                   void* stream) {
+  SQ_CHECK_ARG(plan != nullptr, "sq_tree_attn_ragged: null plan");
+  SQ_CHECK_ARG(layer >= 0 && layer < plan->L, "sq_tree_attn_ragged: bad layer %d", layer);
+  SQ_CHECK_ARG(tree_words <= 32, "sq_tree_attn_ragged: tree_size > 1024 unsupported (32 mask words per row)");
+  SQ_CHECK_ARG(state != nullptr, "sq_tree_attn_ragged: needs the state array");
+  RaggedParts rp;
+  const int rc = make_ragged(parts, n_parts, plan->B, plan->n_max, TILE_Q / plan->GP, "sq_tree_attn_ragged", &rp);
+  if (rc != SQ_OK) return rc;
+  AttnArgs a{};
+  a.q = plan->q; a.ld = plan->ld;
+  a.out = plan->out;
+  a.n = 0; a.H = plan->H; a.Hkv = plan->Hkv; a.M = plan->M; a.GP = plan->GP; a.B = plan->B; a.layer = layer;
+  a.state = state; a.prefix_len_host = 0;
+  a.tree_bits = tree_bits; a.tree_words = tree_bits ? tree_words : 0; a.tree_size = tree_bits ? tree_size : 0;
+  a.scale = 1.0f / sqrtf((float)plan->D);
+  a.debug_flags = plan->debug_flags; a.err_flag = plan->err_flag; a.dbg = plan->dbg;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (plan->D == 64) return launch_attn<64, false, true>(plan, a, 0, st, rp);
+  return launch_attn<128, false, true>(plan, a, 0, st, rp);
 }

@@ -82,6 +82,33 @@ using SeqParam = typename std::conditional<PER_SEQ, const float*, float>::type;
 __device__ __forceinline__ float inv_temp(float inv_T, int) { return inv_T; }
 __device__ __forceinline__ float inv_temp(const float* T, int b) { return 1.0f / T[b]; }
 
+// Ragged launches (RAGGED = true): a by-value kernel argument holding the part list (sq_ragged_part, in list order) and
+// its prefix sums.  row0[j] = sum of n over parts < j (row0[n_parts] = all rows); tile0[j] the same over q tiles of
+// rows_per_tile rows (attention).  RAGGED = false instances take a plain int in its place, so they compile as before.
+struct RaggedParts {
+  int n_parts;
+  int seq[SQ_MAX_BATCH], n[SQ_MAX_BATCH], n0[SQ_MAX_BATCH], kv_end[SQ_MAX_BATCH];
+  int row0[SQ_MAX_BATCH + 1], tile0[SQ_MAX_BATCH + 1];
+};
+template <bool RAGGED>
+using RaggedArg = typename std::conditional<RAGGED, RaggedParts, int>::type;
+
+// Validates a host part list against B sequences and n_max activation rows, and fills `out` (prefix sums over tiles of
+// rows_per_tile rows).  SQ_ERR_INVALID_ARG with a message naming `who` on any bad part.
+int make_ragged(const sq_ragged_part* parts, int n_parts, int B, int n_max, int rows_per_tile, const char* who,
+                RaggedParts* out);
+
+// the part list of a RAGGED instance; nullptr for the placeholder (never dereferenced: RAGGED = false)
+__device__ __forceinline__ const RaggedParts* ragged_ptr(const RaggedParts& rp) { return &rp; }
+__device__ __forceinline__ const RaggedParts* ragged_ptr(int) { return nullptr; }
+
+// the part whose [prefix[j], prefix[j+1]) holds x (at most SQ_MAX_BATCH steps)
+__device__ __forceinline__ int ragged_part(const int* prefix, int n_parts, int x) {
+  int j = 0;
+  while (j + 1 < n_parts && x >= prefix[j + 1]) ++j;
+  return j;
+}
+
 __device__ __forceinline__ int row_base(const int32_t* P_ptr, int n0) {
   return (P_ptr ? (P_ptr[ST_P] - 1) : 0) + n0;
 }

@@ -6,23 +6,28 @@
 namespace sq {
 
 // ---------------------------------------------------------------------------------------------
-// grid (n, B): sequence b's rows go to out rows [b*n, b*n + n); a frozen sequence's rows are left as they are
-template <bool BATCH>
+// grid (n, B): sequence b's rows go to out rows [b*n, b*n + n); a frozen sequence's rows are left as they are.
+// RAGGED: grid (sum of n); out row x belongs to the part whose row range holds it and is that part's row x - row0, of
+// sequence seq at its own n0 (the frozen word is not read).
+template <bool BATCH, bool RAGGED = false>
 __global__ void embed_rows_kernel(const __half* __restrict__ table, const int64_t* __restrict__ tokens, int64_t ld_seq,
-                                  const int32_t* __restrict__ state, int n0, int hidden, __half* __restrict__ out) {
+                                  const int32_t* __restrict__ state, int n0, int hidden, __half* __restrict__ out,
+                                  const __grid_constant__ RaggedArg<RAGGED> rp) {
   pdl_wait();
   pdl_trigger();
-  const int b = seq_index<BATCH>(blockIdx.y);
-  if (BATCH) {
+  const RaggedParts* R = ragged_ptr(rp);
+  const int pj = RAGGED ? ragged_part(R->row0, R->n_parts, blockIdx.x) : 0;   // RAGGED: this CTA's part
+  const int b = RAGGED ? R->seq[pj] : seq_index<BATCH>(blockIdx.y);
+  if (BATCH || RAGGED) {
     state += b * ST_WORDS;
-    if (state[ST_FROZEN]) return;          // its P may leave no room for n rows in tokens
+    if (BATCH && state[ST_FROZEN]) return;          // its P may leave no room for n rows in tokens
     tokens += b * ld_seq;
   }
-  const int r = blockIdx.x;
-  const int base = row_base(state, n0);
+  const int r = RAGGED ? (int)blockIdx.x - R->row0[pj] : blockIdx.x;
+  const int base = row_base(state, RAGGED ? R->n0[pj] : n0);
   const int64_t tok = tokens[base + r];
   const uint4* src = reinterpret_cast<const uint4*>(table + tok * (int64_t)hidden);
-  uint4* dst = reinterpret_cast<uint4*>(out + ((int64_t)b * gridDim.x + r) * hidden);
+  uint4* dst = reinterpret_cast<uint4*>(out + (RAGGED ? (int64_t)blockIdx.x : (int64_t)b * gridDim.x + r) * hidden);
   for (int i = threadIdx.x; i < hidden / 8; i += blockDim.x) dst[i] = src[i];
 }
 
@@ -116,31 +121,34 @@ __global__ void silu_mul_kernel(const __half* __restrict__ gu, __half* __restric
 // One CTA (256 threads) per row.  Work items: for every q/k head and every 16-byte chunk c of the first half of the
 // head, rotate the pair (chunk c, chunk c + D/16) -> two 16-byte loads, two stores; then copy the V heads.
 // grid (n, B): sequence b's rows are qkv rows [b*n, b*n + n), its cache planes k_layer + b*Hkv*M*D (a (B, Hkv, M, D)
-// layer); a frozen sequence writes nothing.
-template <bool BATCH>
+// layer); a frozen sequence writes nothing.  RAGGED: grid (sum of n), qkv row x is row x - row0 of the part holding it,
+// addressed in sequence seq's ids, state row and cache planes as the BATCH instance addresses sequence b.
+template <bool BATCH, bool RAGGED = false>
 __global__ void __launch_bounds__(256) rope_kv_append_kernel(
     __half* __restrict__ qkv, int ld, int H, int Hkv, int D, const __half* __restrict__ cosc,
     const __half* __restrict__ sinc, const int64_t* __restrict__ position_ids, const int64_t* __restrict__ storage_ids,
     int64_t ld_seq, const int32_t* __restrict__ state, int n0, __half* __restrict__ k_layer, __half* __restrict__ v_layer,
-    int M) {
+    int M, const __grid_constant__ RaggedArg<RAGGED> rp) {
   // under programmatic dependent launch: wait for the qkv GEMM, then let the attention launch start its prologue (it
   // waits for this grid's completion itself)
   pdl_wait();
   pdl_trigger();
-  const int b = seq_index<BATCH>(blockIdx.y);
-  if (BATCH) {
+  const RaggedParts* R = ragged_ptr(rp);
+  const int pj = RAGGED ? ragged_part(R->row0, R->n_parts, blockIdx.x) : 0;   // RAGGED: this CTA's part
+  const int b = RAGGED ? R->seq[pj] : seq_index<BATCH>(blockIdx.y);
+  if (BATCH || RAGGED) {
     state += b * ST_WORDS;
-    if (state[ST_FROZEN]) return;
+    if (BATCH && state[ST_FROZEN]) return;
     position_ids += b * ld_seq;
     storage_ids += b * ld_seq;
     k_layer += (int64_t)b * Hkv * M * D;
     v_layer += (int64_t)b * Hkv * M * D;
   }
-  const int r = blockIdx.x;
-  const int base = row_base(state, n0);
+  const int r = RAGGED ? (int)blockIdx.x - R->row0[pj] : blockIdx.x;
+  const int base = row_base(state, RAGGED ? R->n0[pj] : n0);
   const int64_t pos = position_ids[base + r];
   const int64_t slot = storage_ids[base + r];
-  __half* row = qkv + ((int64_t)b * gridDim.x + r) * ld;
+  __half* row = qkv + (RAGGED ? (int64_t)blockIdx.x : (int64_t)b * gridDim.x + r) * ld;
   const int cph = D / 16;                                   // chunk pairs per head
   const uint4* cs = reinterpret_cast<const uint4*>(cosc + pos * D);
   const uint4* sn = reinterpret_cast<const uint4*>(sinc + pos * D);
@@ -179,8 +187,22 @@ extern "C" int sq_embed_rows(const sq_half* table, const int64_t* tokens, const 
   SQ_CHECK_ARG(hidden % 8 == 0 && n >= 0, "sq_embed_rows: hidden %% 8 != 0");
   if (n == 0) return SQ_OK;
   launch_k(embed_rows_kernel<false>, dim3(n), dim3(128), 0, (cudaStream_t)stream, (const __half*)table, tokens, (int64_t)0,
-           state, n0, hidden, (__half*)out);
+           state, n0, hidden, (__half*)out, 0);
   SQ_CHECK_LAUNCH("sq_embed_rows");
+  return SQ_OK;
+}
+
+extern "C" int sq_embed_rows_ragged(const sq_half* table, const int64_t* tokens, int64_t ld_seq, const int32_t* state,
+                                    const sq_ragged_part* parts, int n_parts, int B, int n_max, int hidden, sq_half* out,
+                                    void* stream) {
+  SQ_CHECK_ARG(hidden % 8 == 0, "sq_embed_rows_ragged: hidden %% 8 != 0");
+  SQ_CHECK_ARG(state != nullptr, "sq_embed_rows_ragged: needs the state array");
+  RaggedParts rp;
+  const int rc = make_ragged(parts, n_parts, B, n_max, 1, "sq_embed_rows_ragged", &rp);
+  if (rc != SQ_OK) return rc;
+  launch_k(embed_rows_kernel<false, true>, dim3(rp.row0[n_parts]), dim3(128), 0, (cudaStream_t)stream,
+           (const __half*)table, tokens, ld_seq, state, 0, hidden, (__half*)out, rp);
+  SQ_CHECK_LAUNCH("sq_embed_rows_ragged");
   return SQ_OK;
 }
 
@@ -191,7 +213,7 @@ extern "C" int sq_embed_rows_batch(const sq_half* table, const int64_t* tokens, 
                SQ_MAX_BATCH);
   if (n == 0) return SQ_OK;
   launch_k(embed_rows_kernel<true>, dim3(n, B), dim3(128), 0, (cudaStream_t)stream, (const __half*)table, tokens, ld_seq,
-           state, n0, hidden, (__half*)out);
+           state, n0, hidden, (__half*)out, 0);
   SQ_CHECK_LAUNCH("sq_embed_rows_batch");
   return SQ_OK;
 }
@@ -245,7 +267,7 @@ extern "C" int sq_rope_kv_append(sq_half* qkv, int ld, int H, int Hkv, int D, co
   if (n == 0) return SQ_OK;
   launch_k(rope_kv_append_kernel<false>, dim3(n), dim3(256), 0, (cudaStream_t)stream, (__half*)qkv, ld, H, Hkv, D,
            (const __half*)cos, (const __half*)sin, position_ids, storage_ids, (int64_t)0, state, n0, (__half*)k_layer,
-           (__half*)v_layer, M);
+           (__half*)v_layer, M, 0);
   SQ_CHECK_LAUNCH("sq_rope_kv_append");
   return SQ_OK;
 }
@@ -261,7 +283,24 @@ extern "C" int sq_rope_kv_append_batch(sq_half* qkv, int ld, int H, int Hkv, int
   if (n == 0) return SQ_OK;
   launch_k(rope_kv_append_kernel<true>, dim3(n, B), dim3(256), 0, (cudaStream_t)stream, (__half*)qkv, ld, H, Hkv, D,
            (const __half*)cos, (const __half*)sin, position_ids, storage_ids, ld_seq, state, n0, (__half*)k_layer,
-           (__half*)v_layer, M);
+           (__half*)v_layer, M, 0);
   SQ_CHECK_LAUNCH("sq_rope_kv_append_batch");
+  return SQ_OK;
+}
+
+extern "C" int sq_rope_kv_append_ragged(sq_half* qkv, int ld, int H, int Hkv, int D, const sq_half* cos,
+                                        const sq_half* sin, const int64_t* position_ids, const int64_t* storage_ids, int64_t ld_seq,
+                                        const int32_t* state, const sq_ragged_part* parts, int n_parts, int B, int n_max,
+                                        sq_half* k_layer, sq_half* v_layer, int M, void* stream) {
+  SQ_CHECK_ARG(D % 16 == 0 && ld % 8 == 0, "sq_rope_kv_append_ragged: head dim %d / pitch %d must be multiples of 16 / 8",
+               D, ld);
+  SQ_CHECK_ARG(state != nullptr, "sq_rope_kv_append_ragged: needs the state array");
+  RaggedParts rp;
+  const int rc = make_ragged(parts, n_parts, B, n_max, 1, "sq_rope_kv_append_ragged", &rp);
+  if (rc != SQ_OK) return rc;
+  launch_k(rope_kv_append_kernel<false, true>, dim3(rp.row0[n_parts]), dim3(256), 0, (cudaStream_t)stream, (__half*)qkv,
+           ld, H, Hkv, D, (const __half*)cos, (const __half*)sin, position_ids, storage_ids, ld_seq, state, 0,
+           (__half*)k_layer, (__half*)v_layer, M, rp);
+  SQ_CHECK_LAUNCH("sq_rope_kv_append_ragged");
   return SQ_OK;
 }

@@ -395,25 +395,65 @@ class LlamaRunner:
             ops.embed_rows_batch(self.embed, tokens, n, self.hidden, state, n0=n0)
         else:
             ops.embed_rows(self.embed, tokens, n, self.hidden, state=state, n0=n0)
-        n_seq, n = n, N                                # from here on n counts the rows of all sequences
-        ops.rmsnorm(self.hidden, self.layers[0]["ln1"], self.normed, n, self.eps)
-        for l, ly in enumerate(self.layers):
-            self._project(ly, "wqkv", self.normed, n, self.qkv)
+        n_seq = n
+
+        def attend(l):
             if batch:
                 ops.rope_kv_append_batch(self.qkv, H, Hkv, D, self.cos, self.sin, position_ids, storage_ids, n_seq,
                                          self.k_cache[l], self.v_cache[l], M, state, n0=n0)
                 ops.tree_attn_batch(self.plan, l, n_seq, state=state, n0=n0, kv_end=kv_end, tree_bits=tree_bits,
                                     tree_words=tree_words, tree_size=tree_size)
+                return
+            ops.rope_kv_append(self.qkv, H, Hkv, D, self.cos, self.sin, position_ids, storage_ids, n, self.k_cache[l],
+                               self.v_cache[l], M, state=state, n0=n0)
+            if small:
+                self.draft_plan.attention(l, n, self.qkv, self.attn_out, state, n0, kv_end, tree_bits, tree_words,
+                                          tree_size)
             else:
-                ops.rope_kv_append(self.qkv, H, Hkv, D, self.cos, self.sin, position_ids, storage_ids, n,
-                                   self.k_cache[l], self.v_cache[l], M, state=state, n0=n0)
-                if small:
-                    self.draft_plan.attention(l, n, self.qkv, self.attn_out, state, n0, kv_end, tree_bits, tree_words,
-                                              tree_size)
-                else:
-                    ops.tree_attn(self.plan, l, n, state=state, n0=n0, kv_end=kv_end, prefix_len=prefix_len,
-                                  dense_mask=dense_mask, mask_ld=mask_ld, tree_bits=tree_bits, tree_words=tree_words,
-                                  tree_size=tree_size)
+                ops.tree_attn(self.plan, l, n, state=state, n0=n0, kv_end=kv_end, prefix_len=prefix_len,
+                              dense_mask=dense_mask, mask_ld=mask_ld, tree_bits=tree_bits, tree_words=tree_words,
+                              tree_size=tree_size)
+
+        self._layers(N, attend)                        # the row-wise ops and the GEMMs see the rows of all sequences
+        if skip_lm_head:                               # TP follower ranks: only rank 0 consumes logits
+            return None
+        return self._lm_head(logits_from, N if logits_to is None else logits_to, logits_out)
+
+    @torch.no_grad()
+    def forward_ragged(self, parts, tokens: torch.Tensor, position_ids: torch.Tensor, storage_ids: torch.Tensor, *,
+                       state: torch.Tensor, tree_bits=None, tree_words: int = 0, tree_size: int = 0) -> None:
+        """Forward a chosen set of the engine's B sequences, each with its own row count, at the cost of those rows.
+        parts: (seq, n, n0, kv_end, n_logits, logits_out) per sequence -- n rows of sequence seq in the tree-relative
+        addressing of its state row (as forward(batch=True) with that n0 / kv_end), packed in list order for the row-wise
+        ops and the GEMMs; the logits of its last n_logits rows go to logits_out (n_logits, V).  Sequences not listed are
+        neither read nor written (their SQ_ST_FROZEN word is not consulted)."""
+        if self.tp.size > 1:
+            raise NotImplementedError("forward_ragged runs on one GPU: tensor-parallel engines use forward(batch=True)")
+        geo = [tuple(int(x) for x in p[:4]) for p in parts]
+        row0, _ = ops.ragged_layout(geo, self.B, self.n_max)
+        for (seq, n, _, _), (*_, m, out) in zip(geo, parts):
+            if not 0 < m <= n or out is None or tuple(out.shape) != (m, self.V):
+                raise ValueError(f"sequence {seq}: {m} logit rows of {n} into {None if out is None else tuple(out.shape)}")
+        H, Hkv, D, M = self.H, self.Hkv, self.D, self.M
+        arr = ops.ragged_parts(geo)
+        ops.embed_rows_ragged(self.embed, tokens, arr, self.hidden, state)
+
+        def attend(l):
+            ops.rope_kv_append_ragged(self.qkv, H, Hkv, D, self.cos, self.sin, position_ids, storage_ids, arr,
+                                      self.k_cache[l], self.v_cache[l], M, state)
+            ops.tree_attn_ragged(self.plan, l, arr, state=state, tree_bits=tree_bits, tree_words=tree_words,
+                                 tree_size=tree_size)
+
+        self._layers(row0[-1], attend)
+        for (_, n, _, _), (*_, m, out), r0 in zip(geo, parts, row0):
+            self._lm_head(r0 + n - m, r0 + n, out)
+
+    def _layers(self, n: int, attend):
+        """The decoder layers over activation rows [0, n); attend(l) is layer l's RoPE + KV append and attention."""
+        ops.rmsnorm(self.hidden, self.layers[0]["ln1"], self.normed, n, self.eps)
+        for l, ly in enumerate(self.layers):
+            self._project(ly, "wqkv", self.normed, n, self.qkv)
+            attend(l)
             nxt = self.layers[l + 1]["ln1"] if l + 1 < self.L else self.norm
             if self.peer is not None:
                 torch.mm(self.attn_out[:n], ly["wo"].t(), out=self.peer.buf[0][:n])
@@ -429,13 +469,13 @@ class LlamaRunner:
             self._project(ly, "wd", self.act, n, self.proj)
             self.tp.all_reduce(self.proj[:n])
             ops.add_rmsnorm(self.hidden, self.proj, nxt, self.normed, n, self.eps)
-        if skip_lm_head:                               # TP follower ranks: only rank 0 consumes logits
-            return None
-        end = n if logits_to is None else logits_to
-        m = end - logits_from
-        out = logits_out if logits_out is not None else self.logits[:m]
+
+    def _lm_head(self, start: int, end: int, out: Optional[torch.Tensor]) -> torch.Tensor:
+        """logits of normed rows [start, end) -> out (default: the internal buffer)"""
+        m = end - start
+        out = out if out is not None else self.logits[:m]
         if self.lm_plan is not None and m <= 128 and out.stride(-1) == 1 and out.stride(0) % 8 == 0 and out.data_ptr() % 16 == 0:
-            self.lm_plan.run(m, a_row0=logits_from, out=out)
+            self.lm_plan.run(m, a_row0=start, out=out)
         else:
-            torch.mm(self.normed[logits_from:end], self.lm_head.t(), out=out)
+            torch.mm(self.normed[start:end], self.lm_head.t(), out=out)
         return out

@@ -427,6 +427,57 @@ def tree_attn_batch(plan: AttnPlan, layer, n, *, state, n0=0, kv_end=0, tree_bit
                                          tree_words, tree_size, stream_ptr()), "sq_tree_attn_batch")
 
 
+class RaggedPart(C.Structure):
+    """sq_ragged_part: n rows of sequence seq, nodes [n0, n0 + n) in its tree-relative addressing, attending slots
+    [0, base + kv_end)"""
+    _fields_ = [("seq", C.c_int32), ("n", C.c_int32), ("n0", C.c_int32), ("kv_end", C.c_int32)]
+
+
+def ragged_parts(parts):
+    """(seq, n, n0, kv_end) tuples -> the host array the *_ragged calls take (an array built here is passed through)."""
+    if isinstance(parts, C.Array):
+        return parts
+    parts = [tuple(int(x) for x in p) for p in parts]
+    return (RaggedPart * len(parts))(*parts)
+
+
+def ragged_layout(parts, B: int, n_max: int, rows_per_tile: int = 1):
+    """-> (row0, tile0): lists of len(parts) + 1 prefix sums of the packed rows and of the q tiles of rows_per_tile rows.
+    Raises SequoiaLibError on a part list the ragged calls refuse."""
+    arr = ragged_parts(parts)
+    k = len(arr)
+    row0, tile0 = (C.c_int32 * (k + 1))(), (C.c_int32 * (k + 1))()
+    check(_lib.load().sq_ragged_layout(C.addressof(arr), k, B, n_max, rows_per_tile, C.addressof(row0),
+                                       C.addressof(tile0)), "sq_ragged_layout")
+    return list(row0), list(tile0)
+
+
+def embed_rows_ragged(table, tokens, parts, out, state):
+    """Rows of the listed sequences packed in list order into out (n_max = out's rows); tokens (B, M), state (B, 16)."""
+    arr = ragged_parts(parts)
+    check(_lib.load().sq_embed_rows_ragged(ptr(table), ptr(tokens), _rows(tokens, "tokens"), ptr(state), C.addressof(arr),
+                                           len(arr), state.shape[0], out.shape[0], table.shape[1], ptr(out),
+                                           stream_ptr()), "sq_embed_rows_ragged")
+
+
+def rope_kv_append_ragged(qkv, H, Hkv, D, cos, sin, position_ids, storage_ids, parts, k_layer, v_layer, M, state):
+    """k_layer / v_layer: (B, Hkv, M, D) = one layer of a (L, B, Hkv, M, D) cache; qkv rows packed in list order."""
+    B = state.shape[0]
+    ld = _rows(position_ids, "position_ids")
+    assert _rows(storage_ids, "storage_ids") == ld and k_layer.shape[0] == B
+    arr = ragged_parts(parts)
+    check(_lib.load().sq_rope_kv_append_ragged(ptr(qkv), qkv.shape[-1], H, Hkv, D, ptr(cos), ptr(sin), ptr(position_ids),
+                                               ptr(storage_ids), ld, ptr(state), C.addressof(arr), len(arr), B,
+                                               qkv.shape[0], ptr(k_layer), ptr(v_layer), M, stream_ptr()),
+          "sq_rope_kv_append_ragged")
+
+
+def tree_attn_ragged(plan: AttnPlan, layer, parts, *, state, tree_bits=None, tree_words=0, tree_size=0):
+    arr = ragged_parts(parts)
+    check(_lib.load().sq_tree_attn_ragged(plan.handle, layer, C.addressof(arr), len(arr), ptr(state), ptr(tree_bits),
+                                          tree_words, tree_size, stream_ptr()), "sq_tree_attn_ragged")
+
+
 def sample_level_batch(logits, row_base, row_step, rand, n_parents, k_max, T, mode, *, parent_rows, child_first, n_branch,
                        tokens, state):
     """rand: (B, S, V) (mode 0) or None (mode 1, top-k)."""
