@@ -124,7 +124,15 @@ __global__ void __launch_bounds__(G_THREADS, 1)
     for (int c = 0; c < NCH; ++c)
 #pragma unroll
       for (int e = 0; e < 32; ++e) acc[c][e] = 0.f;
-    int stage = 0;
+    // frees a slot -- in every CTA whose multicast writes into this CTA's slot
+    auto release = [&](int s) {
+      if (lane == 0) {
+        if (MC == 1) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar_empty + 8 * s) : "memory");
+        else
+          for (int r = 0; r < MC; ++r) ptx::mbar_arrive_cluster(bar_empty + 8 * s, (uint32_t)(MC * ks + r));
+      }
+    };
+    int stage = 0, prev = -1;
     uint32_t phase = 0;
     for (int kb = 0; kb < nkb; ++kb) {
       ptx::mbar_wait(bar_full + 8 * stage, phase, g.err_flag, 12);               // TMA bytes have landed
@@ -136,15 +144,14 @@ __global__ void __launch_bounds__(G_THREADS, 1)
         for (int c = 0; c < NCH; ++c)
           ptx::wgmma_ss<0>(acc[c], gmma_desc(sa + k * 32, 16, 1024), gmma_desc(sw + c * 8192 + k * 32, 16, 1024), 1);
       ptx::wgmma_commit();
-      ptx::wgmma_wait_all();
-      // frees the slot -- in every CTA whose multicast writes into this CTA's slot
-      if (lane == 0) {
-        if (MC == 1) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar_empty + 8 * stage) : "memory");
-        else
-          for (int r = 0; r < MC; ++r) ptx::mbar_arrive_cluster(bar_empty + 8 * stage, (uint32_t)(MC * ks + r));
-      }
+      // keep this k-block's group in flight: only the previous one has to be done before its slot is handed back
+      asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory");
+      if (prev >= 0) release(prev);
+      prev = stage;
       if (++stage == STAGES) { stage = 0; phase ^= 1; }
     }
+    ptx::wgmma_wait_all();
+    if (prev >= 0) release(prev);
     // accumulator fragment: acc[c][4j + 2h + e] = tile row rbase + 8h, column 64c + 8j + 2q + e
     const int rbase = wg * 64 + (warp & 3) * 16 + (lane >> 2), q2 = 2 * (lane & 3);
     if (SPLIT == 1 && g.epi == 1) {

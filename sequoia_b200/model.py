@@ -302,10 +302,9 @@ class LlamaRunner:
         self.k_cache = torch.zeros(self.L, batch_size, self.Hkv, max_length, D, dtype=F16, device=dev)
         self.v_cache = torch.zeros_like(self.k_cache)
         self.plan = ops.AttnPlan(self.qkv, n, self.H, self.Hkv, D, self.k_cache, self.v_cache, self.attn_out)
-        # Dense GEMMs.  The weight-streaming shapes go to the hand-written wgmma kernel (csrc/sq_gemm.cu) -- gate_up with the
-        # SwiGLU epilogue fused (weights interleaved, `act` written directly: no gate_up round trip, no silu_mul launch)
-        # and the target's lm_head -- for models whose layers are HBM-stream-sized (hidden >= 2048); q/k/v, o_proj and
-        # down_proj stay on cuBLASLt (torch.mm), which is faster at those shapes.
+        # Dense GEMMs.  For models whose layers are HBM-stream-sized (hidden >= 2048) the target's lm_head (<= 128 rows) and
+        # the gate_up of 97-128-row forwards (below) run on the hand-written wgmma kernel (csrc/sq_gemm.cu); every other
+        # projection and row count runs on cuBLASLt (torch.mm), which is faster there.
         self.gemm_err = torch.zeros(4, dtype=torch.int32, device=dev)
         self.lm_plan = None
         if weight_format == "fp8":
@@ -319,18 +318,21 @@ class LlamaRunner:
                     del q
             torch.cuda.empty_cache()
         stream_sized = h >= 2048
-        # (a fused-epilogue plan cannot split K, so a narrow shard -- TP-4/8 of a 7B -- would leave most SMs idle: those
-        # stay on cuBLASLt + sq_silu_mul).  The plans serve forwards of <= 128 rows; larger ones (prefill, the 768-row verify
-        # of config 4: compute-bound, not a weight stream) go to cuBLASLt on the SAME weight tensor, which is why gate_up is
-        # kept row-major in the interleaved order (16 gate rows | 16 up rows) rather than pre-tiled.
-        gu_bn, gu_split, _ = ops.gemm_pick_tiles(2 * self.I, h, ops.GEMM_SWIGLU) if self.I % 16 == 0 and h % 64 == 0 else (0, 1, 1)
-        gu_ctas = (-(-2 * self.I // gu_bn)) * gu_split if gu_bn else 0
+        # Layer projections of the 97-128-row verify (config 2's 128-node tree) on sq_gemm: the ones it streams faster than
+        # cuBLASLt on an H100 (DESIGN §4 table).  Only gate_up wins there, with the SwiGLU epilogue fused (one launch, no
+        # gate_up round trip, no silu_mul).  q/k/v, o_proj and down_proj stay on cuBLASLt, and so does every other row
+        # count: prefill, the first verify and the 768-row verify of config 4 are compute-bound, not a weight stream, and
+        # config 3's 65-row tree is better served by cuBLASLt's 64-row tiles than by the plan's 128-row activation tile.
+        # Those go to cuBLASLt on the SAME weight tensor, which is why gate_up is kept row-major in the interleaved order
+        # (16 gate rows | 16 up rows) rather than pre-tiled.  Tensor-parallel shards keep cuBLASLt + sq_silu_mul, and so
+        # does a tile with the 2-CTA activation multicast (the 13B gate_up): every multicast tile measured 2-4x slower.
+        ok = stream_sized and tp == 1 and weight_format == "fp16" and self.I % 16 == 0 and h % 64 == 0
         self.gu_interleaved = False
-        if stream_sized and gu_ctas >= 120 and weight_format == "fp16":
+        if ok and ops.gemm_pick_tiles(2 * self.I, h, ops.GEMM_SWIGLU)[2] == 1:
             self.gu_interleaved = True
             for ly in self.layers:
                 ly["wgu"] = ops.interleave_gate_up(ly["wgu"][:self.I], ly["wgu"][self.I:])
-                ly["gu_plan"] = ops.GemmPlan(self.normed, ly["wgu"], self.act, self.gemm_err, swiglu=True)
+                ly["wgu_plan"] = ops.GemmPlan(self.normed, ly["wgu"], self.act, self.gemm_err, swiglu=True)
         if stream_sized and V % 32 == 0 and h % 64 == 0:
             self.lm_plan = ops.GemmPlan(self.normed, self.lm_head, self.logits, self.gemm_err)
         # Small draft models (csrc/sq_draft.cu): a dedicated attention kernel replaces sq_tree_attn for the draft's
@@ -346,7 +348,7 @@ class LlamaRunner:
 
     def _gate_up_act(self, ly, n: int):
         """act[:n] = silu(normed[:n] @ Wg.T) * (normed[:n] @ Wu.T)   (Engine/Llama_modules.py:272)"""
-        plan = ly.get("gu_plan")
+        plan = ly.get("wgu_plan")
         # the plan's activation tile is always 128 rows: worth it when most of them are real (config 2: 128 rows); for the
         # 65-row tree of config 3 cuBLASLt's 64-row tiles ingest half as much activation per SM
         if plan is not None and 96 < n <= 128:
