@@ -415,6 +415,29 @@ int sq_rope_kv_append_ragged(sq_half* qkv, int ld, int H, int Hkv, int D, const 
 int sq_tree_attn_ragged(sq_attn_plan* plan, int layer, const sq_ragged_part* parts, int n_parts, const int32_t* state,
                         const uint32_t* tree_bits, int tree_words, int tree_size, void* stream);
 
+/* ---- per-sequence counter-based random numbers (csrc/sq_rng.cu): seeded BatchTree sequences draw r, rand and the bonus
+ * noise on the device, each from a stream of its own ----
+ * Generator: Random123 philox4x32-10.  Sequence b's key is its 64-bit seed, (seeds[b] & 0xffffffff, seeds[b] >> 32).
+ * Element e of a stream is word e % 4 of the output block for counter (i & 0xffffffff, i >> 32, purpose, step),
+ * i = e / 4.  Purposes:
+ *   0 = r:           M elements, step 0;
+ *   1 = rand:        S*V elements, node-major (node*V + v), step 0;
+ *   2 = bonus noise: V elements, step = the sequence's verify count since it was seeded (0-based), mod 2^32.
+ * Uniforms (purposes 0, 1): u = fp16((w >> 21) * 2^-11), the 2048 values k/2048 of torch's CPU fp16 uniform_.
+ * Noise (purpose 2): u = fp32((w >> 8) + 0.5) * 2^-24 (one round-to-nearest-even), noise = fp16(max(-logf(u), 2^-24)):
+ * positive and finite, so the walk's residual / noise never divides by zero.
+ * seeds: (B,) uint64 and steps: (B,) int64 device arrays. */
+/* `count` uniforms of `purpose` (0 or 1) into row b of `out` (row pitch ld_seq halfs) for every slot b of the host list
+ * host_seqs[0 .. n_seqs), one launch.  Refused with SQ_ERR_INVALID_ARG before any launch: B outside 1..SQ_MAX_BATCH,
+ * a slot out of range or listed twice, a null pointer, a purpose other than 0 or 1, count < 1 or ld_seq < count. */
+int sq_rng_uniform_seqs(sq_half* out, int64_t ld_seq, int64_t count, const uint64_t* seeds, const int32_t* host_seqs,
+                        int n_seqs, int B, int purpose, void* stream);
+/* Row b of the (B, ld_noise) noise at step steps[b] for every sequence whose SQ_ST_FROZEN word is 0, then steps[b] += 1
+ * on the device; a frozen sequence's row and counter are left untouched.  Graph capturable, needs nothing from the host
+ * per replay.  V and ld_noise multiples of 8, ld_noise >= V, rows 16-byte aligned. */
+int sq_rng_exponential_batch(sq_half* noise, int64_t ld_noise, int V, const uint64_t* seeds, int64_t* steps,
+                             const int32_t* state, int B, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

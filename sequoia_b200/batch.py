@@ -61,14 +61,34 @@ def _per_seq(value, B: int, name: str) -> List[float]:
     return vals
 
 
+def check_seed(seed) -> int:
+    """A per-sequence seed: an integer in [0, 2^64)."""
+    if isinstance(seed, bool) or not isinstance(seed, numbers.Integral):
+        raise ValueError(f"a seed must be an integer in [0, 2^64), got {seed!r}")
+    seed = int(seed)
+    if not 0 <= seed < 1 << 64:
+        raise ValueError(f"a seed must be an integer in [0, 2^64), got {seed}")
+    return seed
+
+
+def _as_int64(seed: int) -> int:
+    """The int64 with the bits of the uint64 `seed` (how the device arrays hold it)."""
+    return seed - (1 << 64) if seed >= 1 << 63 else seed
+
+
 class BatchTree:
     """Batched SpecTree ("spec") / GreedyTree ("greedy") over `len(prompts)` sequences.  The engines must have been built
     with batch_size == len(prompts).  verify() returns one (valid_tokens, accept_length, terminal) per sequence.
-    temperature and top_p: one value for all sequences, or one per sequence; "greedy" ignores both."""
+    temperature and top_p: one value for all sequences, or one per sequence; "greedy" ignores both.
+    seeds: None (r and rand drawn with torch's CPU generator as a lone SpecTree draws them, the bonus noise with torch's
+    CUDA generator), or one integer in [0, 2^64) per prompt: each sequence then draws all its random numbers on the
+    device from a Philox stream keyed by its seed, so its output does not depend on its slot or its neighbours ("greedy"
+    takes seeds and ignores them)."""
 
     def __init__(self, draft, target, prompts: Sequence[torch.Tensor], grow_map: dict, policy: str = "spec",
                  temperature: Union[float, Sequence[float]] = 0.6, top_p: Union[float, Sequence[float]] = 1.0,
-                 max_length: int = 256, max_target_seq: Optional[int] = None):
+                 max_length: int = 256, max_target_seq: Optional[int] = None,
+                 seeds: Optional[Sequence[int]] = None):
         if policy not in POLICIES:
             raise ValueError(f"BatchTree policy {policy!r} is not supported (only {POLICIES}); greedys, specinfer and the "
                              "*TreeTest policies run one sequence at a time")
@@ -76,6 +96,11 @@ class BatchTree:
         temps, top_ps = _per_seq(temperature, B, "temperature"), _per_seq(top_p, B, "top_p")
         for t, p in zip(temps, top_ps):
             check_sampling(t, p)
+        if seeds is not None:
+            seeds = list(seeds)
+            if len(seeds) != B:
+                raise ValueError(f"seeds: {len(seeds)} values for {B} sequences")
+            seeds = [check_seed(s) for s in seeds]
         for name, eng in (("draft", draft), ("target", target)):
             if eng.engine.batch_size != B:
                 raise ValueError(f"{name} engine holds {eng.engine.batch_size} sequences, got {B} prompts")
@@ -128,11 +153,22 @@ class BatchTree:
         self.last: List[tuple] = [None] * B
         self.ground_truth_len = [len(p) for p in prompts]
         self.target_kv_len = [0] * B
-        if not self.greedy:
+        # seeded: each sequence draws r, rand and its bonus noise on the device from a counter-based stream of its own
+        # (sq_rng.cu); steps[b] counts sequence b's verifies since it was seeded and advances inside the graphs
+        self.seeded = seeds is not None
+        if self.seeded:
+            self.seeds = torch.tensor([_as_int64(s) for s in seeds], **i64)
+            self.steps = torch.zeros(B, **i64)
+        if self.greedy:
+            self.r = self.rand = None
+        elif self.seeded:
+            self.r = torch.empty(B, M, dtype=F16, device=dev)
+            self.rand = torch.empty(B, S, V, dtype=F16, device=dev)
+            ops.rng_uniform_seqs(self.r, self.seeds, range(B), ops.RNG_R)
+            ops.rng_uniform_seqs(self.rand, self.seeds, range(B), ops.RNG_RAND)
+        else:
             r, rand = draw_random(prompts, M, S, V)
             self.r, self.rand = r.to(dev), rand.to(dev)
-        else:
-            self.r = self.rand = None
         for b, p in enumerate(prompts):
             self._load_prompt(b, p)
         with torch.inference_mode():
@@ -169,10 +205,13 @@ class BatchTree:
         self.state[b, ST_FROZEN] = 1
 
     @torch.inference_mode()
-    def admit(self, b: int, prompt: torch.Tensor, temperature: Optional[float] = None, top_p: Optional[float] = None):
+    def admit(self, b: int, prompt: torch.Tensor, temperature: Optional[float] = None, top_p: Optional[float] = None,
+              seed: Optional[int] = None):
         """Start `prompt` in the frozen slot b (finished, out of room, or stopped with freeze), at its own temperature and
         top_p (default: the slot's previous values).  The next verify() runs its first verify next to the steady
-        sequences.  The slot draws r and rand as a lone SpecTree on the prompt would, and runs its draft prefill now."""
+        sequences.  The slot draws r and rand as a lone SpecTree on the prompt would, and runs its draft prefill now.
+        A seeded tree takes the prompt's `seed` (required there, refused otherwise): r and rand are then filled on the
+        device from that seed's stream and the slot's noise counter restarts at 0."""
         if not 0 <= b < self.B:
             raise IndexError(f"slot {b} out of range for a batch of {self.B}")
         if not self.frozen[b]:
@@ -183,6 +222,12 @@ class BatchTree:
         T = self.temps[b] if temperature is None else float(temperature)
         tp = self.top_ps[b] if top_p is None else float(top_p)
         check_sampling(T, tp)
+        if self.seeded and seed is None:
+            raise ValueError("this BatchTree was built with seeds: admit needs the prompt's seed=")
+        if not self.seeded and seed is not None:
+            raise ValueError("seed= needs a BatchTree built with seeds")
+        if seed is not None:
+            seed = check_seed(seed)
         self.temps[b], self.top_ps[b] = T, tp
         self.T_dev[b] = T
         self.top_p_dev[b] = tp
@@ -195,7 +240,13 @@ class BatchTree:
         self.last[b] = None
         self.ground_truth_len[b] = P
         self.target_kv_len[b] = 0
-        if not self.greedy:
+        if self.seeded:
+            self.seeds[b] = _as_int64(seed)
+            self.steps[b] = 0
+            if not self.greedy:
+                ops.rng_uniform_seqs(self.r, self.seeds, [b], ops.RNG_R)
+                ops.rng_uniform_seqs(self.rand, self.seeds, [b], ops.RNG_RAND)
+        elif not self.greedy:
             r, rand = draw_random([prompt], self.M, self.S, self.V)
             self.r[b].copy_(_h2d(r[0]), non_blocking=True)
             self.rand[b].copy_(_h2d(rand[0]), non_blocking=True)
@@ -238,7 +289,10 @@ class BatchTree:
         if self.use_top_p:
             ops.top_p_filter_per_seq_(self.target_logits, self.top_p_dev, self.T_dev, self.S)
         if self.external_noise is None:
-            self.noise.exponential_(1.0)
+            if self.seeded:
+                ops.rng_exponential_batch(self.noise, self.seeds, self.steps, self.state)
+            else:
+                self.noise.exponential_(1.0)
         ops.accept_stochastic_batch_per_seq(self.target_logits, self.draft_logits, self.row_base, self.row_step, self.r,
                                             self.noise, st.succ_off, st.succ, st.depth, self.S, self.T_dev, self.tokens,
                                             self.position_ids, self.accept_idx, self.state, self.max_target_seq)
@@ -298,14 +352,18 @@ class BatchTree:
     def _caches(self):
         return [t for e in (self.draft, self.target) for t in (e.engine.kv_cache.k_cache, e.engine.kv_cache.v_cache)]
 
+    def _captured_bufs(self):
+        """The device buffers a graph's warm-up run writes (the noise counters of a seeded tree included, so that a
+        sequence's noise does not depend on when the graphs were captured)."""
+        bufs = [self.tokens, self.position_ids, self.state, self.draft_logits, self.target_logits, self.noise]
+        return bufs + [self.steps] if self.seeded else bufs
+
     def _snapshot(self):
-        return dict(bufs=[t.clone() for t in (self.tokens, self.position_ids, self.state, self.draft_logits,
-                                              self.target_logits, self.noise)],
+        return dict(bufs=[t.clone() for t in self._captured_bufs()],
                     kv=[t.clone() for t in self._caches()], rng=torch.cuda.get_rng_state(self.device))
 
     def _restore(self, s):
-        for t, c in zip((self.tokens, self.position_ids, self.state, self.draft_logits, self.target_logits, self.noise),
-                        s["bufs"]):
+        for t, c in zip(self._captured_bufs(), s["bufs"]):
             t.copy_(c)
         for t, c in zip(self._caches(), s["kv"]):
             t.copy_(c)

@@ -548,6 +548,45 @@ def top_p_filter_per_seq_(logits, top_p, T, rows_per_seq: int):
     return logits
 
 
+# ---- per-sequence counter-based random numbers (csrc/sq_rng.cu; stream layout in include/sequoia_b200.h) -------------------
+RNG_R, RNG_RAND, RNG_NOISE = 0, 1, 2     # purposes: r (M), rand (S*V, node-major), bonus noise (V, one step per verify)
+
+
+def _seeds(seeds, B, name):
+    if seeds.dtype != torch.int64 or not seeds.is_cuda or seeds.dim() != 1 or seeds.shape[0] < B or seeds.stride(0) != 1:
+        raise TypeError(f"{name}: seeds must be a contiguous ({B},) int64 CUDA tensor (the uint64 seeds' bits)")
+
+
+def rng_uniform_seqs(out, seeds, slots, purpose: int):
+    """Fill row b of `out` ((B, ...) fp16, each row contiguous) with the uniforms of `purpose` (RNG_R or RNG_RAND) of the
+    stream keyed by seeds[b], for every slot b in `slots` (host list), in one launch.  seeds: (B,) int64 on the device."""
+    _need(out, F16, "rng_uniform_seqs")
+    B = out.shape[0]
+    _seeds(seeds, B, "rng_uniform_seqs")
+    row = out[0]
+    if not row.is_contiguous():
+        raise ValueError(f"rng_uniform_seqs: rows of out must be contiguous, got strides {tuple(out.stride())}")
+    slots = [int(b) for b in slots]
+    arr = (C.c_int32 * max(len(slots), 1))(*slots)
+    check(_lib.load().sq_rng_uniform_seqs(ptr(out), out.stride(0), row.numel(), ptr(seeds), C.addressof(arr), len(slots),
+                                          B, purpose, stream_ptr()), "sq_rng_uniform_seqs")
+    return out
+
+
+def rng_exponential_batch(noise, seeds, steps, state):
+    """Row b of the (B, V) fp16 noise = the Exp(1) draws of step steps[b] of seeds[b]'s stream, for every sequence not
+    frozen in `state`; then steps[b] += 1 on the device.  seeds, steps: (B,) int64 on the device."""
+    _need(noise, F16, "rng_exponential_batch")
+    B = state.shape[0]
+    _seeds(seeds, B, "rng_exponential_batch")
+    if steps.dtype != torch.int64 or not steps.is_cuda or steps.dim() != 1 or steps.shape[0] < B or steps.stride(0) != 1:
+        raise TypeError(f"rng_exponential_batch: steps must be a contiguous ({B},) int64 CUDA tensor")
+    if noise.shape[0] < B:
+        raise ValueError(f"rng_exponential_batch: {noise.shape[0]} noise rows for {B} sequences")
+    check(_lib.load().sq_rng_exponential_batch(ptr(noise), _rows(noise, "noise"), noise.shape[-1], ptr(seeds), ptr(steps),
+                                               ptr(state), B, stream_ptr()), "sq_rng_exponential_batch")
+
+
 def accept_greedy_batch(target_token, succ_off, succ, depth, S, tokens, position_ids, accept_idx, state, max_target_seq):
     """target_token (B*S) int64."""
     ld = _rows(tokens, "tokens")

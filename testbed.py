@@ -188,12 +188,12 @@ def simulation_baseline(target, prompts, T, top_p, M, new_tokens: int = 32, stop
     return dict(decoded_tokens=decoded, seconds=total_time, latency=total_time / max(decoded, 1))
 
 
-def decode_refill(tree, prompts, limits, stop=DEFAULT_STOP, step_times=None):
+def decode_refill(tree, prompts, limits, stop=DEFAULT_STOP, step_times=None, seeds=None):
     """Decode every prompt of a queue on a BatchTree whose B slots start with prompts[:B]: each slot that finishes (a stop
     token, its length limit `limits[i]`, or out of room) takes the next prompt, until the queue is empty.
     -> (outputs, decoded tokens, per-sequence target steps, admission order); outputs[i] = prompt i's committed tokens.
     step_times: a list that receives ("steady" | "admission", seconds) per step; an admission step is timed from the
-    first admit() of the step to the end of its verify."""
+    first admit() of the step to the end of its verify.  seeds: for a seeded tree, prompt i's seed is seeds[i]."""
     B = len(tree.frozen)
     slot = list(range(B))                        # prompt index decoding in each slot (None: the queue ran out)
     length = [len(p) for p in prompts[:B]]
@@ -203,7 +203,10 @@ def decode_refill(tree, prompts, limits, stop=DEFAULT_STOP, step_times=None):
     while any(i is not None for i in slot):
         t0 = time.perf_counter()
         for b in pending:
-            tree.admit(b, prompts[slot[b]])
+            if seeds is None:
+                tree.admit(b, prompts[slot[b]])
+            else:
+                tree.admit(b, prompts[slot[b]], seed=seeds[slot[b]])
         kind = "admission" if pending else "steady"
         pending = []
         tree.construct_grow_map()
@@ -256,23 +259,25 @@ def decode_chunk(tree, chunk, limits, stop=DEFAULT_STOP):
 
 @torch.inference_mode()
 def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: int, stop=DEFAULT_STOP,
-                     refill: bool = False):
+                     refill: bool = False, seeds=None):
     """--batch B: the same metric loop with B prompts decoded together (sequoia_b200.batch.BatchTree).  Chunked: B
     prompts at a time, each chunk until its last sequence stops.  refill: one batch whose finished slots take the next
-    prompt (BatchTree.admit)."""
+    prompt (BatchTree.admit).  seeds: one per prompt (--device-rng): each sequence draws its random numbers on the device
+    from its own seed."""
     from sequoia_b200.batch import BatchTree
     steps = decoded = 0                          # steps: target steps summed over sequences (per-sequence tokens / step)
     total_time = 0.0
     limits = [MAX_NEW_LEN] * len(prompts)
     prompts = [p.to(DEV) for p in prompts]
     chunks = [prompts[:B]] if refill else [prompts[i:i + B] for i in range(0, len(prompts), B)]
-    for chunk in chunks:
+    for c, chunk in enumerate(chunks):
+        i0 = c * B
         tree = BatchTree(draft, target, chunk, grow_map, policy=policy, temperature=T, top_p=top_p, max_length=M,
-                         max_target_seq=M)
+                         max_target_seq=M, seeds=None if seeds is None else seeds[i0:i0 + len(chunk)])
         torch.cuda.synchronize()
         t1 = time.time()
         if refill:
-            _, d, s, _ = decode_refill(tree, prompts, limits, stop)
+            _, d, s, _ = decode_refill(tree, prompts, limits, stop, seeds=seeds)
         else:
             d, s = decode_chunk(tree, chunk, limits[:len(chunk)], stop)
         decoded += d
@@ -310,6 +315,9 @@ def build_parser():
                          "prompt count must divide)")
     ap.add_argument("--refill", action="store_true",
                     help="with --batch: keep the batch full, each finished slot takes the next prompt of the queue")
+    ap.add_argument("--device-rng", action="store_true",
+                    help="with --batch: each prompt draws its random numbers on the device from a stream of its own, "
+                         "seeded (seed << 32) | prompt index, so its output does not depend on its slot or its neighbours")
     ap.add_argument("--target-weights", type=str, default="fp16", choices=["fp16", "fp8"],
                     help="fp8: the target's layer projections quantized to E4M3 with per-channel scales at load")
     return ap
@@ -328,6 +336,17 @@ def check_batch_args(args, n_prompts: int) -> int:
     return args.batch
 
 
+def device_rng_seeds(args, n_prompts: int):
+    """--device-rng: prompt i's seed (args.seed << 32) | i; None without the flag.  Refused without --batch."""
+    if not args.device_rng:
+        return None
+    if args.batch == 1 and not args.refill:
+        raise SystemExit("--device-rng runs with --batch (the batched tree); the lone trees keep the reference's draws")
+    if not 0 <= args.seed < 1 << 32:
+        raise SystemExit(f"--device-rng needs --seed in [0, 2^32), got {args.seed}")
+    return [(args.seed << 32) | i for i in range(n_prompts)]
+
+
 def main(argv=None):
     args = build_parser().parse_args(argv)
     print(args)
@@ -339,6 +358,7 @@ def main(argv=None):
     stop = stop_tokens(args.target)
     if args.target_weights != "fp16" and args.offloading:
         raise SystemExit("--target-weights fp8 runs without --offloading")
+    seeds = device_rng_seeds(args, len(prompts))
     if args.batch != 1 or args.refill:
         B = check_batch_args(args, len(prompts))
         target = GraphInferenceEngineTG(max_length=args.M, model_name_or_path=args.target, dtype=torch.float16,
@@ -349,7 +369,7 @@ def main(argv=None):
         grow_map = torch.load(path)
         assert args.M >= MAX_NEW_LEN + grow_map["size"], "--M must hold 256 tokens + the tree (README.md:47 of the reference)"
         res = simulation_batch(target, draft, prompts, grow_map, args.tree, args.T, args.P, args.M, B, stop=stop,
-                               refill=args.refill)
+                               refill=args.refill, seeds=seeds)
         print(json.dumps({k: (round(v, 5) if isinstance(v, float) else v) for k, v in res.items()}))
         return res
     target = (tcls(max_length=args.M, model_name_or_path=args.target, dtype=torch.float16, device=DEV)
