@@ -150,3 +150,87 @@ def test_tp_driver_follower_protocol_gloo():
     assert log[3] == ("forward", S, 1 + 2 + 3 + 4, 0, S, 0, True) and log[4] == ("gather", 0, 103, [101, 109])
     assert log[5] == ("forward", S, 2 + 3 + 4 + 5, 0, S, 0, True) and log[6] == ("gather", 1, 104, [101, 109])
     assert len(log) == 7
+
+
+# ------------------------------------------------------------------------------------------------ peer block layout
+def _ll_accepts(N, n, rows_max, own_max):
+    """sq_tp_allreduce_ll_add_rmsnorm's size check (own_max == rows_max is its one-shot form)."""
+    return n <= rows_max and (own_max == rows_max or (n + N - 1) // N <= own_max)
+
+
+def _layout_cases():
+    return [(N, n_max, hidden) for N in range(2, 9)
+            for n_max, hidden in [(1, 4096), (N - 1 or 1, 2048), (N + 1, 1028), (128, 4096), (257, 8192), (768, 8192),
+                                  (1024, 5120), (300, 16384)]]
+
+
+def test_peer_layout_regions_hold_every_kernel_access():
+    """The regions of PeerBuffers' block do not overlap, fit in `total`, and hold the highest byte each kernel in sq_tp.cu
+    can touch for any n <= n_max it accepts (indexing restated from the kernels)."""
+    from sequoia_b200.peer import FLAG_BYTES, MBOX_WORDS, peer_layout
+    for N, n_max, hidden in _layout_cases():
+        for form in (None, True, False):
+            L = peer_layout(N, n_max, hidden, ll_oneshot=form)
+            regs = L.regions()
+            # 16-byte words everywhere; at hidden % 8 == 4 (LL only) the partials are read 8 bytes at a time
+            assert regs[0][1] == 0 and all(off % (16 if hidden % 8 == 0 or name not in ("proj_b", "red_a", "red_b") else 8) == 0
+                                           for name, off, _ in regs), (N, n_max, hidden, regs)
+            for (a, oa, sa), (b, ob, _) in zip(regs, regs[1:]):
+                assert oa + sa <= ob, (N, n_max, hidden, a, b)
+            assert regs[-1][1] + regs[-1][2] <= L.total
+            size = {name: sz for name, _, sz in regs}
+            rows = L.push_rows
+            assert rows == min(n_max, 256)
+            # highest byte + 1 touched, per region
+            assert n_max * hidden * 2 <= size["proj_a"] and n_max * hidden * 2 <= size["red_a"]    # pull partials / red rows
+            assert 4 * N <= size["flags"] and 4 * 3 <= size["epoch"]                               # flags[s], epoch[0..2]
+            assert 4 * n_max <= size["rowflags_a"]                                                  # rowflags[r], r < n
+            assert (((N - 1) * rows + rows - 1) * hidden + hidden) * 2 <= size["recv_a"]            # recv[(rank*rows_max+r)*hidden]
+            assert 4 * N * rows <= size["pflags"]                                                   # pflags[src*rows_max + r]
+            oneshot = L.ll_own == rows
+            lrow_max = max((n - 1) if oneshot else (n - 1) // N for n in range(1, n_max + 1)
+                           if _ll_accepts(N, n, rows, L.ll_own))
+            assert lrow_max < L.ll_own
+            assert (((N - 1) * L.ll_own + lrow_max) * (hidden // 4) + hidden // 4) * 16 <= size["ll1_a"]
+            assert ((rows - 1) * (hidden // 4) + hidden // 4) * 16 <= size["ll2_a"]                 # ll2[r * hidden/4 + p]
+            assert 2 * MBOX_WORDS * 8 == size["mbox_0"] == size["mbox_1"]
+            assert FLAG_BYTES == 1024
+            assert size["proj_b"] == size["proj_a"] and size["recv_b"] == size["recv_a"] and size["ll1_b"] == size["ll1_a"]
+
+
+def test_peer_layout_ll_form():
+    """own_max == rows_max (the LL kernel's one-shot form) exactly where the one-shot form is intended: below 4 ranks, or
+    a single row (where the two-shot gather area of one row per source is the one-shot area).  Forcing the form gives
+    own_max = rows_max or ceil(rows_max / N)."""
+    from sequoia_b200.peer import peer_layout
+    for N, n_max, hidden in _layout_cases():
+        L = peer_layout(N, n_max, hidden)
+        intended = N <= 3 or L.push_rows == 1
+        assert (L.ll_own == L.push_rows) == intended == L.ll_oneshot, (N, n_max)
+        assert L.ll_own == (L.push_rows if N <= 3 else -(-L.push_rows // N))
+        assert peer_layout(N, n_max, hidden, ll_oneshot=True).ll_own == L.push_rows
+        two = peer_layout(N, n_max, hidden, ll_oneshot=False)
+        assert two.ll_own == -(-two.push_rows // N) and two.ll_oneshot == (two.push_rows == 1)
+
+
+def test_tp_protocol_table():
+    """The all-reduce kernel chosen for (N, n, hidden) under the defaults and each SQ_TP_SHOT."""
+    from sequoia_b200.peer import tp_protocol
+    P, T, O, LL = "push", "two_shot", "one_shot", "ll"
+    points = [(1, 4096), (128, 4096), (256, 8192), (257, 4096), (129, 8192), (128, 16384), (256, 16384), (768, 8192),
+              (64, 1028)]
+    for N in range(2, 9):
+        for n, h in points:
+            ll_fits = n <= 256 and n * h * 2 <= 4 << 20 and h <= 8192
+            pull = T if N >= 4 else O
+            want = {"": LL if (4 <= N <= 7 and ll_fits) else pull,
+                    "1": O, "2": T,
+                    "3": P if (n <= 256 and (N - 1) * n * h * 2 <= 8 << 20) else pull,
+                    "4": LL if ll_fits else pull}
+            for shot, w in want.items():
+                assert tp_protocol(N, n, h, shot) == w, (N, n, h, shot)
+    # literal spot checks of the defaults: config 2 (128 rows x 4096) and config 4 (768 rows x 8192)
+    assert [tp_protocol(N, 128, 4096) for N in range(2, 9)] == [O, O, LL, LL, LL, LL, T]
+    assert [tp_protocol(N, 768, 8192) for N in range(2, 9)] == [O, O, T, T, T, T, T]
+    assert [tp_protocol(N, 128, 16384) for N in range(2, 9)] == [O, O, T, T, T, T, T]      # LL holds hidden <= 8192 only
+    assert tp_protocol(2, 256, 16384, "3") == P and tp_protocol(3, 256, 16384, "3") == O
