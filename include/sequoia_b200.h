@@ -383,6 +383,30 @@ int sq_top_p_filter_per_seq(sq_half* logits, int64_t ld, int n, int V, const flo
 int sq_accept_greedy_batch(const int64_t* target_token, const int32_t* succ_off, const int32_t* succ, const int32_t* depth,
                            int S, int64_t* tokens, int64_t* position_ids, int64_t ld_seq, int32_t* accept_idx,
                            int64_t ld_acc, int32_t* state, int B, int max_target_seq, void* stream);
+/* Per-sequence policy: greedy is a (B,) int32 device array, nonzero = the sequence decodes greedily (GreedyTree), zero = it
+ * samples (SpecTree).  One decode step of a mixed batch launches all three forms, each of which writes only its own
+ * policy's sequences:
+ *   sq_sample_level_batch_mixed: sq_sample_level_batch_per_seq with mode 1 (top-k) for a greedy sequence, mode 0 at T[b]
+ *     otherwise (T[b] of a greedy sequence is never read); rand is required;
+ *   sq_accept_greedy_batch_mixed: sq_accept_greedy_batch for the greedy sequences only;
+ *   sq_accept_stochastic_batch_mixed: sq_accept_stochastic_batch_per_seq for the sampling sequences only.
+ * A frozen sequence is left alone as in the per-sequence forms.  Refused with SQ_ERR_INVALID_ARG before any launch: a null
+ * greedy or T array, and everything the per-sequence forms refuse (B outside 1..SQ_MAX_BATCH included). */
+int sq_sample_level_batch_mixed(const sq_half* logits, int64_t ld_logits, const int32_t* row_base, const int32_t* row_step,
+                                const sq_half* rand, int64_t ld_rand, int64_t ld_rand_seq, const int32_t* parent_rows,
+                                const int32_t* child_first, const int32_t* n_branch, int n_parents, int k_max, int V,
+                                const float* T, const int32_t* greedy, int64_t* tokens, int64_t ld_seq,
+                                const int32_t* state, int B, void* stream);
+int sq_accept_greedy_batch_mixed(const int64_t* target_token, const int32_t* succ_off, const int32_t* succ,
+                                 const int32_t* depth, int S, int64_t* tokens, int64_t* position_ids, int64_t ld_seq,
+                                 int32_t* accept_idx, int64_t ld_acc, int32_t* state, const int32_t* greedy, int B,
+                                 int max_target_seq, void* stream);
+int sq_accept_stochastic_batch_mixed(const sq_half* target_logits, int64_t ld_t, const sq_half* draft_logits,
+                                     int64_t ld_d, const int32_t* row_base, const int32_t* row_step, const sq_half* r,
+                                     const sq_half* noise, int64_t ld_noise, const int32_t* succ_off, const int32_t* succ,
+                                     const int32_t* depth, int S, int V, const float* T, const int32_t* greedy,
+                                     int64_t* tokens, int64_t* position_ids, int64_t ld_seq, int32_t* accept_idx,
+                                     int64_t ld_acc, int32_t* state, int B, int max_target_seq, int policy, void* stream);
 
 /* ---- ragged batches: a forward over a chosen set of the B sequences, each with its own row count ----
  * A part list names the sequences to run.  Part j is n rows of sequence seq in that sequence's tree-relative addressing:

@@ -98,6 +98,11 @@ _SIGNATURES = {
     "sq_tree_attn_ragged": (i32, [vp, i32, vp, i32, vp, vp, i32, i32, vp]),
     "sq_rng_uniform_seqs": (i32, [vp, i64, i64, vp, vp, i32, i32, i32, vp]),
     "sq_rng_exponential_batch": (i32, [vp, i64, i32, vp, vp, vp, i32, vp]),
+    "sq_sample_level_batch_mixed": (i32, [vp, i64, vp, vp, vp, i64, i64, vp, vp, vp, i32, i32, i32, vp, vp, vp, i64, vp,
+                                          i32, vp]),
+    "sq_accept_greedy_batch_mixed": (i32, [vp, vp, vp, vp, i32, vp, vp, i64, vp, i64, vp, vp, i32, i32, vp]),
+    "sq_accept_stochastic_batch_mixed": (i32, [vp, i64, vp, i64, vp, vp, vp, vp, i64, vp, vp, vp, i32, i32, vp, vp, vp, vp,
+                                               i64, vp, i64, vp, i32, i32, i32, vp]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

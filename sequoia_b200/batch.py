@@ -10,6 +10,10 @@ lm_head GEMM).
 A sequence that is terminal, or has no room for another tree in max_length, is frozen: its state word SQ_ST_FROZEN is
 set and every batched kernel leaves its tokens, state and KV rows alone.  A frozen slot can take a new prompt with
 admit(); the other sequences keep decoding.
+
+Each sequence has its own policy, "spec" or "greedy".  While all are equal the tree launches the single-policy kernels;
+once both are present (mixed mode, which then stays on) the sampler and the two walks are the *_mixed forms, which read
+the (B,) int32 device array greedy_dev, and every sequence decodes as it would in a tree of its own policy.
 """
 from __future__ import annotations
 
@@ -41,6 +45,23 @@ def _h2d(t: torch.Tensor) -> torch.Tensor:
     """A copy source that does not block the host: device tensors as they are, host tensors pinned (the caching host
     allocator keeps the pinned block until the copy has run)."""
     return t if t.is_cuda else t.pin_memory()
+
+
+def check_policy(policy) -> str:
+    if not isinstance(policy, str) or policy not in POLICIES:
+        raise ValueError(f"BatchTree policy {policy!r} is not supported (only {POLICIES}); greedys, specinfer and the "
+                         "*TreeTest policies run one sequence at a time")
+    return policy
+
+
+def _policies(policy, B: int) -> List[str]:
+    """One policy string for all B sequences, or a sequence of B strings."""
+    if isinstance(policy, str) or not isinstance(policy, Sequence):
+        return [check_policy(policy)] * B
+    pols = [check_policy(p) for p in policy]
+    if len(pols) != B:
+        raise ValueError(f"policy: {len(pols)} values for {B} sequences")
+    return pols
 
 
 def check_sampling(temperature: float, top_p: float):
@@ -79,20 +100,21 @@ def _as_int64(seed: int) -> int:
 class BatchTree:
     """Batched SpecTree ("spec") / GreedyTree ("greedy") over `len(prompts)` sequences.  The engines must have been built
     with batch_size == len(prompts).  verify() returns one (valid_tokens, accept_length, terminal) per sequence.
-    temperature and top_p: one value for all sequences, or one per sequence; "greedy" ignores both.
+    policy: one of "spec" / "greedy" for all sequences, or one per sequence.
+    temperature and top_p: one value for all sequences, or one per sequence; "greedy" sequences ignore both (their
+    temperature must still be a valid one).
     seeds: None (r and rand drawn with torch's CPU generator as a lone SpecTree draws them, the bonus noise with torch's
     CUDA generator), or one integer in [0, 2^64) per prompt: each sequence then draws all its random numbers on the
     device from a Philox stream keyed by its seed, so its output does not depend on its slot or its neighbours ("greedy"
     takes seeds and ignores them)."""
 
-    def __init__(self, draft, target, prompts: Sequence[torch.Tensor], grow_map: dict, policy: str = "spec",
+    def __init__(self, draft, target, prompts: Sequence[torch.Tensor], grow_map: dict,
+                 policy: Union[str, Sequence[str]] = "spec",
                  temperature: Union[float, Sequence[float]] = 0.6, top_p: Union[float, Sequence[float]] = 1.0,
                  max_length: int = 256, max_target_seq: Optional[int] = None,
                  seeds: Optional[Sequence[int]] = None):
-        if policy not in POLICIES:
-            raise ValueError(f"BatchTree policy {policy!r} is not supported (only {POLICIES}); greedys, specinfer and the "
-                             "*TreeTest policies run one sequence at a time")
         B = len(prompts)
+        policies = _policies(policy, B)
         temps, top_ps = _per_seq(temperature, B, "temperature"), _per_seq(top_p, B, "top_p")
         for t, p in zip(temps, top_ps):
             check_sampling(t, p)
@@ -110,14 +132,18 @@ class BatchTree:
         if dev.type != "cuda":
             raise RuntimeError("sequoia_b200 trees run on a CUDA device only (there is no CPU path)")
         self.draft, self.target = draft, target
-        self.policy, self.greedy = policy, policy == "greedy"
+        self.policies = policies
+        # mixed: both policies present (from here on, for the tree's life); greedy: every sequence greedy, never mixed
+        self.mixed = len(set(policies)) > 1
+        self.greedy = not self.mixed and policies[0] == "greedy"
         self.temps, self.top_ps = temps, top_ps
         self.B, self.M = B, max_length
         self.max_target_seq = max_target_seq or max_length
         self.st = st = _Static(grow_map, dev)
         S = self.S = st.S
         V = self.V = draft.engine.model_config.vocab_size
-        check_vocab(policy, V)
+        for pol in set(policies):
+            check_vocab(pol, V)
         M = max_length
         for p in prompts:
             if len(p) + S - 1 > M:
@@ -125,9 +151,12 @@ class BatchTree:
         self.device = dev
         # sampling parameters live on the device, so the captured graphs serve any values an admission brings; the top-p
         # filter joins the steady / post graphs only once a sequence has had top_p < 1 (one recapture, see admit)
+        # (a greedy sequence's top_p is 1 on the device, so the filter leaves its rows alone)
         self.T_dev = torch.tensor(temps, dtype=torch.float32, device=dev)
-        self.top_p_dev = torch.tensor(top_ps, dtype=torch.float32, device=dev)
-        self.use_top_p = not self.greedy and any(p < 1.0 for p in top_ps)
+        self.top_p_dev = torch.tensor([1.0 if pol == "greedy" else p for pol, p in zip(policies, top_ps)],
+                                      dtype=torch.float32, device=dev)
+        self.greedy_dev = torch.tensor([pol == "greedy" for pol in policies], dtype=torch.int32, device=dev)
+        self.use_top_p = any(pol == "spec" and p < 1.0 for pol, p in zip(policies, top_ps))
         i64 = dict(dtype=torch.int64, device=dev)
         self.tokens = torch.zeros(B, M, **i64)
         self.position_ids = torch.zeros(B, M, **i64)
@@ -159,6 +188,8 @@ class BatchTree:
         if self.seeded:
             self.seeds = torch.tensor([_as_int64(s) for s in seeds], **i64)
             self.steps = torch.zeros(B, **i64)
+        # r and rand: for every slot once any sequence samples (CPU draws for every prompt in prompt order, greedy ones
+        # included, so a sampling sequence's numbers do not depend on its neighbours' policies)
         if self.greedy:
             self.r = self.rand = None
         elif self.seeded:
@@ -206,12 +237,17 @@ class BatchTree:
 
     @torch.inference_mode()
     def admit(self, b: int, prompt: torch.Tensor, temperature: Optional[float] = None, top_p: Optional[float] = None,
-              seed: Optional[int] = None):
-        """Start `prompt` in the frozen slot b (finished, out of room, or stopped with freeze), at its own temperature and
-        top_p (default: the slot's previous values).  The next verify() runs its first verify next to the steady
-        sequences.  The slot draws r and rand as a lone SpecTree on the prompt would, and runs its draft prefill now.
+              seed: Optional[int] = None, policy: Optional[str] = None):
+        """Start `prompt` in the frozen slot b (finished, out of room, or stopped with freeze), at its own policy,
+        temperature and top_p (default: the slot's previous values).  The next verify() runs its first verify next to the
+        steady sequences.  The slot draws r and rand as a lone SpecTree on the prompt would, and runs its draft prefill now.
         A seeded tree takes the prompt's `seed` (required there, refused otherwise): r and rand are then filled on the
-        device from that seed's stream and the slot's noise counter restarts at 0."""
+        device from that seed's stream and the slot's noise counter restarts at 0.
+        The first admission that puts both policies in the batch starts mixed mode: the draft, steady and post graphs are
+        captured once more, on their next use.  A tree built all-greedy allocates r and rand at its first "spec"
+        admission."""
+        if policy is not None:
+            check_policy(policy)
         if not 0 <= b < self.B:
             raise IndexError(f"slot {b} out of range for a batch of {self.B}")
         if not self.frozen[b]:
@@ -228,13 +264,25 @@ class BatchTree:
             raise ValueError("seed= needs a BatchTree built with seeds")
         if seed is not None:
             seed = check_seed(seed)
-        self.temps[b], self.top_ps[b] = T, tp
+        pol = self.policies[b] if policy is None else policy
+        # (every other slot holds the tree's one policy until then, so a different one means both are present; at B = 1
+        # it is a switch, which the single-policy graphs do not serve either)
+        enter_mixed = not self.mixed and pol != ("greedy" if self.greedy else "spec")
+        self.temps[b], self.top_ps[b], self.policies[b] = T, tp, pol
         self.T_dev[b] = T
-        self.top_p_dev[b] = tp
-        if tp < 1.0 and not self.greedy and not self.use_top_p:
+        self.top_p_dev[b] = 1.0 if pol == "greedy" else tp
+        self.greedy_dev[b] = 1 if pol == "greedy" else 0
+        if enter_mixed:
+            self.mixed, self.greedy = True, False  # the mixed sampler and walks enter every graph: capture them once more
+            for name in ("draft", "steady", "post"):
+                self.graphs.pop(name, None)
+        if tp < 1.0 and pol == "spec" and not self.use_top_p:
             self.use_top_p = True                  # the filter enters op_accept: capture steady and post once more
             for name in ("steady", "post"):
                 self.graphs.pop(name, None)
+        if pol == "spec" and self.r is None:       # the first sampling sequence of a tree built all-greedy
+            self.r = torch.zeros(self.B, self.M, dtype=F16, device=self.device)
+            self.rand = torch.zeros(self.B, self.S, self.V, dtype=F16, device=self.device)
         self._load_prompt(b, prompt)
         self.frozen[b] = False
         self.last[b] = None
@@ -243,10 +291,10 @@ class BatchTree:
         if self.seeded:
             self.seeds[b] = _as_int64(seed)
             self.steps[b] = 0
-            if not self.greedy:
+            if pol == "spec":
                 ops.rng_uniform_seqs(self.r, self.seeds, [b], ops.RNG_R)
                 ops.rng_uniform_seqs(self.rand, self.seeds, [b], ops.RNG_RAND)
-        elif not self.greedy:
+        elif self.r is not None:                   # (a greedy prompt of a mixed batch draws too: stream alignment)
             r, rand = draw_random([prompt], self.M, self.S, self.V)
             self.r[b].copy_(_h2d(r[0]), non_blocking=True)
             self.rand[b].copy_(_h2d(rand[0]), non_blocking=True)
@@ -255,6 +303,11 @@ class BatchTree:
     # ---- the op sequences ------------------------------------------------------------------------------------------------
     def op_sample(self, i: int):
         lv = self.st.levels[i]
+        if self.mixed:
+            ops.sample_level_batch_mixed(self.draft_logits, self.row_base, self.row_step, self.rand, lv["n_parents"],
+                                         lv["k"], self.T_dev, self.greedy_dev, parent_rows=lv["parents"],
+                                         child_first=lv["first"], n_branch=lv["nb"], tokens=self.tokens, state=self.state)
+            return
         ops.sample_level_batch_per_seq(self.draft_logits, self.row_base, self.row_step, self.rand, lv["n_parents"],
                                        lv["k"], self.T_dev, 1 if self.greedy else 0, parent_rows=lv["parents"],
                                        child_first=lv["first"], n_branch=lv["nb"], tokens=self.tokens, state=self.state)
@@ -286,6 +339,11 @@ class BatchTree:
             ops.accept_greedy_batch(self.target_token, st.succ_off, st.succ, st.depth, self.S, self.tokens,
                                     self.position_ids, self.accept_idx, self.state, self.max_target_seq)
             return
+        if self.mixed:                             # the greedy sequences' walk; the sampling ones' follows below
+            ops.argmax_rows(self.target_logits, self.target_token)
+            ops.accept_greedy_batch_mixed(self.target_token, st.succ_off, st.succ, st.depth, self.S, self.greedy_dev,
+                                          self.tokens, self.position_ids, self.accept_idx, self.state,
+                                          self.max_target_seq)
         if self.use_top_p:
             ops.top_p_filter_per_seq_(self.target_logits, self.top_p_dev, self.T_dev, self.S)
         if self.external_noise is None:
@@ -293,6 +351,12 @@ class BatchTree:
                 ops.rng_exponential_batch(self.noise, self.seeds, self.steps, self.state)
             else:
                 self.noise.exponential_(1.0)
+        if self.mixed:
+            ops.accept_stochastic_batch_mixed(self.target_logits, self.draft_logits, self.row_base, self.row_step, self.r,
+                                              self.noise, st.succ_off, st.succ, st.depth, self.S, self.T_dev,
+                                              self.greedy_dev, self.tokens, self.position_ids, self.accept_idx, self.state,
+                                              self.max_target_seq)
+            return
         ops.accept_stochastic_batch_per_seq(self.target_logits, self.draft_logits, self.row_base, self.row_step, self.r,
                                             self.noise, st.succ_off, st.succ, st.depth, self.S, self.T_dev, self.tokens,
                                             self.position_ids, self.accept_idx, self.state, self.max_target_seq)

@@ -196,12 +196,15 @@ __global__ void __launch_bounds__(ANT) accept_stochastic_kernel(
 }
 
 // BATCH: grid (B), one walk per sequence; target_token rows of S per sequence, the rest as in BatchArgs.
-template <bool BATCH>
+// MIXED (BATCH only): only the sequences with greedy[b] nonzero walk; the others' blocks exit as a frozen one does.
+template <bool BATCH, bool MIXED = false>
 __global__ void accept_greedy_kernel(const int64_t* __restrict__ target_token, const int32_t* __restrict__ succ_off,
                                      const int32_t* __restrict__ succ, const int32_t* __restrict__ depth, int S,
                                      int64_t* __restrict__ tokens, int64_t* __restrict__ position_ids,
                                      int32_t* __restrict__ accept_idx, int32_t* __restrict__ state,
-                                     int max_target_seq, int64_t ld_seq, int64_t ld_acc) {
+                                     int max_target_seq, int64_t ld_seq, int64_t ld_acc,
+                                     const int32_t* __restrict__ greedy) {
+  static_assert(BATCH || !MIXED, "a per-sequence policy needs the batched kernel");
   __shared__ int32_t sh_acc[1024];
   __shared__ int sh_n, sh_term;
   __shared__ long long sh_bonus;
@@ -209,6 +212,7 @@ __global__ void accept_greedy_kernel(const int64_t* __restrict__ target_token, c
   if (BATCH) {
     state += b * ST_WORDS;
     if (state[ST_FROZEN]) return;
+    if (MIXED && !greedy[b]) return;
     target_token += (int64_t)b * S;
     tokens += b * ld_seq;
     position_ids += b * ld_seq;
@@ -275,8 +279,29 @@ extern "C" int sq_accept_greedy(const int64_t* target_token, const int32_t* succ
                                 int32_t* accept_idx, int32_t* state, int max_target_seq, void* stream) {
   SQ_CHECK_ARG(S >= 1 && S <= 1024, "sq_accept_greedy: S=%d unsupported", S);
   accept_greedy_kernel<false><<<1, 256, 0, (cudaStream_t)stream>>>(target_token, succ_off, succ, depth, S, tokens,
-                                                                   position_ids, accept_idx, state, max_target_seq, 0, 0);
+                                                                   position_ids, accept_idx, state, max_target_seq, 0, 0,
+                                                                   nullptr);
   SQ_CHECK_LAUNCH("sq_accept_greedy");
+  return SQ_OK;
+}
+
+// sq_accept_greedy_batch (greedy == nullptr) and its mixed-policy form
+static int accept_greedy_batch(const char* name, const int64_t* target_token, const int32_t* succ_off,
+                               const int32_t* succ, const int32_t* depth, int S, int64_t* tokens, int64_t* position_ids,
+                               int64_t ld_seq, int32_t* accept_idx, int64_t ld_acc, int32_t* state, int B,
+                               int max_target_seq, const int32_t* greedy, void* stream) {
+  SQ_CHECK_ARG(S >= 1 && S <= 1024, "%s: S=%d unsupported", name, S);
+  SQ_CHECK_ARG(B >= 1 && B <= SQ_MAX_BATCH, "%s: B=%d (1..%d)", name, B, SQ_MAX_BATCH);
+  SQ_CHECK_ARG(ld_acc >= S && ld_seq >= 1, "%s: accept_idx rows of %lld < S=%d", name, (long long)ld_acc, S);
+  if (greedy)
+    accept_greedy_kernel<true, true><<<B, 256, 0, (cudaStream_t)stream>>>(
+        target_token, succ_off, succ, depth, S, tokens, position_ids, accept_idx, state, max_target_seq, ld_seq, ld_acc,
+        greedy);
+  else
+    accept_greedy_kernel<true><<<B, 256, 0, (cudaStream_t)stream>>>(target_token, succ_off, succ, depth, S, tokens,
+                                                                    position_ids, accept_idx, state, max_target_seq,
+                                                                    ld_seq, ld_acc, nullptr);
+  SQ_CHECK_LAUNCH(name);
   return SQ_OK;
 }
 
@@ -284,30 +309,33 @@ extern "C" int sq_accept_greedy_batch(const int64_t* target_token, const int32_t
                                       const int32_t* depth, int S, int64_t* tokens, int64_t* position_ids, int64_t ld_seq,
                                       int32_t* accept_idx, int64_t ld_acc, int32_t* state, int B, int max_target_seq,
                                       void* stream) {
-  SQ_CHECK_ARG(S >= 1 && S <= 1024, "sq_accept_greedy_batch: S=%d unsupported", S);
-  SQ_CHECK_ARG(B >= 1 && B <= SQ_MAX_BATCH, "sq_accept_greedy_batch: B=%d (1..%d)", B, SQ_MAX_BATCH);
-  SQ_CHECK_ARG(ld_acc >= S && ld_seq >= 1, "sq_accept_greedy_batch: accept_idx rows of %lld < S=%d", (long long)ld_acc, S);
-  accept_greedy_kernel<true><<<B, 256, 0, (cudaStream_t)stream>>>(target_token, succ_off, succ, depth, S, tokens,
-                                                                  position_ids, accept_idx, state, max_target_seq, ld_seq,
-                                                                  ld_acc);
-  SQ_CHECK_LAUNCH("sq_accept_greedy_batch");
-  return SQ_OK;
+  return accept_greedy_batch("sq_accept_greedy_batch", target_token, succ_off, succ, depth, S, tokens, position_ids, ld_seq,
+                             accept_idx, ld_acc, state, B, max_target_seq, nullptr, stream);
 }
 
-// sq_accept_stochastic_batch (T_seq == nullptr) and its per-sequence form
+extern "C" int sq_accept_greedy_batch_mixed(const int64_t* target_token, const int32_t* succ_off, const int32_t* succ,
+                                            const int32_t* depth, int S, int64_t* tokens, int64_t* position_ids,
+                                            int64_t ld_seq, int32_t* accept_idx, int64_t ld_acc, int32_t* state,
+                                            const int32_t* greedy, int B, int max_target_seq, void* stream) {
+  SQ_CHECK_ARG(greedy != nullptr, "sq_accept_greedy_batch_mixed: null greedy array");
+  return accept_greedy_batch("sq_accept_greedy_batch_mixed", target_token, succ_off, succ, depth, S, tokens, position_ids,
+                             ld_seq, accept_idx, ld_acc, state, B, max_target_seq, greedy, stream);
+}
+
+// sq_accept_stochastic_batch (T_seq == nullptr), its per-sequence form and (greedy != nullptr) the mixed-policy form
 static int accept_stochastic_batch(const char* name, const sq_half* target_logits, int64_t ld_t,
                                    const sq_half* draft_logits, int64_t ld_d, const int32_t* row_base,
                                    const int32_t* row_step, const sq_half* r, const sq_half* noise, int64_t ld_noise,
                                    const int32_t* succ_off, const int32_t* succ, const int32_t* depth, int S, int V,
                                    float T, const float* T_seq, int64_t* tokens, int64_t* position_ids, int64_t ld_seq,
                                    int32_t* accept_idx, int64_t ld_acc, int32_t* state, int B, int max_target_seq,
-                                   int policy, void* stream) {
+                                   int policy, void* stream, const int32_t* greedy = nullptr) {
   SQ_CHECK_ARG(S >= 1 && S <= 1024, "%s: S=%d unsupported", name, S);
   SQ_CHECK_ARG(B >= 1 && B <= SQ_MAX_BATCH, "%s: B=%d (1..%d)", name, B, SQ_MAX_BATCH);
   SQ_CHECK_ARG((policy & ~3) == 0, "%s: unknown policy bits %d", name, policy);
   SQ_CHECK_ARG(row_base && row_step, "%s: null draft-row table", name);
   SQ_CHECK_ARG(ld_acc >= S && ld_noise >= V, "%s: accept_idx / noise rows too short", name);
-  BatchArgs ba{B, ld_seq, ld_noise, ld_acc, row_base, row_step};
+  BatchArgs ba{B, ld_seq, ld_noise, ld_acc, row_base, row_step, greedy};
   return sq::launch_accept_cluster(target_logits, ld_t, draft_logits, ld_d, r, noise, succ_off, succ, depth, S, V, T, tokens,
                                    position_ids, accept_idx, state, max_target_seq, policy, stream, &ba, T_seq);
 }
@@ -335,4 +363,17 @@ extern "C" int sq_accept_stochastic_batch_per_seq(const sq_half* target_logits, 
   return accept_stochastic_batch("sq_accept_stochastic_batch_per_seq", target_logits, ld_t, draft_logits, ld_d, row_base,
                                  row_step, r, noise, ld_noise, succ_off, succ, depth, S, V, 1.0f, T, tokens, position_ids,
                                  ld_seq, accept_idx, ld_acc, state, B, max_target_seq, policy, stream);
+}
+
+extern "C" int sq_accept_stochastic_batch_mixed(const sq_half* target_logits, int64_t ld_t, const sq_half* draft_logits,
+                                                int64_t ld_d, const int32_t* row_base, const int32_t* row_step,
+                                                const sq_half* r, const sq_half* noise, int64_t ld_noise,
+                                                const int32_t* succ_off, const int32_t* succ, const int32_t* depth, int S,
+                                                int V, const float* T, const int32_t* greedy, int64_t* tokens,
+                                                int64_t* position_ids, int64_t ld_seq, int32_t* accept_idx, int64_t ld_acc,
+                                                int32_t* state, int B, int max_target_seq, int policy, void* stream) {
+  SQ_CHECK_ARG(T != nullptr && greedy != nullptr, "sq_accept_stochastic_batch_mixed: null temperature or greedy array");
+  return accept_stochastic_batch("sq_accept_stochastic_batch_mixed", target_logits, ld_t, draft_logits, ld_d, row_base,
+                                 row_step, r, noise, ld_noise, succ_off, succ, depth, S, V, 1.0f, T, tokens, position_ids,
+                                 ld_seq, accept_idx, ld_acc, state, B, max_target_seq, policy, stream, greedy);
 }

@@ -77,7 +77,9 @@ struct ClusterCtx {
 // exchange (the whole cluster reads the same word).
 // PER_SEQ (BATCH only): `temp` is the (B,) temperature array and the walk of sequence b scales both the target and the
 // draft rows by 1/T[b]; otherwise `temp` is the scalar 1/T.
-template <bool BATCH, int NCH, bool PER_SEQ = false>
+// MIXED (PER_SEQ only): the cluster of a sequence with ba.greedy[b] nonzero exits where a frozen one does and writes
+// nothing (its walk is the greedy kernel's).
+template <bool BATCH, int NCH, bool PER_SEQ = false, bool MIXED = false>
 __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(CNT) accept_stochastic_cluster_kernel(
     const __half* __restrict__ target_logits, int64_t ld_t, const __half* __restrict__ draft_logits, int64_t ld_d,
     const __half* __restrict__ r, const __half* __restrict__ noise, const int32_t* __restrict__ succ_off,
@@ -85,6 +87,7 @@ __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(CNT) accept_stochas
     int64_t* __restrict__ tokens, int64_t* __restrict__ position_ids, int32_t* __restrict__ accept_idx,
     int32_t* __restrict__ state, int max_target_seq, int policy, BatchArgs ba) {
   static_assert(BATCH || !PER_SEQ, "per-sequence parameters need the batched kernel");
+  static_assert(PER_SEQ || !MIXED, "a per-sequence policy needs the per-sequence temperature");
   __shared__ Xch xch;
   __shared__ float red[CNW];
   __shared__ int32_t sh_acc[1024];
@@ -94,6 +97,7 @@ __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(CNT) accept_stochas
   if (BATCH) {
     state += b * ST_WORDS;
     if (state[ST_FROZEN]) return;
+    if (MIXED && ba.greedy[b]) return;
     target_logits += (int64_t)b * S * ld_t;
     r += b * ba.ld_seq;
     noise += b * ba.ld_noise;
@@ -299,6 +303,13 @@ static int launch_accept_nch(const sq_half* target_logits, int64_t ld_t, const s
                              const int32_t* depth, int S, int V, float T, int64_t* tokens, int64_t* position_ids,
                              int32_t* accept_idx, int32_t* state, int max_target_seq, int policy, void* stream,
                              const BatchArgs* batch, const float* T_seq) {
+  if (batch && T_seq && batch->greedy) {
+    accept_stochastic_cluster_kernel<true, NCH, true, true><<<dim3(CL, batch->B), CNT, 0, (cudaStream_t)stream>>>(
+        (const __half*)target_logits, ld_t, (const __half*)draft_logits, ld_d, (const __half*)r, (const __half*)noise,
+        succ_off, succ, depth, S, V, T_seq, tokens, position_ids, accept_idx, state, max_target_seq, policy, *batch);
+    SQ_CHECK_LAUNCH("sq_accept_stochastic_batch_mixed");
+    return SQ_OK;
+  }
   if (batch && T_seq) {
     accept_stochastic_cluster_kernel<true, NCH, true><<<dim3(CL, batch->B), CNT, 0, (cudaStream_t)stream>>>(
         (const __half*)target_logits, ld_t, (const __half*)draft_logits, ld_d, (const __half*)r, (const __half*)noise,

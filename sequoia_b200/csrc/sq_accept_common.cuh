@@ -6,12 +6,14 @@ namespace sq {
 
 // Per-sequence addressing of the batched walks (sequence b = blockIdx.y): tokens / position_ids / r rows of ld_seq
 // elements, noise rows of ld_noise, accept_idx rows of ld_acc, target logits (B*S, V), and the draft-logit row of node k
-// at row_base[k] + b * row_step[k].
+// at row_base[k] + b * row_step[k].  greedy: the (B,) per-sequence policy of the mixed walks (nonzero = greedy), nullptr
+// for every other batched walk.
 struct BatchArgs {
   int B;
   int64_t ld_seq, ld_noise, ld_acc;
   const int32_t* row_base;
   const int32_t* row_step;
+  const int32_t* greedy = nullptr;
   template <bool BATCH>
   __device__ __forceinline__ int64_t row(int node, int b) const {
     return BATCH ? (int64_t)row_base[node] + (int64_t)b * row_step[node] : node;

@@ -190,14 +190,22 @@ __device__ __forceinline__ void wide_topk_merge(const uint64_t* gk, int n, int k
 // WIDE: grid (n * n_parents, B), clusters of n = ceil(V / SLICE) CTAs; the whole cluster reads the same frozen word and
 // k_need, so it takes every exit together.
 // PER_SEQ (BATCH only): `temp` is the (B,) temperature array and mode 0 uses T[b]; otherwise `temp` is the scalar 1/T.
-template <bool BATCH, bool WIDE, bool PER_SEQ = false>
+// MIXED (PER_SEQ only): `mode` is the (B,) int32 `greedy` array: sequence b draws as mode 1 when greedy[b] is nonzero, else
+// as mode 0 at T[b].  b is the grid's y index, so the choice is uniform per block (per cluster when WIDE).
+template <bool MIXED>
+using ModeArg = typename std::conditional<MIXED, const int32_t*, int>::type;
+__device__ __forceinline__ int seq_mode(int mode, int) { return mode; }
+__device__ __forceinline__ int seq_mode(const int32_t* greedy, int b) { return greedy[b] ? 1 : 0; }
+
+template <bool BATCH, bool WIDE, bool PER_SEQ = false, bool MIXED = false>
 __global__ void __launch_bounds__(NT) sample_level_kernel(
     const __half* __restrict__ logits, int64_t ld_logits, const __half* __restrict__ rand, int64_t ld_rand,
     const int32_t* __restrict__ parent_rows, const int32_t* __restrict__ child_first,
-    const int32_t* __restrict__ n_branch, int k_max, int V, SeqParam<PER_SEQ> temp, int mode,
+    const int32_t* __restrict__ n_branch, int k_max, int V, SeqParam<PER_SEQ> temp, ModeArg<MIXED> mode,
     int64_t* __restrict__ positions, int64_t* __restrict__ tokens, const int32_t* __restrict__ state,
     const int32_t* __restrict__ drow_base, const int32_t* __restrict__ drow_step, int64_t ld_rand_seq, int64_t ld_seq) {
   static_assert(BATCH || !PER_SEQ, "per-sequence parameters need the batched kernel");
+  static_assert(PER_SEQ || !MIXED, "a per-sequence policy needs the per-sequence temperature");
   __shared__ float red[NW];
   __shared__ uint32_t redu[NW];
   Slice sl{};
@@ -228,7 +236,7 @@ __global__ void __launch_bounds__(NT) sample_level_kernel(
   {
     Pack8 x[CH];
     load_row(logits + lrow * ld_logits, V, x);
-    if (mode == 0) {
+    if (seq_mode(mode, b) == 0) {
       const float inv_T = inv_temp(temp, b);
       float mx, sum;
       if constexpr (WIDE) {
@@ -751,6 +759,10 @@ using namespace sq;
   SQ_CHECK_ARG((V) % 8 == 0 && (V) > 0 && (V) <= SLICE * MAX_SLICES, "V=%d must be a multiple of 8, <= %d", (V), \
                SLICE * MAX_SLICES)
 
+// the host's view of a sample_level_batch `mode` argument: 0 / 1, or 0 for a greedy array (some sequence may sample)
+static int seq_mode_host(int mode) { return mode; }
+static int seq_mode_host(const int32_t*) { return 0; }
+
 // V > SLICE: `rows` clusters of ceil(V / SLICE) CTAs along x (times grid_y)
 template <typename... KArgs, typename... Args>
 static cudaError_t launch_wide(void (*kern)(KArgs...), int rows, int grid_y, int V, cudaStream_t st, Args&&... args) {
@@ -814,30 +826,32 @@ extern "C" int sq_sample_level(const sq_half* logits, int64_t ld_logits, const s
   return SQ_OK;
 }
 
-// sq_sample_level_batch and its per-sequence form: `temp` is 1/T (PER_SEQ = false) or the (B,) T array
-template <bool PER_SEQ>
+// sq_sample_level_batch and its per-sequence forms: `temp` is 1/T (PER_SEQ = false) or the (B,) T array; `mode` is 0 / 1
+// or (MIXED) the (B,) greedy array
+template <bool PER_SEQ, bool MIXED = false>
 static int sample_level_batch(const char* name, const sq_half* logits, int64_t ld_logits, const int32_t* row_base,
                               const int32_t* row_step, const sq_half* rand, int64_t ld_rand, int64_t ld_rand_seq,
                               const int32_t* parent_rows, const int32_t* child_first, const int32_t* n_branch,
-                              int n_parents, int k_max, int V, SeqParam<PER_SEQ> temp, int mode, int64_t* tokens,
-                              int64_t ld_seq, const int32_t* state, int B, void* stream) {
+                              int n_parents, int k_max, int V, SeqParam<PER_SEQ> temp, ModeArg<MIXED> mode,
+                              int64_t* tokens, int64_t ld_seq, const int32_t* state, int B, void* stream) {
   SQ_CHECK_V_WIDE(V);
   SQ_CHECK_ARG(B >= 1 && B <= SQ_MAX_BATCH, "%s: B=%d (1..%d)", name, B, SQ_MAX_BATCH);
   if (n_parents == 0 || k_max == 0) return SQ_OK;
-  SQ_CHECK_ARG(mode == 1 || rand != nullptr, "%s: rand required for mode 0", name);
+  // (MIXED: any sequence may draw as mode 0, so rand is always required)
+  SQ_CHECK_ARG(seq_mode_host(mode) == 1 || rand != nullptr, "%s: rand required for mode 0", name);
   SQ_CHECK_ARG(tokens && child_first && n_branch && parent_rows && state && row_base && row_step,
                "%s: null table or buffer", name);
   SQ_CHECK_ARG(k_max <= V, "%s: k_max > V", name);
   if (V > SLICE) {
     SQ_CHECK_ARG(k_max <= WIDE_KMAX, "%s: k_max=%d > %d with V > %d", name, k_max, WIDE_KMAX, SLICE);
-    SQ_CHECK_WIDE_LAUNCH(launch_wide(sample_level_kernel<true, true, PER_SEQ>, n_parents, B, V, (cudaStream_t)stream,
+    SQ_CHECK_WIDE_LAUNCH(launch_wide(sample_level_kernel<true, true, PER_SEQ, MIXED>, n_parents, B, V, (cudaStream_t)stream,
                                      (const __half*)logits, ld_logits, (const __half*)rand, ld_rand, parent_rows,
                                      child_first, n_branch, k_max, V, temp, mode, (int64_t*)nullptr, tokens, state,
                                      row_base, row_step, ld_rand_seq, ld_seq),
                          name);
     return SQ_OK;
   }
-  sample_level_kernel<true, false, PER_SEQ><<<dim3(n_parents, B), NT, 0, (cudaStream_t)stream>>>(
+  sample_level_kernel<true, false, PER_SEQ, MIXED><<<dim3(n_parents, B), NT, 0, (cudaStream_t)stream>>>(
       (const __half*)logits, ld_logits, (const __half*)rand, ld_rand, parent_rows, child_first, n_branch, k_max, V, temp,
       mode, nullptr, tokens, state, row_base, row_step, ld_rand_seq, ld_seq);
   SQ_CHECK_LAUNCH(name);
@@ -864,6 +878,18 @@ extern "C" int sq_sample_level_batch_per_seq(const sq_half* logits, int64_t ld_l
   return sample_level_batch<true>("sq_sample_level_batch_per_seq", logits, ld_logits, row_base, row_step, rand, ld_rand,
                                   ld_rand_seq, parent_rows, child_first, n_branch, n_parents, k_max, V, T, mode, tokens,
                                   ld_seq, state, B, stream);
+}
+
+extern "C" int sq_sample_level_batch_mixed(const sq_half* logits, int64_t ld_logits, const int32_t* row_base,
+                                           const int32_t* row_step, const sq_half* rand, int64_t ld_rand,
+                                           int64_t ld_rand_seq, const int32_t* parent_rows, const int32_t* child_first,
+                                           const int32_t* n_branch, int n_parents, int k_max, int V, const float* T,
+                                           const int32_t* greedy, int64_t* tokens, int64_t ld_seq, const int32_t* state,
+                                           int B, void* stream) {
+  SQ_CHECK_ARG(T != nullptr && greedy != nullptr, "sq_sample_level_batch_mixed: null temperature or greedy array");
+  return sample_level_batch<true, true>("sq_sample_level_batch_mixed", logits, ld_logits, row_base, row_step, rand,
+                                        ld_rand, ld_rand_seq, parent_rows, child_first, n_branch, n_parents, k_max, V, T,
+                                        greedy, tokens, ld_seq, state, B, stream);
 }
 
 // Sampling with replacement (the SpecInfer policy) has no large-vocabulary instance: V <= 32768 only.

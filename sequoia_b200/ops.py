@@ -595,3 +595,55 @@ def accept_greedy_batch(target_token, succ_off, succ, depth, S, tokens, position
                                              ptr(position_ids), ld, ptr(accept_idx), _rows(accept_idx, "accept_idx"),
                                              ptr(state), state.shape[0], max_target_seq, stream_ptr()),
           "sq_accept_greedy_batch")
+
+
+# ---- per-sequence policy: greedy and sampled sequences in one batch (include/sequoia_b200.h) -----------------------------
+def _greedy_arg(greedy, B, name):
+    if greedy is None or greedy.dtype != torch.int32 or not greedy.is_cuda or greedy.dim() != 1 or greedy.shape[0] < B \
+            or greedy.stride(0) != 1:
+        raise TypeError(f"{name}: greedy must be a contiguous ({B},) int32 CUDA tensor (nonzero = greedy)")
+
+
+def sample_level_batch_mixed(logits, row_base, row_step, rand, n_parents, k_max, T, greedy, *, parent_rows, child_first,
+                             n_branch, tokens, state):
+    """sample_level_batch_per_seq with sequence b drawing as mode 1 (top-k) when greedy[b] != 0, else as mode 0 at T[b].
+    rand: (B, S, V), required (its rows of greedy sequences are not read)."""
+    B = state.shape[0]
+    _seq_params("sample_level_batch_mixed", B, T=T)
+    _greedy_arg(greedy, B, "sample_level_batch_mixed")
+    if rand is not None:
+        assert rand.dim() == 3 and rand.stride(-1) == 1
+    check(_lib.load().sq_sample_level_batch_mixed(
+        ptr(logits), logits.stride(0), ptr(row_base), ptr(row_step), ptr(rand), rand.stride(1) if rand is not None else 0,
+        rand.stride(0) if rand is not None else 0, ptr(parent_rows), ptr(child_first), ptr(n_branch), n_parents, k_max,
+        logits.shape[-1], ptr(T), ptr(greedy), ptr(tokens), _rows(tokens, "tokens"), ptr(state), B, stream_ptr()),
+        "sq_sample_level_batch_mixed")
+
+
+def accept_greedy_batch_mixed(target_token, succ_off, succ, depth, S, greedy, tokens, position_ids, accept_idx, state,
+                              max_target_seq):
+    """accept_greedy_batch for the sequences with greedy[b] != 0 only."""
+    B = state.shape[0]
+    _greedy_arg(greedy, B, "accept_greedy_batch_mixed")
+    ld = _rows(tokens, "tokens")
+    assert _rows(position_ids, "position_ids") == ld
+    check(_lib.load().sq_accept_greedy_batch_mixed(ptr(target_token), ptr(succ_off), ptr(succ), ptr(depth), S, ptr(tokens),
+                                                   ptr(position_ids), ld, ptr(accept_idx), _rows(accept_idx, "accept_idx"),
+                                                   ptr(state), ptr(greedy), B, max_target_seq, stream_ptr()),
+          "sq_accept_greedy_batch_mixed")
+
+
+def accept_stochastic_batch_mixed(target_logits, draft_logits, row_base, row_step, r, noise, succ_off, succ, depth, S, T,
+                                  greedy, tokens, position_ids, accept_idx, state, max_target_seq, policy=0):
+    """accept_stochastic_batch_per_seq for the sequences with greedy[b] == 0 only."""
+    B = state.shape[0]
+    _seq_params("accept_stochastic_batch_mixed", B, T=T)
+    _greedy_arg(greedy, B, "accept_stochastic_batch_mixed")
+    V = target_logits.shape[-1]
+    ld = _rows(tokens, "tokens")
+    assert _rows(position_ids, "position_ids") == ld and _rows(r, "r") == ld
+    check(_lib.load().sq_accept_stochastic_batch_mixed(
+        ptr(target_logits), target_logits.stride(0), ptr(draft_logits), draft_logits.stride(0), ptr(row_base),
+        ptr(row_step), ptr(r), ptr(noise), _rows(noise, "noise"), ptr(succ_off), ptr(succ), ptr(depth), S, V, ptr(T),
+        ptr(greedy), ptr(tokens), ptr(position_ids), ld, ptr(accept_idx), _rows(accept_idx, "accept_idx"), ptr(state), B,
+        max_target_seq, policy, stream_ptr()), "sq_accept_stochastic_batch_mixed")

@@ -188,12 +188,13 @@ def simulation_baseline(target, prompts, T, top_p, M, new_tokens: int = 32, stop
     return dict(decoded_tokens=decoded, seconds=total_time, latency=total_time / max(decoded, 1))
 
 
-def decode_refill(tree, prompts, limits, stop=DEFAULT_STOP, step_times=None, seeds=None):
+def decode_refill(tree, prompts, limits, stop=DEFAULT_STOP, step_times=None, seeds=None, policies=None):
     """Decode every prompt of a queue on a BatchTree whose B slots start with prompts[:B]: each slot that finishes (a stop
     token, its length limit `limits[i]`, or out of room) takes the next prompt, until the queue is empty.
     -> (outputs, decoded tokens, per-sequence target steps, admission order); outputs[i] = prompt i's committed tokens.
     step_times: a list that receives ("steady" | "admission", seconds) per step; an admission step is timed from the
-    first admit() of the step to the end of its verify.  seeds: for a seeded tree, prompt i's seed is seeds[i]."""
+    first admit() of the step to the end of its verify.  seeds: for a seeded tree, prompt i's seed is seeds[i].
+    policies: prompt i decodes with policies[i] ("spec" / "greedy"); None keeps each slot's policy."""
     B = len(tree.frozen)
     slot = list(range(B))                        # prompt index decoding in each slot (None: the queue ran out)
     length = [len(p) for p in prompts[:B]]
@@ -203,10 +204,12 @@ def decode_refill(tree, prompts, limits, stop=DEFAULT_STOP, step_times=None, see
     while any(i is not None for i in slot):
         t0 = time.perf_counter()
         for b in pending:
-            if seeds is None:
-                tree.admit(b, prompts[slot[b]])
-            else:
-                tree.admit(b, prompts[slot[b]], seed=seeds[slot[b]])
+            kw = {}
+            if seeds is not None:
+                kw["seed"] = seeds[slot[b]]
+            if policies is not None:
+                kw["policy"] = policies[slot[b]]
+            tree.admit(b, prompts[slot[b]], **kw)
         kind = "admission" if pending else "steady"
         pending = []
         tree.construct_grow_map()
@@ -259,11 +262,11 @@ def decode_chunk(tree, chunk, limits, stop=DEFAULT_STOP):
 
 @torch.inference_mode()
 def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: int, stop=DEFAULT_STOP,
-                     refill: bool = False, seeds=None):
+                     refill: bool = False, seeds=None, policies=None):
     """--batch B: the same metric loop with B prompts decoded together (sequoia_b200.batch.BatchTree).  Chunked: B
     prompts at a time, each chunk until its last sequence stops.  refill: one batch whose finished slots take the next
     prompt (BatchTree.admit).  seeds: one per prompt (--device-rng): each sequence draws its random numbers on the device
-    from its own seed."""
+    from its own seed.  policies: one per prompt (--policies), in place of `policy` for all."""
     from sequoia_b200.batch import BatchTree
     steps = decoded = 0                          # steps: target steps summed over sequences (per-sequence tokens / step)
     total_time = 0.0
@@ -272,12 +275,13 @@ def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: i
     chunks = [prompts[:B]] if refill else [prompts[i:i + B] for i in range(0, len(prompts), B)]
     for c, chunk in enumerate(chunks):
         i0 = c * B
-        tree = BatchTree(draft, target, chunk, grow_map, policy=policy, temperature=T, top_p=top_p, max_length=M,
+        pol = policy if policies is None else policies[i0:i0 + len(chunk)]
+        tree = BatchTree(draft, target, chunk, grow_map, policy=pol, temperature=T, top_p=top_p, max_length=M,
                          max_target_seq=M, seeds=None if seeds is None else seeds[i0:i0 + len(chunk)])
         torch.cuda.synchronize()
         t1 = time.time()
         if refill:
-            _, d, s, _ = decode_refill(tree, prompts, limits, stop, seeds=seeds)
+            _, d, s, _ = decode_refill(tree, prompts, limits, stop, seeds=seeds, policies=policies)
         else:
             d, s = decode_chunk(tree, chunk, limits[:len(chunk)], stop)
         decoded += d
@@ -318,6 +322,9 @@ def build_parser():
     ap.add_argument("--device-rng", action="store_true",
                     help="with --batch: each prompt draws its random numbers on the device from a stream of its own, "
                          "seeded (seed << 32) | prompt index, so its output does not depend on its slot or its neighbours")
+    ap.add_argument("--policies", type=str, default=None,
+                    help="with --batch and --tree spec: a comma-separated list of spec / greedy; prompt i decodes with "
+                         "policies[i %% len], greedy and sampled prompts in one batch")
     ap.add_argument("--target-weights", type=str, default="fp16", choices=["fp16", "fp8"],
                     help="fp8: the target's layer projections quantized to E4M3 with per-channel scales at load")
     return ap
@@ -347,6 +354,22 @@ def device_rng_seeds(args, n_prompts: int):
     return [(args.seed << 32) | i for i in range(n_prompts)]
 
 
+def prompt_policies(args, n_prompts: int):
+    """--policies: prompt i's policy policies[i % len]; None without the flag.  Refused without --batch, with a --tree
+    other than spec, and with an entry other than spec / greedy."""
+    if args.policies is None:
+        return None
+    if args.batch == 1 and not args.refill:
+        raise SystemExit("--policies runs with --batch (the batched tree)")
+    if args.tree != "spec":
+        raise SystemExit(f"--policies takes the place of --tree spec, got --tree {args.tree}")
+    pols = [p.strip() for p in args.policies.split(",")]
+    bad = [p for p in pols if p not in ("spec", "greedy")]
+    if bad:
+        raise SystemExit(f"--policies: entries must be spec or greedy, got {args.policies!r}")
+    return [pols[i % len(pols)] for i in range(n_prompts)]
+
+
 def main(argv=None):
     args = build_parser().parse_args(argv)
     print(args)
@@ -359,6 +382,7 @@ def main(argv=None):
     if args.target_weights != "fp16" and args.offloading:
         raise SystemExit("--target-weights fp8 runs without --offloading")
     seeds = device_rng_seeds(args, len(prompts))
+    policies = prompt_policies(args, len(prompts))
     if args.batch != 1 or args.refill:
         B = check_batch_args(args, len(prompts))
         target = GraphInferenceEngineTG(max_length=args.M, model_name_or_path=args.target, dtype=torch.float16,
@@ -369,7 +393,7 @@ def main(argv=None):
         grow_map = torch.load(path)
         assert args.M >= MAX_NEW_LEN + grow_map["size"], "--M must hold 256 tokens + the tree (README.md:47 of the reference)"
         res = simulation_batch(target, draft, prompts, grow_map, args.tree, args.T, args.P, args.M, B, stop=stop,
-                               refill=args.refill, seeds=seeds)
+                               refill=args.refill, seeds=seeds, policies=policies)
         print(json.dumps({k: (round(v, 5) if isinstance(v, float) else v) for k, v in res.items()}))
         return res
     target = (tcls(max_length=args.M, model_name_or_path=args.target, dtype=torch.float16, device=DEV)
