@@ -7,7 +7,8 @@
 //     keeps 192-200 KB per SM in flight; wgmma m64n64k16 (fp16 in, fp32 accumulators in registers), BN/64 per k-step;
 //   * narrow outputs (o_proj / down_proj: N = hidden = 32 slices only) are split along K over a thread-block cluster
 //     (1, SPLIT, 1): each CTA streams 1/SPLIT of K, pushes its fp32 partial rows into the shared memory of the row's
-//     owner CTA (st.shared::cluster), one cluster barrier, owners add in a fixed order and store fp16.
+//     owner CTA (st.shared::cluster), one cluster barrier, owners add in a fixed order and store fp16;
+//     gemm_tn_deep_kernel does the same at split 2 with the full ring, pushing into the owner's ring once it is drained.
 #include <cstdio>
 #include <cstdlib>
 
@@ -18,7 +19,12 @@ struct sq_gemm_plan {
   CUtensorMap tm_a, tm_w;
   __half* c;
   int ldc, n_max, N, K, bn, split, stages, mc, pdl, tiled, epi, n_out;
+  int deep;   // split-K on gemm_tn_deep_kernel (ring as deep as the split-1 instance of that BN)
   int* err_flag;
+#ifdef SQ_GEMM_STAMPS
+  unsigned long long* stamps;
+  int max_clusters;
+#endif
 };
 
 namespace sq {
@@ -30,23 +36,66 @@ struct GemmArgs {
   int m0;                           // first activation / output row of this launch (row tiles of 128 for n > 128)
   int epi, n_out;                   // epi 1: weight rows interleave 16 gate | 16 up rows -> out = silu(gate) * up, n_out columns
   int* err_flag;
+#ifdef SQ_GEMM_STAMPS
+  unsigned long long* stamps;       // per CTA: SM id, %globaltimer at first TMA issue, first full slot, last full slot, exit
+#endif
 };
+
+#ifdef SQ_GEMM_STAMPS
+// Probe build only (tools/gemm_mc_probe.py compiles this file with -DSQ_GEMM_STAMPS): the library never defines it.
+__device__ __forceinline__ unsigned long long globaltimer() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
+  return t;
+}
+#define SQ_STAMP(slot, value) \
+  do { if (g.stamps) g.stamps[(blockIdx.y * gridDim.x + blockIdx.x) * 5 + (slot)] = (value); } while (0)
+#else
+#define SQ_STAMP(slot, value) do { } while (0)
+#endif
 
 constexpr int G_BK = 64;
 constexpr int G_THREADS = 384;       // warpgroup 0: TMA (one lane), warpgroups 1, 2: wgmma + epilogue for rows 0-63 / 64-127
 constexpr int G_CONSUMER_WARPS = 8;  // arrivals per CTA on an empty-slot barrier
 
-template <int BN, int STAGES, int SPLIT>
+// RING_RED: the split-K reduction slots reuse the ring (free once the k-loop is over) instead of their own region, which
+// leaves room for a deeper ring at split > 1 (gemm_tn_deep_kernel)
+template <int BN, int STAGES, int SPLIT, bool RING_RED = false>
 struct GemmSmem {
   static constexpr int A_BYTES = 128 * 128;            // 128 rows x 64 halfs
   static constexpr int W_BYTES = BN * 128;
   static constexpr int STAGE_BYTES = A_BYTES + ((W_BYTES + 1023) / 1024) * 1024;   // stages stay 1024 B aligned (SW128)
   static constexpr int OFF_BAR = STAGES * STAGE_BYTES; // full[STAGES], empty[STAGES]
-  static constexpr int OFF_RED = OFF_BAR + 256;        // split-K: SPLIT slots x (128/SPLIT rows) x (BN+4) floats
+  static constexpr int OFF_RED = RING_RED ? 0 : OFF_BAR + 256;   // split-K: SPLIT slots x (128/SPLIT rows) x (BN+4) floats
   static constexpr int R_STRIDE = BN + 4;
   static constexpr int RED_BYTES = SPLIT > 1 ? 128 * R_STRIDE * 4 : 0;
-  static constexpr int TOTAL = OFF_RED + RED_BYTES;
+  static constexpr int TOTAL = RING_RED ? OFF_BAR + 256 : OFF_RED + RED_BYTES;
+  static_assert(!RING_RED || RED_BYTES <= OFF_BAR, "reduction slots must fit in the ring");
 };
+
+// barrier.cluster without .aligned: the producer warpgroup reaches it divergently (lane 0 after its loop)
+__device__ __forceinline__ void cluster_arrive_wait() {
+  asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+}
+
+// Weight tiles are read once per forward: load them with an L2 evict-first policy so that the 405 MB a 7B layer streams
+// through the 50 MB L2 does not push out the activation slab every CTA re-reads (evict-last).
+__device__ __forceinline__ uint64_t l2_policy_evict_first() {
+  uint64_t p;
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+  return p;
+}
+__device__ __forceinline__ uint64_t l2_policy_evict_last() {
+  uint64_t p;
+  asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
+  return p;
+}
+__device__ __forceinline__ void tma_load_2d_hint(uint32_t dst, const CUtensorMap* tm, uint32_t bar, int c0, int c1, uint64_t policy) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, %4}], [%2], %5;" ::"r"(dst),
+      "l"(tm), "r"(bar), "r"(c0), "r"(c1), "l"(policy)
+      : "memory");
+}
 
 __device__ __forceinline__ void tma_load_2d_mc(uint32_t dst, const CUtensorMap* tm, uint32_t bar, int c0, int c1, uint16_t mask) {
   asm volatile(
@@ -56,12 +105,14 @@ __device__ __forceinline__ void tma_load_2d_mc(uint32_t dst, const CUtensorMap* 
 }
 
 // MC = CTAs (along N) that share one activation K-slab: each loads 128/MC of its rows and multicasts them to all.
-template <int BN, int STAGES, int SPLIT, int MC>
-__global__ void __launch_bounds__(G_THREADS, 1)
-    gemm_tn_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_w, GemmArgs g) {
+// RING_RED (split > 1, MC == 1): the partial rows land in the owners' rings, after a cluster barrier that every CTA passes
+// once its k-loop has read its last slot.
+template <int BN, int STAGES, int SPLIT, int MC, bool RING_RED>
+__device__ __forceinline__ void gemm_tn_body(const CUtensorMap& tm_a, const CUtensorMap& tm_w, GemmArgs g) {
   // cluster (MC, SPLIT): rank = mcr + MC * ks.  CTAs with the same ks share the activation slab (multicast group); CTAs
   // with the same mcr hold the K-splits of one output tile (DSMEM reduction group).
-  using SM = GemmSmem<BN, STAGES, SPLIT>;
+  static_assert(!RING_RED || (SPLIT > 1 && MC == 1), "ring reduction: split-K without multicast");
+  using SM = GemmSmem<BN, STAGES, SPLIT, RING_RED>;
   constexpr int NCH = BN / 64;                             // 64-column accumulator chunks (one wgmma m64n64k16 each)
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -90,14 +141,21 @@ __global__ void __launch_bounds__(G_THREADS, 1)
     // ===== TMA producer =====
     if (tid == 0) {
       asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+#ifdef SQ_GEMM_STAMPS
+      uint32_t smid;
+      asm volatile("mov.u32 %0, %smid;" : "=r"(smid));
+      SQ_STAMP(0, smid);
+      SQ_STAMP(1, globaltimer());
+#endif
       // Weights do not depend on the previous kernel: under programmatic dependent launch the first ring of weight
       // tiles streams in while that kernel is still running; only the activation loads wait for it.
+      const uint64_t pol_w = l2_policy_evict_first(), pol_a = l2_policy_evict_last();
       const int pre = nkb < STAGES ? nkb : STAGES;
       for (int kb = 0; kb < pre; ++kb) {
         const uint32_t sa = s_base + kb * SM::STAGE_BYTES, sw = sa + SM::A_BYTES;
         ptx::mbar_expect_tx(bar_full + 8 * kb, SM::A_BYTES + SM::W_BYTES);
-        if (g.tiled) ptx::tma_load_2d(sw, &tm_w, bar_full + 8 * kb, 0, ((int)blockIdx.x * g.kb_total + kb0 + kb) * BN);
-        else ptx::tma_load_2d(sw, &tm_w, bar_full + 8 * kb, (kb0 + kb) * G_BK, n0);
+        if (g.tiled) tma_load_2d_hint(sw, &tm_w, bar_full + 8 * kb, 0, ((int)blockIdx.x * g.kb_total + kb0 + kb) * BN, pol_w);
+        else tma_load_2d_hint(sw, &tm_w, bar_full + 8 * kb, (kb0 + kb) * G_BK, n0, pol_w);
       }
       asm volatile("griddepcontrol.wait;" ::: "memory");
       int stage = 0;
@@ -107,15 +165,16 @@ __global__ void __launch_bounds__(G_THREADS, 1)
         if (kb >= pre) {
           ptx::mbar_wait_one(bar_empty + 8 * stage, phase ^ 1, g.err_flag, 11);   // slot free in EVERY CTA of the cluster
           ptx::mbar_expect_tx(bar_full + 8 * stage, SM::A_BYTES + SM::W_BYTES);
-          if (g.tiled) ptx::tma_load_2d(sw, &tm_w, bar_full + 8 * stage, 0, ((int)blockIdx.x * g.kb_total + kb0 + kb) * BN);
-          else ptx::tma_load_2d(sw, &tm_w, bar_full + 8 * stage, (kb0 + kb) * G_BK, n0);
+          if (g.tiled) tma_load_2d_hint(sw, &tm_w, bar_full + 8 * stage, 0, ((int)blockIdx.x * g.kb_total + kb0 + kb) * BN, pol_w);
+          else tma_load_2d_hint(sw, &tm_w, bar_full + 8 * stage, (kb0 + kb) * G_BK, n0, pol_w);
         }
-        if (MC == 1) ptx::tma_load_2d(sa, &tm_a, bar_full + 8 * stage, (kb0 + kb) * G_BK, g.m0);
+        if (MC == 1) tma_load_2d_hint(sa, &tm_a, bar_full + 8 * stage, (kb0 + kb) * G_BK, g.m0, pol_a);
         else tma_load_2d_mc(sa + mcr * (SM::A_BYTES / MC), &tm_a, bar_full + 8 * stage, (kb0 + kb) * G_BK, g.m0 + mcr * (128 / MC),
                             (uint16_t)(((1u << MC) - 1u) << (MC * ks)));
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
     }
+    if constexpr (RING_RED) cluster_arrive_wait();   // (the consumers' barrier before their pushes: see below)
   } else {
     // ===== consumers: warpgroup wg owns tile rows [64 wg, 64 wg + 64), all BN columns, accumulators in registers =====
     const int wg = (warp >> 2) - 1;
@@ -136,6 +195,10 @@ __global__ void __launch_bounds__(G_THREADS, 1)
     uint32_t phase = 0;
     for (int kb = 0; kb < nkb; ++kb) {
       ptx::mbar_wait(bar_full + 8 * stage, phase, g.err_flag, 12);               // TMA bytes have landed
+#ifdef SQ_GEMM_STAMPS
+      if (tid == 128 && kb == 0) SQ_STAMP(2, globaltimer());
+      if (tid == 128 && kb == nkb - 1) SQ_STAMP(3, globaltimer());
+#endif
       const uint32_t sa = s_base + stage * SM::STAGE_BYTES + wg * 8192, sw = s_base + stage * SM::STAGE_BYTES + SM::A_BYTES;
       ptx::wgmma_fence();
 #pragma unroll
@@ -152,6 +215,9 @@ __global__ void __launch_bounds__(G_THREADS, 1)
     }
     ptx::wgmma_wait_all();
     if (prev >= 0) release(prev);
+    // every CTA of the cluster has read its last ring slot (and no TMA write is pending: each was waited for) before any
+    // partial row is pushed into a ring
+    if constexpr (RING_RED) cluster_arrive_wait();
     // accumulator fragment: acc[c][4j + 2h + e] = tile row rbase + 8h, column 64c + 8j + 2q + e
     const int rbase = wg * 64 + (warp & 3) * 16 + (lane >> 2), q2 = 2 * (lane & 3);
     if (SPLIT == 1 && g.epi == 1) {
@@ -242,6 +308,24 @@ __global__ void __launch_bounds__(G_THREADS, 1)
       *reinterpret_cast<uint2*>(g.c + (int64_t)(g.m0 + row) * g.ldc + n0 + cc * 4) = pk;
     }
   }
+#ifdef SQ_GEMM_STAMPS
+  __syncthreads();
+  if (tid == 0) SQ_STAMP(4, globaltimer());
+#endif
+}
+
+template <int BN, int STAGES, int SPLIT, int MC>
+__global__ void __launch_bounds__(G_THREADS, 1)
+    gemm_tn_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_w, GemmArgs g) {
+  gemm_tn_body<BN, STAGES, SPLIT, MC, false>(tm_a, tm_w, g);
+}
+
+// Split-K with the ring of the split-1 instances (8 stages at BN 64, 6 at BN 128): at split 2 the 4-stage ring of
+// gemm_tn_kernel keeps too few bytes in flight per SM to stream the narrow o_proj / down_proj shapes at HBM rate.
+template <int BN, int STAGES, int SPLIT>
+__global__ void __launch_bounds__(G_THREADS, 1)
+    gemm_tn_deep_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_w, GemmArgs g) {
+  gemm_tn_body<BN, STAGES, SPLIT, 1, true>(tm_a, tm_w, g);
 }
 
 }  // namespace sq
@@ -275,7 +359,9 @@ static int encode_2d(CUtensorMap* tm, const void* base, uint64_t inner, uint64_t
 
 // Tile selection: put a CTA on (nearly) every SM with the widest N tile that allows -- per-SM ingest, not HBM, is what
 // limits a 128-row weight stream, and the activation tile every CTA re-reads is pure overhead: a wider BN and a 2-CTA
-// multicast of the activation slab both raise the weight share of each SM's ingest.
+// multicast of the activation slab both raise the weight share of each SM's ingest.  Clusters of more than 2 CTAs are not
+// picked: the H100 holds 30 clusters of 4 at this kernel's shared memory (cudaOccupancyMaxActiveClusters), so the 32 of
+// an N = 4096 split-4 grid ran in two waves (DESIGN §4).
 static int sm_count() {
   static int n_sm = 0;
   if (!n_sm) {
@@ -297,13 +383,13 @@ static void choose_tiles(sq_gemm_plan* p, bool allow_split) {
   double best_score = -1.0;
   for (int bn : cands) {
     const int tiles = (N + bn - 1) / bn;
-    for (int split : {1, 2, 4}) {
+    for (int split : {1, 2}) {
       if (kb % split || (split > 1 && !allow_split)) continue;
-      if (split > 1 && (bn > 128 || N % bn)) continue;       // DSMEM reduction buffers: BN <= 128, no ragged tile
+      if (split > 1 && (bn > 128 || N % bn)) continue;       // split-K instances: BN <= 128, no ragged tile
       const int ctas = tiles * split;
       if (ctas > n_sm) continue;
       for (int mc : {1, 2}) {
-        if (mc == 2 && tiles % 2) continue;
+        if (mc == 2 && (tiles % 2 || split > 1)) continue;   // a cluster of at most 2 CTAs
         // modelled weight bandwidth ~ CTAs x weight share of the per-SM ingest; split-K pays a reduction tail
         const double a_share = 128.0 / mc, share = bn / (bn + a_share);
         double score = ctas * share;
@@ -313,22 +399,24 @@ static void choose_tiles(sq_gemm_plan* p, bool allow_split) {
     }
   }
   p->bn = best_bn; p->split = best_split; p->mc = best_mc;
+  p->deep = best_split > 1;                             // split-K on the deep ring (gemm_tn_deep_kernel)
 }
 
 static void pick_tiles(sq_gemm_plan* p) {
   const int kb = p->K / 64;
   const bool allow_split = p->epi == 0;                 // a fused epilogue needs the whole K sum in one CTA
   choose_tiles(p, allow_split);
-  // tuning / tests: "bn,split,mc" (an illegal triple is ignored: check sq_gemm_plan_info).  The attention kernel's
-  // counterpart is SQ_ATTN_SPLITS (sq_attn.cu).
+  // tuning / tests: "bn,split,mc" names an instance of run_tile's table; "bn,2,1,1" the deep-ring split-K kernel (an
+  // illegal tile is ignored: check sq_gemm_plan_info).  The attention kernel's counterpart is SQ_ATTN_SPLITS (sq_attn.cu).
   const char* force = getenv("SQ_GEMM_FORCE");
   if (force) {
-    int fb = 0, fs = 0, fm = 1;
-    const int nf = sscanf(force, "%d,%d,%d", &fb, &fs, &fm);
+    int fb = 0, fs = 0, fm = 1, fd = 0;
+    const int nf = sscanf(force, "%d,%d,%d,%d", &fb, &fs, &fm, &fd);
     const bool bn_ok = fb == 64 || fb == 128 || fb == 192 || fb == 256;
     if (nf >= 2 && bn_ok && (fs == 1 || fs == 2 || fs == 4) && kb % fs == 0 && (fm == 1 || fm == 2) &&
         !(fs > 1 && (fb > 128 || p->N % fb || !allow_split)) && !(fm == 2 && ((p->N + fb - 1) / fb) % 2)) {
       p->bn = fb; p->split = fs; p->mc = fm;
+      p->deep = nf == 4 && fd == 1 && fs == 2 && fm == 1;
     }
   }
 }
@@ -381,7 +469,7 @@ static int plan_create(sq_gemm_plan** plan, const sq_half* a, int lda, int n_max
   {
     p->pdl = pdl_enabled() ? 1 : 0;
   }
-  p->stages = p->split > 1 ? 4 : (p->bn == 256 ? 4 : p->bn == 192 ? 5 : p->bn == 128 ? 6 : 8);   // == the dispatch table below
+  p->stages = p->split > 1 && !p->deep ? 4 : (p->bn == 256 ? 4 : p->bn == 192 ? 5 : p->bn == 128 ? 6 : 8);   // == run_tile / run_deep_tile
   int rc = encode_2d(&p->tm_a, a, (uint64_t)K, (uint64_t)n_max, (uint64_t)lda * 2, 64, (uint32_t)(128 / p->mc),
                      CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
   if (!rc) {
@@ -399,14 +487,18 @@ extern "C" int sq_gemm_plan_destroy(sq_gemm_plan* plan) {
   return SQ_OK;
 }
 
-template <int BN, int STAGES, int SPLIT, int MC>
+template <int BN, int STAGES, int SPLIT, int MC, bool DEEP = false>
 static int launch_gemm(sq_gemm_plan* p, GemmArgs& g, cudaStream_t st) {
-  using SM = GemmSmem<BN, STAGES, SPLIT>;
+  using SM = GemmSmem<BN, STAGES, SPLIT, DEEP>;
   constexpr int smem = SM::TOTAL + 1024;
   static_assert(smem <= 227 * 1024, "shared memory budget");
+  static_assert(!DEEP || MC == 1, "gemm_tn_deep_kernel has no multicast");
+  void (*kernel)(CUtensorMap, CUtensorMap, GemmArgs);
+  if constexpr (DEEP) kernel = gemm_tn_deep_kernel<BN, STAGES, SPLIT>;
+  else kernel = gemm_tn_kernel<BN, STAGES, SPLIT, MC>;
   static bool attr = false;
   if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_tn_kernel<BN, STAGES, SPLIT, MC>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) { set_error("sq_gemm: smem attr: %s", cudaGetErrorString(e)); return SQ_ERR_CUDA; }
     attr = true;
   }
@@ -427,7 +519,17 @@ static int launch_gemm(sq_gemm_plan* p, GemmArgs& g, cudaStream_t st) {
     at[1].val.programmaticStreamSerializationAllowed = 1;
     cfg.numAttrs = 2;
   }
-  cudaError_t e = cudaLaunchKernelEx(&cfg, gemm_tn_kernel<BN, STAGES, SPLIT, MC>, p->tm_a, p->tm_w, g);
+#ifdef SQ_GEMM_STAMPS
+  if (p->max_clusters < 0) {   // probe build: how many (MC, SPLIT) clusters of this instance the device holds at once
+    cfg.numAttrs = 1;
+    if (cudaOccupancyMaxActiveClusters(&p->max_clusters, kernel, &cfg) != cudaSuccess) {
+      cudaGetLastError();
+      p->max_clusters = -2;
+    }
+    return SQ_OK;
+  }
+#endif
+  cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, p->tm_a, p->tm_w, g);
   if (e != cudaSuccess) { set_error("sq_gemm: launch failed: %s", cudaGetErrorString(e)); return SQ_ERR_CUDA; }
   SQ_CHECK_LAUNCH("sq_gemm");
   return SQ_OK;
@@ -442,6 +544,14 @@ static int run_tile(sq_gemm_plan* plan, GemmArgs& g, cudaStream_t st) {
   SQ_G(64, 8, 1, 1); SQ_G(64, 8, 1, 2); SQ_G(64, 4, 2, 1); SQ_G(64, 4, 4, 1); SQ_G(64, 4, 2, 2); SQ_G(64, 4, 4, 2);
 #undef SQ_G
   set_error("sq_gemm_run: no kernel for bn=%d split=%d mc=%d", bn, sp, mc);
+  return SQ_ERR_UNSUPPORTED;
+}
+
+// Split-K tiles on the deep ring (picked by choose_tiles only; SQ_GEMM_FORCE always names a run_tile instance)
+static int run_deep_tile(sq_gemm_plan* plan, GemmArgs& g, cudaStream_t st) {
+  if (plan->bn == 64 && plan->split == 2) return launch_gemm<64, 8, 2, 1, true>(plan, g, st);
+  if (plan->bn == 128 && plan->split == 2) return launch_gemm<128, 6, 2, 1, true>(plan, g, st);
+  set_error("sq_gemm_run: no deep-ring kernel for bn=%d split=%d", plan->bn, plan->split);
   return SQ_ERR_UNSUPPORTED;
 }
 
@@ -464,7 +574,10 @@ extern "C" int sq_gemm_run_at(sq_gemm_plan* plan, int n, int a_row0, sq_half* c,
     if (c) { g.ldc = ldc; g.c = (__half*)c - (int64_t)a_row0 * ldc; }
     else { g.ldc = plan->ldc; g.c = plan->c; }
     g.err_flag = plan->err_flag;
-    const int rc = run_tile(plan, g, (cudaStream_t)stream);
+#ifdef SQ_GEMM_STAMPS
+    g.stamps = plan->stamps;
+#endif
+    const int rc = plan->deep ? run_deep_tile(plan, g, (cudaStream_t)stream) : run_tile(plan, g, (cudaStream_t)stream);
     if (rc != SQ_OK) return rc;
   }
   return SQ_OK;
@@ -484,3 +597,20 @@ extern "C" int sq_gemm_plan_info(sq_gemm_plan* plan, int* bn, int* split, int* s
   *bn = plan->bn; *split = plan->split; *stages = plan->stages + 100 * plan->mc;
   return SQ_OK;
 }
+
+#ifdef SQ_GEMM_STAMPS
+/* Probe build only.  Stamps: NULL or 5 u64 per CTA (see GemmArgs::stamps) for the plan's following runs. */
+extern "C" int sq_gemm_probe_set_stamps(sq_gemm_plan* plan, unsigned long long* stamps) {
+  plan->stamps = stamps;
+  return SQ_OK;
+}
+/* cudaOccupancyMaxActiveClusters for the plan's instance at its grid, cluster shape and shared-memory size (no launch). */
+extern "C" int sq_gemm_probe_max_clusters(sq_gemm_plan* plan, int* max_clusters) {
+  plan->max_clusters = -1;
+  GemmArgs g{};
+  const int rc = run_tile(plan, g, nullptr);
+  *max_clusters = plan->max_clusters;
+  plan->max_clusters = 0;
+  return rc;
+}
+#endif

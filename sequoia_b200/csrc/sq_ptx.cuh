@@ -62,11 +62,13 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* tm,
       "l"(tm), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
-// mbarrier arrive on the barrier at the same shared-memory offset in CTA `cta` of the cluster (may be this CTA)
+// mbarrier arrive on the barrier at the same shared-memory offset in CTA `cta` of the cluster (may be this CTA).  Default
+// (release, CTA scope) semantics, as the arrive on a local barrier: it hands back a ring slot whose reads (wgmma) have
+// completed.  A .release.cluster arrive made every k-block of sq_gemm's 2-CTA multicast 3-4x slower on the H100.
 __device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t cta) {
   asm volatile(
       "{\n\t.reg .b32 ra;\n\tmapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}" ::"r"(bar), "r"(cta)
+      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}" ::"r"(bar), "r"(cta)
       : "memory");
 }
 // warpgroup MMA (wgmma): every call is issued by all 128 threads of a warpgroup

@@ -25,6 +25,11 @@ import torch
 from . import ops
 
 F16 = torch.float16
+# Layer projections besides the fused gate_up that run on an sq_gemm plan in forwards of 97-128 rows (LlamaRunner), and
+# the (BN, split) the library must pick for them: the route is taken only at the tile that was measured to make a whole
+# 7B layer faster (DESIGN §4).  down_proj's split-K over 64-wide tiles on the deep ring beats cuBLASLt; q/k/v and o_proj
+# on their best tiles made the layer slower or no faster, so they stay on cuBLASLt.
+VERIFY_PLANS = {"wd": (64, 2)}
 
 
 @dataclass
@@ -303,7 +308,7 @@ class LlamaRunner:
         self.v_cache = torch.zeros_like(self.k_cache)
         self.plan = ops.AttnPlan(self.qkv, n, self.H, self.Hkv, D, self.k_cache, self.v_cache, self.attn_out)
         # Dense GEMMs.  For models whose layers are HBM-stream-sized (hidden >= 2048) the target's lm_head (<= 128 rows) and
-        # the gate_up of 97-128-row forwards (below) run on the hand-written wgmma kernel (csrc/sq_gemm.cu); every other
+        # the gate_up and down_proj of 97-128-row forwards (below) run on the hand-written wgmma kernel (csrc/sq_gemm.cu); every other
         # projection and row count runs on cuBLASLt (torch.mm), which is faster there.
         self.gemm_err = torch.zeros(4, dtype=torch.int32, device=dev)
         self.lm_plan = None
@@ -319,13 +324,14 @@ class LlamaRunner:
             torch.cuda.empty_cache()
         stream_sized = h >= 2048
         # Layer projections of the 97-128-row verify (config 2's 128-node tree) on sq_gemm: the ones it streams faster than
-        # cuBLASLt on an H100 (DESIGN §4 table).  Only gate_up wins there, with the SwiGLU epilogue fused (one launch, no
-        # gate_up round trip, no silu_mul).  q/k/v, o_proj and down_proj stay on cuBLASLt, and so does every other row
-        # count: prefill, the first verify and the 768-row verify of config 4 are compute-bound, not a weight stream, and
+        # cuBLASLt on an H100 (DESIGN §4 table): gate_up, with the SwiGLU epilogue fused (one launch, no gate_up round
+        # trip, no silu_mul), and down_proj (VERIFY_PLANS, below).  q/k/v and o_proj stay on cuBLASLt, and so does every
+        # other row count: prefill, the first verify and the 768-row verify of config 4 are compute-bound, not a weight stream, and
         # config 3's 65-row tree is better served by cuBLASLt's 64-row tiles than by the plan's 128-row activation tile.
         # Those go to cuBLASLt on the SAME weight tensor, which is why gate_up is kept row-major in the interleaved order
         # (16 gate rows | 16 up rows) rather than pre-tiled.  Tensor-parallel shards keep cuBLASLt + sq_silu_mul, and so
-        # does a tile with the 2-CTA activation multicast (the 13B gate_up): every multicast tile measured 2-4x slower.
+        # does a tile with the 2-CTA activation multicast (the 13B gate_up's (256, 1, 2)): no longer slow, but a 13B layer
+        # has not been timed on it.
         ok = stream_sized and tp == 1 and weight_format == "fp16" and self.I % 16 == 0 and h % 64 == 0
         self.gu_interleaved = False
         if ok and ops.gemm_pick_tiles(2 * self.I, h, ops.GEMM_SWIGLU)[2] == 1:
@@ -333,6 +339,16 @@ class LlamaRunner:
             for ly in self.layers:
                 ly["wgu"] = ops.interleave_gate_up(ly["wgu"][:self.I], ly["wgu"][self.I:])
                 ly["wgu_plan"] = ops.GemmPlan(self.normed, ly["wgu"], self.act, self.gemm_err, swiglu=True)
+        # The projections of VERIFY_PLANS in the same forwards, where the library picks the measured tile for their shape.
+        # A plan also chains to its neighbours by programmatic dependent launch: its first ring of weight tiles streams in
+        # while the preceding kernel finishes, where cuBLASLt starts its weight stream only once that kernel has ended.
+        if ok:
+            io = dict(wqkv=(self.normed, self.qkv), wo=(self.attn_out, self.proj), wd=(self.act, self.proj))
+            for k, tile in VERIFY_PLANS.items():
+                if ops.gemm_pick_tiles(*self.layers[0][k].shape)[:2] != tile:
+                    continue
+                for ly in self.layers:
+                    ly[k + "_plan"] = ops.GemmPlan(io[k][0], ly[k], io[k][1], self.gemm_err)
         if stream_sized and V % 32 == 0 and h % 64 == 0:
             self.lm_plan = ops.GemmPlan(self.normed, self.lm_head, self.logits, self.gemm_err)
         # Small draft models (csrc/sq_draft.cu): a dedicated attention kernel replaces sq_tree_attn for the draft's
@@ -358,8 +374,11 @@ class LlamaRunner:
         ops.silu_mul(self.gate_up, self.act, n, interleaved=self.gu_interleaved)
 
     def _project(self, ly, k: str, a: torch.Tensor, n: int, out: torch.Tensor):
-        """out[:n] = a[:n] @ W_k.T: torch.mm on an fp16 weight, the FP8 plan (bound to a / out) on a quantized one"""
+        """out[:n] = a[:n] @ W_k.T: torch.mm on an fp16 weight, the FP8 plan (bound to a / out) on a quantized one, the
+        fp16 sq_gemm plan (bound likewise) for the 97-128 rows of a verify"""
         plan = ly.get(k + "_fp8")
+        if plan is None and 96 < n <= 128:
+            plan = ly.get(k + "_plan")
         if plan is not None:
             plan.run(n)
         else:

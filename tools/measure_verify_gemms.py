@@ -8,8 +8,10 @@ Every timing is a CUDA graph that cycles over COPIES weight copies (>= 6, 2+ GB 
 not from the 50 MB L2.  It reports us per call, weight GB/s and that rate's share of the H100 SXM data-sheet 3.35 TB/s.
 
 --layer also times one 7B-shaped decoder layer as the model runs it (rmsnorm, qkv, RoPE + KV append, attention, o_proj,
-add_rmsnorm, gate_up (+ silu_mul), down_proj, add_rmsnorm) on a 4-layer LlamaRunner, once with every projection on
-cuBLASLt and once on the runner's own routes: programmatic dependent launch only shows up in such a chain.
+add_rmsnorm, gate_up (+ silu_mul), down_proj, add_rmsnorm) on a 4-layer LlamaRunner, on each route of --routes:
+programmatic dependent launch only shows up in such a chain.  A route is "model" (the runner's own routes), "cublas"
+(every projection on torch.mm + sq_silu_mul), or "+"-joined projections on sq_gemm plans, each with the tile the library
+picks or a forced one: "gu+qkv+o=64:2:1+down=128:4:1" (gu = the fused gate_up plan; the others stay on cuBLASLt).
 
 Prints the card and its power limit first; --json writes every number.  Needs a GPU."""
 import argparse
@@ -30,6 +32,7 @@ SHAPES = {                       # projection: (N, K, SwiGLU epilogue) of Llama-
     "gate_up": (22016, 4096, True),
     "down_proj": (4096, 11008, False),
     "lm_head": (32000, 4096, False),
+    "gate_up_13b": (27648, 5120, True),              # Llama-2-13B (not in the default set: --only gate_up_13b)
 }
 
 
@@ -86,6 +89,8 @@ def tile_candidates(N, K, swiglu):
         for split in (1, 2, 4):
             if kb % split or (split > 1 and (swiglu or bn > 128 or N % bn)):
                 continue
+            if split == 2:
+                out.append((bn, 2, 1, 1))                    # split-K on the deep ring (gemm_tn_deep_kernel)
             for mc in (1, 2, 4):
                 tiles = -(-N // bn)
                 if tiles % mc:
@@ -99,7 +104,7 @@ def measure_shapes(ns, copies, reps, sweep, only):
     err = torch.zeros(4, dtype=torch.int32, device=dev)
     rows = []
     for name, (N, K, swiglu) in SHAPES.items():
-        if only and name not in only:
+        if (only and name not in only) or (not only and name.endswith("_13b")):
             continue
         gen = torch.Generator(device=dev).manual_seed(0)
         a = (torch.randn(128, K, device=dev, generator=gen) * 0.5).half()
@@ -122,12 +127,12 @@ def measure_shapes(ns, copies, reps, sweep, only):
 
         variants = [("default", None)]
         if sweep:
-            variants += [(f"{bn},{sp},{mc}", f"{bn},{sp},{mc}") for bn, sp, mc in tile_candidates(N, K, swiglu)]
+            variants += [(",".join(map(str, t)), ",".join(map(str, t))) for t in tile_candidates(N, K, swiglu)]
         plans = {}
         for label, force in variants:
             ps = [make_plan(a, w, act if swiglu else c, err, swiglu, force) for w in wi]
             info = ps[0].info()
-            if force and (info[0], info[1], info[2] // 100) != tuple(int(x) for x in force.split(",")):
+            if force and (info[0], info[1], info[2] // 100) != tuple(int(x) for x in force.split(",")[:3]):
                 continue                                         # the library rejected the forced tile
             plans[label] = ps
         for n in ns:
@@ -166,7 +171,8 @@ def measure_shapes(ns, copies, reps, sweep, only):
 
 
 def measure_layer(ns, reps, routes):
-    """One 7B-shaped decoder layer per call (a 4-layer runner, so each layer's 405 MB of weights comes from HBM)."""
+    """One 7B-shaped decoder layer per call (a 4-layer runner, so each layer's 405 MB of weights comes from HBM).  Also
+    compares each route's logits (4 layers + lm_head, same inputs and cache) with the first route's."""
     from sequoia_b200 import model
     cfg = model.NAMED_CONFIGS["llama-2-7b"]
     model.NAMED_CONFIGS["llama-2-7b-4l"] = model.LlamaConfigLite(cfg.hidden_size, cfg.intermediate_size, 4,
@@ -179,29 +185,52 @@ def measure_layer(ns, reps, routes):
     ids = torch.randint(0, 32000, (M,), device=dev)
     pos = torch.arange(M, device=dev)
     mask = torch.zeros(128, M, dtype=torch.float16, device=dev)
-    out = []
+    out, first = [], {}
     for route in routes:
         restore = route_set(r, route)
         for n in ns:
             sto = torch.arange(P, P + n, device=dev)
             fn = lambda i: r.forward(n, ids, pos[P:P + n], sto, kv_end=P + n, dense_mask=mask, mask_ld=M, skip_lm_head=True)
             t = graph_time_us(fn, 1, reps) / r.L
-            out.append({"route": route, "n": n, "us_per_layer": round(t, 2)})
-            print(f"layer  route {route:8s} n={n:3d}  {t:8.2f} us per 7B layer", flush=True)
+            logits = r.forward(n, ids, pos[P:P + n], sto, kv_end=P + n, dense_mask=mask, mask_ld=M).double()
+            ref = first.setdefault(n, logits.clone())
+            d = ((logits - ref).abs().max() / ref.abs().max()).item()
+            out.append({"route": route, "n": n, "us_per_layer": round(t, 2), "logit_rel_diff_vs_first_route": d})
+            print(f"layer  route {route:40s} n={n:3d}  {t:8.2f} us per 7B layer   logits vs route {routes[0]}: "
+                  f"max |diff| / max |logit| = {d:.2e}", flush=True)
         restore()
     if any(r.gemm_err.tolist()):
         raise RuntimeError(f"sq_gemm watchdog flag set: {r.gemm_err.tolist()}")
     return out
 
 
+ROUTE_KEYS = {"gu": "wgu", "qkv": "wqkv", "o": "wo", "down": "wd"}
+
+
 def route_set(r, route):
-    """'model': the runner's own routes; 'cublas': every layer projection on torch.mm (+ sq_silu_mul)."""
+    """Install `route` (see the module docstring) on runner r; returns the function that puts the runner's own back."""
+    from sequoia_b200 import ops
     if route == "model":
         return lambda: None
     saved = [{k: ly.pop(k) for k in list(ly) if k.endswith("_plan")} for ly in r.layers]
+    io = dict(wqkv=(r.normed, r.qkv), wo=(r.attn_out, r.proj), wd=(r.act, r.proj))
+    for part in ([] if route == "cublas" else route.split("+")):
+        name, _, tile = part.partition("=")
+        k = ROUTE_KEYS[name]
+        for ly, s in zip(r.layers, saved):
+            if k == "wgu":
+                if "wgu_plan" not in s:
+                    raise ValueError("the runner built no fused gate_up plan")
+                ly["wgu_plan"] = s["wgu_plan"]
+            else:
+                ly[k + "_plan"] = make_plan(io[k][0], ly[k], io[k][1], r.gemm_err, False, tile.replace(":", ","))
+                if tile and ly[k + "_plan"].info()[:2] != tuple(int(x) for x in tile.split(":")[:2]):
+                    raise ValueError(f"tile {tile} refused for {k}")
 
     def restore():
         for ly, s in zip(r.layers, saved):
+            for k in [k for k in ly if k.endswith("_plan")]:
+                del ly[k]
             ly.update(s)
     return restore
 
@@ -214,6 +243,7 @@ def main():
     ap.add_argument("--only", default="", help="comma-separated projections")
     ap.add_argument("--sweep", action="store_true", help="also time every legal sq_gemm tile")
     ap.add_argument("--layer", action="store_true", help="also time a whole 7B layer on each route")
+    ap.add_argument("--routes", default="cublas,model", help="comma-separated layer routes (see above)")
     ap.add_argument("--json", default=None, help="write the results here")
     args = ap.parse_args()
     if not torch.cuda.is_available():
@@ -224,7 +254,7 @@ def main():
     res = {"card": info, "shapes": measure_shapes(ns, max(args.copies, 6), args.reps, args.sweep,
                                                   [x for x in args.only.split(",") if x])}
     if args.layer:
-        res["layer"] = measure_layer(ns, args.reps, ("cublas", "model"))
+        res["layer"] = measure_layer(ns, args.reps, args.routes.split(","))
     if args.json:
         os.makedirs(os.path.dirname(os.path.abspath(args.json)), exist_ok=True)
         with open(args.json, "w") as f:
