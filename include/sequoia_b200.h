@@ -162,6 +162,14 @@ int sq_residual(const sq_half* p, const sq_half* q, sq_half* out, int V, void* s
  * ascending index.  No-op when top_p >= 1. */
 int sq_top_p_filter(sq_half* logits, int64_t ld, int n, int V, float top_p, float T, void* stream);
 
+/* Top-k filter, in place on n rows: exactly k tokens of each row keep their logit, every other one is set to -inf.
+ * Ranking is on the raw fp16 logit, value descending, equal values by ascending index (a stable descending sort, the tie
+ * rule of sq_top_p_filter; -0 ranks with +0, NaN above +inf), so the kept set does not depend on the temperature.  -inf
+ * entries rank last: a row with fewer than k finite logits loses nothing finite.  k == 0 is off and k >= V filters
+ * nothing (no launch); k < 0 is refused.  To compose with top-p, run this first: sq_top_p_filter then renormalises over
+ * the survivors (a -inf logit has probability 0), the temperature -> top_k -> top_p order of common samplers. */
+int sq_top_k_filter(sq_half* logits, int64_t ld, int n, int V, int k, void* stream);
+
 /* argmax over V per row -> int64 (GreedyTree.py:186). */
 int sq_argmax_rows(const sq_half* logits, int64_t ld, int n, int V, int64_t* out, void* stream);
 
@@ -379,6 +387,11 @@ int sq_accept_stochastic_batch_per_seq(const sq_half* target_logits, int64_t ld_
                                        void* stream);
 int sq_top_p_filter_per_seq(sq_half* logits, int64_t ld, int n, int V, const float* top_p, const float* T,
                             int rows_per_seq, void* stream);
+/* sq_top_k_filter with row r of the n rows at the k of sequence r / rows_per_seq, read from the (B,) int32 device array
+ * top_k (rows_per_seq must divide n); a row whose k <= 0 or k >= V is left untouched.  With an all-equal array it computes
+ * bit for bit what the scalar call computes.  A null array is refused with SQ_ERR_INVALID_ARG. */
+int sq_top_k_filter_per_seq(sq_half* logits, int64_t ld, int n, int V, const int32_t* top_k, int rows_per_seq,
+                            void* stream);
 /* target_token (B*S) int64 */
 int sq_accept_greedy_batch(const int64_t* target_token, const int32_t* succ_off, const int32_t* succ, const int32_t* depth,
                            int S, int64_t* tokens, int64_t* position_ids, int64_t ld_seq, int32_t* accept_idx,

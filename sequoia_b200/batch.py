@@ -3,9 +3,9 @@
 A steady step is the same two graph replays and one host sync as a single-sequence tree (sequoia_b200.tree), for all B
 sequences together: every per-sequence kernel is one launch for the batch, the row-wise kernels and the GEMMs see B*n
 rows.  Sequence b's device data: row b of state (B, 16), tokens / position_ids / storage_ids / r (B, M), rand (B, S, V),
-noise (B, V), accept_idx (B, S), its temperature and top_p (B,); rows b*S .. b*S+S-1 of the target logits (B*S, V); the
-draft logits of node k at row_base[k] + b*row_step[k] (each tree level of all sequences is one block, written by one
-lm_head GEMM).
+noise (B, V), accept_idx (B, S), its temperature and top_p (B,) and top_k (B,) int32; rows b*S .. b*S+S-1 of the target
+logits (B*S, V); the draft logits of node k at row_base[k] + b*row_step[k] (each tree level of all sequences is one
+block, written by one lm_head GEMM).
 
 A sequence that is terminal, or has no room for another tree in max_length, is frozen: its state word SQ_ST_FROZEN is
 set and every batched kernel leaves its tokens, state and KV rows alone.  A frozen slot can take a new prompt with
@@ -14,6 +14,11 @@ admit(); the other sequences keep decoding.
 Each sequence has its own policy, "spec" or "greedy".  While all are equal the tree launches the single-policy kernels;
 once both are present (mixed mode, which then stays on) the sampler and the two walks are the *_mixed forms, which read
 the (B,) int32 device array greedy_dev, and every sequence decodes as it would in a tree of its own policy.
+
+A sampled sequence draws from softmax(top_p(top_k(logits)) / T): the accept walk filters the target rows first to the
+top_k best raw logits (0 = off), then to top_p, and speculative sampling stays exact for the filtered distribution.
+Each filter joins the captured graphs the first time a sampled sequence needs it (one recapture each); after that any
+values run in the same graphs.
 """
 from __future__ import annotations
 
@@ -72,6 +77,23 @@ def check_sampling(temperature: float, top_p: float):
         raise ValueError(f"top_p must be in (0, 1], got {top_p}")
 
 
+def check_top_k(top_k) -> int:
+    """A top_k: an integer >= 0 (0 = off; a value >= the vocabulary size filters nothing)."""
+    if isinstance(top_k, bool) or not isinstance(top_k, numbers.Integral) or top_k < 0:
+        raise ValueError(f"top_k must be an integer >= 0 (0 = off), got {top_k!r}")
+    return int(top_k)
+
+
+def _top_ks(top_k, B: int) -> List[int]:
+    """One top_k for all B sequences, or a sequence of B of them."""
+    if isinstance(top_k, Sequence) and not isinstance(top_k, str):
+        ks = [check_top_k(k) for k in top_k]
+        if len(ks) != B:
+            raise ValueError(f"top_k: {len(ks)} values for {B} sequences")
+        return ks
+    return [check_top_k(top_k)] * B
+
+
 def _per_seq(value, B: int, name: str) -> List[float]:
     """One value (a Python, numpy or 0-d tensor scalar) for all B sequences, or a sequence of B values."""
     if isinstance(value, numbers.Real) or (isinstance(value, torch.Tensor) and value.dim() == 0):
@@ -103,6 +125,9 @@ class BatchTree:
     policy: one of "spec" / "greedy" for all sequences, or one per sequence.
     temperature and top_p: one value for all sequences, or one per sequence; "greedy" sequences ignore both (their
     temperature must still be a valid one).
+    top_k: one integer >= 0 for all sequences, or one per sequence: a sampled sequence keeps the top_k best target logits
+    of each row (raw value descending, equal values by ascending index) before top_p and its softmax; 0, and any value
+    >= the vocabulary size, is off.  "greedy" sequences ignore it.
     seeds: None (r and rand drawn with torch's CPU generator as a lone SpecTree draws them, the bonus noise with torch's
     CUDA generator), or one integer in [0, 2^64) per prompt: each sequence then draws all its random numbers on the
     device from a Philox stream keyed by its seed, so its output does not depend on its slot or its neighbours ("greedy"
@@ -112,9 +137,10 @@ class BatchTree:
                  policy: Union[str, Sequence[str]] = "spec",
                  temperature: Union[float, Sequence[float]] = 0.6, top_p: Union[float, Sequence[float]] = 1.0,
                  max_length: int = 256, max_target_seq: Optional[int] = None,
-                 seeds: Optional[Sequence[int]] = None):
+                 seeds: Optional[Sequence[int]] = None, top_k: Union[int, Sequence[int]] = 0):
         B = len(prompts)
         policies = _policies(policy, B)
+        top_ks = _top_ks(top_k, B)
         temps, top_ps = _per_seq(temperature, B, "temperature"), _per_seq(top_p, B, "top_p")
         for t, p in zip(temps, top_ps):
             check_sampling(t, p)
@@ -136,7 +162,7 @@ class BatchTree:
         # mixed: both policies present (from here on, for the tree's life); greedy: every sequence greedy, never mixed
         self.mixed = len(set(policies)) > 1
         self.greedy = not self.mixed and policies[0] == "greedy"
-        self.temps, self.top_ps = temps, top_ps
+        self.temps, self.top_ps, self.top_ks = temps, top_ps, top_ks
         self.B, self.M = B, max_length
         self.max_target_seq = max_target_seq or max_length
         self.st = st = _Static(grow_map, dev)
@@ -157,6 +183,10 @@ class BatchTree:
                                       dtype=torch.float32, device=dev)
         self.greedy_dev = torch.tensor([pol == "greedy" for pol in policies], dtype=torch.int32, device=dev)
         self.use_top_p = any(pol == "spec" and p < 1.0 for pol, p in zip(policies, top_ps))
+        # the same for top_k (0 for a greedy sequence; k >= V is off and held as V, which fits int32)
+        self.top_k_dev = torch.tensor([0 if pol == "greedy" else min(k, V) for pol, k in zip(policies, top_ks)],
+                                      dtype=torch.int32, device=dev)
+        self.use_top_k = any(pol == "spec" and 0 < k < V for pol, k in zip(policies, top_ks))
         i64 = dict(dtype=torch.int64, device=dev)
         self.tokens = torch.zeros(B, M, **i64)
         self.position_ids = torch.zeros(B, M, **i64)
@@ -237,17 +267,21 @@ class BatchTree:
 
     @torch.inference_mode()
     def admit(self, b: int, prompt: torch.Tensor, temperature: Optional[float] = None, top_p: Optional[float] = None,
-              seed: Optional[int] = None, policy: Optional[str] = None):
+              seed: Optional[int] = None, policy: Optional[str] = None, top_k: Optional[int] = None):
         """Start `prompt` in the frozen slot b (finished, out of room, or stopped with freeze), at its own policy,
-        temperature and top_p (default: the slot's previous values).  The next verify() runs its first verify next to the
-        steady sequences.  The slot draws r and rand as a lone SpecTree on the prompt would, and runs its draft prefill now.
+        temperature, top_p and top_k (default: the slot's previous values).  The next verify() runs its first verify next
+        to the steady sequences.  The slot draws r and rand as a lone SpecTree on the prompt would, and runs its draft
+        prefill now.
         A seeded tree takes the prompt's `seed` (required there, refused otherwise): r and rand are then filled on the
         device from that seed's stream and the slot's noise counter restarts at 0.
         The first admission that puts both policies in the batch starts mixed mode: the draft, steady and post graphs are
         captured once more, on their next use.  A tree built all-greedy allocates r and rand at its first "spec"
-        admission."""
+        admission.  The first "spec" admission with 0 < top_k < V (in a tree that had none) captures the steady and post
+        graphs once more: the top-k filter joins the accept step."""
         if policy is not None:
             check_policy(policy)
+        if top_k is not None:
+            top_k = check_top_k(top_k)
         if not 0 <= b < self.B:
             raise IndexError(f"slot {b} out of range for a batch of {self.B}")
         if not self.frozen[b]:
@@ -265,6 +299,7 @@ class BatchTree:
         if seed is not None:
             seed = check_seed(seed)
         pol = self.policies[b] if policy is None else policy
+        k = self.top_ks[b] if top_k is None else top_k
         # (every other slot holds the tree's one policy until then, so a different one means both are present; at B = 1
         # it is a switch, which the single-policy graphs do not serve either)
         enter_mixed = not self.mixed and pol != ("greedy" if self.greedy else "spec")
@@ -272,12 +307,18 @@ class BatchTree:
         self.T_dev[b] = T
         self.top_p_dev[b] = 1.0 if pol == "greedy" else tp
         self.greedy_dev[b] = 1 if pol == "greedy" else 0
+        self.top_ks[b] = k
+        self.top_k_dev[b] = 0 if pol == "greedy" else min(k, self.V)
         if enter_mixed:
             self.mixed, self.greedy = True, False  # the mixed sampler and walks enter every graph: capture them once more
             for name in ("draft", "steady", "post"):
                 self.graphs.pop(name, None)
         if tp < 1.0 and pol == "spec" and not self.use_top_p:
             self.use_top_p = True                  # the filter enters op_accept: capture steady and post once more
+            for name in ("steady", "post"):
+                self.graphs.pop(name, None)
+        if 0 < k < self.V and pol == "spec" and not self.use_top_k:
+            self.use_top_k = True                  # the same for the top-k filter
             for name in ("steady", "post"):
                 self.graphs.pop(name, None)
         if pol == "spec" and self.r is None:       # the first sampling sequence of a tree built all-greedy
@@ -344,6 +385,8 @@ class BatchTree:
             ops.accept_greedy_batch_mixed(self.target_token, st.succ_off, st.succ, st.depth, self.S, self.greedy_dev,
                                           self.tokens, self.position_ids, self.accept_idx, self.state,
                                           self.max_target_seq)
+        if self.use_top_k:                         # top_k before top_p: top_p renormalises over the k survivors
+            ops.top_k_filter_per_seq_(self.target_logits, self.top_k_dev, self.S)
         if self.use_top_p:
             ops.top_p_filter_per_seq_(self.target_logits, self.top_p_dev, self.T_dev, self.S)
         if self.external_noise is None:

@@ -749,6 +749,178 @@ __global__ void __launch_bounds__(NT) top_p_filter_kernel(__half* __restrict__ l
   }
 }
 
+// ---------------------------------------------------------------------------------------------
+// Top-k filter, in place: exactly k tokens of the row keep their logit and every other one becomes -inf.  The ranking is a
+// stable descending sort of the raw fp16 logits (value descending, equal values by ascending index), so the kept set does
+// not depend on the temperature.  No sort: top_p_filter_kernel's two-level histogram select with token COUNTS in place of
+// probability masses -- level 0 finds the high byte of the k-th key, level 1 its low byte inside that bin.  Counts are
+// integers, so the result does not depend on the order of the atomics.  Keys above the boundary key stay, keys below it are
+// removed, and of the tokens equal to it the first k - (count ranked before it) by index stay.
+// WIDE: as top_p_filter_kernel (cluster-summed histograms; the boundary tie group ranked across slices in rank order).
+// PER_SEQ: `top_k` is the (B,) int32 array and row r belongs to sequence r / rows_per_seq; a row whose k <= 0 or k >= V is
+// left untouched (the whole cluster reads the same k).  Otherwise `top_k` is the scalar k, 0 < k < V.
+template <bool PER_SEQ>
+using SeqInt = typename std::conditional<PER_SEQ, const int32_t*, int>::type;
+
+// ord16 with the order torch.sort gives fp16 values: -0 equal to +0, NaN above +inf
+__device__ __forceinline__ uint32_t topk_key(__half h) {
+  const uint32_t b = __half_as_ushort(h);
+  if ((b & 0x7FFFu) > 0x7C00u) return 0xFFFFu;
+  return b == 0x8000u ? 0x8000u : ord16(h);
+}
+
+template <bool WIDE, bool PER_SEQ = false>
+__global__ void __launch_bounds__(NT) top_k_filter_kernel(__half* __restrict__ logits, int64_t ld, int V,
+                                                           SeqInt<PER_SEQ> top_k, int rows_per_seq) {
+  __shared__ uint32_t whist[NW][256];
+  __shared__ uint32_t hist[256];
+  __shared__ int sel[2];            // boundary bin, count ranked before it
+  __shared__ uint32_t wtot[CH][NW];
+  pdl_wait();
+  Slice sl{};
+  __half* row;
+  if constexpr (WIDE) sl = slice_of(V);
+  int k;
+  if constexpr (PER_SEQ) {
+    k = top_k[(WIDE ? sl.row : (int)blockIdx.x) / rows_per_seq];
+    if (k <= 0 || k >= V) return;
+  } else {
+    k = top_k;
+  }
+  if constexpr (WIDE) {
+    row = logits + sl.row * ld + sl.base;
+    V = sl.V;
+  } else {
+    row = logits + blockIdx.x * ld;
+  }
+  const int nvec = V / 8;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  Pack8 x[CH];
+  load_row(row, V, x);
+  uint32_t before = 0u;             // tokens ranked before the current boundary bin
+  int hi = -1, key_b = -1;
+  for (int level = 0; level < 2; ++level) {
+    for (int i = threadIdx.x; i < NW * 256; i += NT) (&whist[0][0])[i] = 0u;
+    __syncthreads();
+#pragma unroll
+    for (int i = 0; i < CH; ++i)
+      if (i * NT + (int)threadIdx.x < nvec) {
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+          const uint32_t key = topk_key(x[i].h[e]);
+          if (level == 0 || (int)(key >> 8) == hi) atomicAdd(&whist[warp][level == 0 ? (key >> 8) : (key & 255u)], 1u);
+        }
+      }
+    __syncthreads();
+    uint32_t t = 0u;
+    if (threadIdx.x < 256) {
+#pragma unroll 8
+      for (int w = 0; w < NW; ++w) t += whist[w][threadIdx.x];
+    }
+    if constexpr (WIDE) {
+      __shared__ uint32_t ghist[2][MAX_SLICES][256];
+      cg::cluster_group cl = cg::this_cluster();
+      if (threadIdx.x < 256)
+        for (int r = 0; r < sl.n(); ++r) *cl.map_shared_rank(&ghist[level][sl.rank()][threadIdx.x], r) = t;
+      cl.sync();
+      if (threadIdx.x < 256) {
+        t = 0u;
+        for (int r = 0; r < sl.n(); ++r) t += ghist[level][r][threadIdx.x];
+      }
+    }
+    if (threadIdx.x < 256) hist[threadIdx.x] = t;
+    if (threadIdx.x == 0) sel[0] = -1;
+    __syncthreads();
+    if (warp == 0) {
+      // lane l owns bins 255-8l .. 248-8l (descending order of value); exclusive scan over the lanes
+      uint32_t m[8], tot = 0u;
+#pragma unroll
+      for (int b = 0; b < 8; ++b) { m[b] = hist[255 - 8 * lane - b]; tot += m[b]; }
+      uint32_t inc = tot;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const uint32_t s = __shfl_up_sync(0xffffffffu, inc, o);
+        if (lane >= o) inc += s;
+      }
+      uint32_t a = before + inc - tot;
+#pragma unroll
+      for (int b = 0; b < 8; ++b) {
+        if (a < (uint32_t)k && a + m[b] >= (uint32_t)k) { sel[0] = 255 - 8 * lane - b; sel[1] = (int)a; }   // unique
+        a += m[b];
+      }
+    }
+    __syncthreads();
+    const int bb = sel[0];
+    if (bb < 0) return;             // (0 < k < V always finds a bin; block- and cluster-uniform all the same)
+    before = (uint32_t)sel[1];
+    if (level == 0) hi = bb; else key_b = (hi << 8) | bb;
+    __syncthreads();
+  }
+  // ties on the boundary key: the first k - before of them (ascending index) stay
+  int cs[CH], excl[CH];
+#pragma unroll
+  for (int i = 0; i < CH; ++i) {
+    cs[i] = 0;
+    if (i * NT + (int)threadIdx.x < nvec) {
+#pragma unroll
+      for (int e = 0; e < 8; ++e) cs[i] += ((int)topk_key(x[i].h[e]) == key_b) ? 1 : 0;
+    }
+  }
+  int inc[CH];
+#pragma unroll
+  for (int i = 0; i < CH; ++i) {
+    int v = cs[i];
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int s = __shfl_up_sync(0xffffffffu, v, o);
+      if (lane >= o) v += s;
+    }
+    inc[i] = v;
+    if (lane == 31) wtot[i][warp] = (uint32_t)v;
+  }
+  __syncthreads();
+  int total = 0;
+#pragma unroll
+  for (int i = 0; i < CH; ++i) {
+    int v = (int)wtot[i][lane];
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int s = __shfl_up_sync(0xffffffffu, v, o);
+      if (lane >= o) v += s;
+    }
+    const int prev = __shfl_sync(0xffffffffu, v, (warp + 31) & 31);
+    excl[i] = total + (warp ? prev : 0) + inc[i] - cs[i];
+    total += __shfl_sync(0xffffffffu, v, 31);
+  }
+  if constexpr (WIDE) {             // tie members in lower slices rank first
+    __shared__ uint32_t gcnt[MAX_SLICES];
+    cg::cluster_group cl = cg::this_cluster();
+    if ((int)threadIdx.x < sl.n()) *cl.map_shared_rank(&gcnt[sl.rank()], (int)threadIdx.x) = (uint32_t)total;
+    cl.sync();
+    int below = 0;
+    for (int r = 0; r < sl.rank(); ++r) below += (int)gcnt[r];
+#pragma unroll
+    for (int i = 0; i < CH; ++i) excl[i] += below;
+  }
+  const int t_keep = k - (int)before;
+#pragma unroll
+  for (int i = 0; i < CH; ++i) {
+    const int c = i * NT + threadIdx.x;
+    if (c >= nvec) continue;
+    bool any = false;
+    int rank = excl[i];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      const int key = (int)topk_key(x[i].h[e]);
+      const bool rm = (key < key_b) || (key == key_b && rank >= t_keep);
+      if (key == key_b) ++rank;
+      if (rm) x[i].h[e] = __ushort_as_half((unsigned short)0xFC00u);     // -inf
+      any |= rm;
+    }
+    if (any) reinterpret_cast<uint4*>(row)[c] = x[i].u;
+  }
+}
+
 }  // namespace sq
 
 using namespace sq;
@@ -964,5 +1136,36 @@ extern "C" int sq_top_p_filter_per_seq(sq_half* logits, int64_t ld, int n, int V
   }
   top_p_filter_kernel<false, true><<<n, NT, 0, (cudaStream_t)stream>>>((__half*)logits, ld, V, T, top_p, rows_per_seq);
   SQ_CHECK_LAUNCH("sq_top_p_filter_per_seq");
+  return SQ_OK;
+}
+
+extern "C" int sq_top_k_filter(sq_half* logits, int64_t ld, int n, int V, int k, void* stream) {
+  SQ_CHECK_V_WIDE(V);
+  SQ_CHECK_ARG(k >= 0, "sq_top_k_filter: k=%d must be >= 0 (0 = off)", k);
+  if (n == 0 || k == 0 || k >= V) return SQ_OK;                    // off, or every token is among the k best
+  if (V > SLICE) {
+    SQ_CHECK_WIDE_LAUNCH(launch_wide(top_k_filter_kernel<true>, n, 1, V, (cudaStream_t)stream, (__half*)logits, ld, V, k,
+                                     0), "sq_top_k_filter");
+    return SQ_OK;
+  }
+  top_k_filter_kernel<false><<<n, NT, 0, (cudaStream_t)stream>>>((__half*)logits, ld, V, k, 0);
+  SQ_CHECK_LAUNCH("sq_top_k_filter");
+  return SQ_OK;
+}
+
+extern "C" int sq_top_k_filter_per_seq(sq_half* logits, int64_t ld, int n, int V, const int32_t* top_k, int rows_per_seq,
+                                       void* stream) {
+  SQ_CHECK_V_WIDE(V);
+  SQ_CHECK_ARG(top_k != nullptr, "sq_top_k_filter_per_seq: null top_k array");
+  SQ_CHECK_ARG(rows_per_seq >= 1 && n >= 0 && n % rows_per_seq == 0,
+               "sq_top_k_filter_per_seq: rows_per_seq=%d does not divide n=%d", rows_per_seq, n);
+  if (n == 0) return SQ_OK;
+  if (V > SLICE) {
+    SQ_CHECK_WIDE_LAUNCH(launch_wide(top_k_filter_kernel<true, true>, n, 1, V, (cudaStream_t)stream, (__half*)logits, ld,
+                                     V, top_k, rows_per_seq), "sq_top_k_filter_per_seq");
+    return SQ_OK;
+  }
+  top_k_filter_kernel<false, true><<<n, NT, 0, (cudaStream_t)stream>>>((__half*)logits, ld, V, top_k, rows_per_seq);
+  SQ_CHECK_LAUNCH("sq_top_k_filter_per_seq");
   return SQ_OK;
 }

@@ -160,6 +160,15 @@ def top_p_filter_(logits, top_p: float, T: float):
     return logits
 
 
+def top_k_filter_(logits, k: int):
+    """Top-k filter in place on (n, V) fp16 logits: the k best of each row (raw logit descending, equal values by
+    ascending index) keep their value, every other one becomes -inf.  k == 0 is off, k >= V filters nothing."""
+    _need(logits, F16, "top_k_filter_")
+    n, V = logits.shape
+    check(_lib.load().sq_top_k_filter(ptr(logits), logits.stride(0), n, V, int(k), stream_ptr()), "sq_top_k_filter")
+    return logits
+
+
 def argmax_rows(logits, out=None):
     n, V = logits.shape
     if out is None:
@@ -545,6 +554,20 @@ def top_p_filter_per_seq_(logits, top_p, T, rows_per_seq: int):
     _seq_params("top_p_filter_per_seq_", B, top_p=top_p, T=T)
     check(_lib.load().sq_top_p_filter_per_seq(ptr(logits), logits.stride(0), n, V, ptr(top_p), ptr(T), rows_per_seq,
                                               stream_ptr()), "sq_top_p_filter_per_seq")
+    return logits
+
+
+def top_k_filter_per_seq_(logits, top_k, rows_per_seq: int):
+    """top_k_filter_ in place on (n, V) fp16 logits whose row r belongs to sequence r // rows_per_seq, at that sequence's
+    top_k[b] ((B,) int32 on the device); rows of a sequence with top_k <= 0 or >= V are left untouched."""
+    _need(logits, F16, "top_k_filter_per_seq_")
+    n, V = logits.shape
+    B = n // rows_per_seq if rows_per_seq > 0 else 0
+    if top_k is None or top_k.dtype != torch.int32 or not top_k.is_cuda or top_k.dim() != 1 or top_k.shape[0] < B \
+            or top_k.stride(0) != 1:
+        raise TypeError(f"top_k_filter_per_seq_: top_k must be a contiguous ({B},) int32 CUDA tensor")
+    check(_lib.load().sq_top_k_filter_per_seq(ptr(logits), logits.stride(0), n, V, ptr(top_k), rows_per_seq,
+                                              stream_ptr()), "sq_top_k_filter_per_seq")
     return logits
 
 

@@ -262,11 +262,12 @@ def decode_chunk(tree, chunk, limits, stop=DEFAULT_STOP):
 
 @torch.inference_mode()
 def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: int, stop=DEFAULT_STOP,
-                     refill: bool = False, seeds=None, policies=None):
+                     refill: bool = False, seeds=None, policies=None, top_k: int = 0):
     """--batch B: the same metric loop with B prompts decoded together (sequoia_b200.batch.BatchTree).  Chunked: B
     prompts at a time, each chunk until its last sequence stops.  refill: one batch whose finished slots take the next
     prompt (BatchTree.admit).  seeds: one per prompt (--device-rng): each sequence draws its random numbers on the device
-    from its own seed.  policies: one per prompt (--policies), in place of `policy` for all."""
+    from its own seed.  policies: one per prompt (--policies), in place of `policy` for all.  top_k: every sampled
+    prompt's top-k filter (--top-k, 0 = off)."""
     from sequoia_b200.batch import BatchTree
     steps = decoded = 0                          # steps: target steps summed over sequences (per-sequence tokens / step)
     total_time = 0.0
@@ -277,7 +278,7 @@ def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: i
         i0 = c * B
         pol = policy if policies is None else policies[i0:i0 + len(chunk)]
         tree = BatchTree(draft, target, chunk, grow_map, policy=pol, temperature=T, top_p=top_p, max_length=M,
-                         max_target_seq=M, seeds=None if seeds is None else seeds[i0:i0 + len(chunk)])
+                         max_target_seq=M, seeds=None if seeds is None else seeds[i0:i0 + len(chunk)], top_k=top_k)
         torch.cuda.synchronize()
         t1 = time.time()
         if refill:
@@ -325,6 +326,8 @@ def build_parser():
     ap.add_argument("--policies", type=str, default=None,
                     help="with --batch and --tree spec: a comma-separated list of spec / greedy; prompt i decodes with "
                          "policies[i %% len], greedy and sampled prompts in one batch")
+    ap.add_argument("--top-k", type=int, default=0,
+                    help="with --batch: keep the K best target logits of each row before top_p (0 = off)")
     ap.add_argument("--target-weights", type=str, default="fp16", choices=["fp16", "fp8"],
                     help="fp8: the target's layer projections quantized to E4M3 with per-channel scales at load")
     return ap
@@ -370,6 +373,16 @@ def prompt_policies(args, n_prompts: int):
     return [pols[i % len(pols)] for i in range(n_prompts)]
 
 
+def batch_top_k(args) -> int:
+    """--top-k: every prompt's top_k (0 = off).  Refused below 0, and without --batch: the lone trees keep the
+    reference's sampling."""
+    if args.top_k < 0:
+        raise SystemExit(f"--top-k must be >= 0, got {args.top_k}")
+    if args.top_k and args.batch == 1 and not args.refill:
+        raise SystemExit("--top-k runs with --batch (the batched tree); the lone trees keep the reference's sampling")
+    return args.top_k
+
+
 def main(argv=None):
     args = build_parser().parse_args(argv)
     print(args)
@@ -383,6 +396,7 @@ def main(argv=None):
         raise SystemExit("--target-weights fp8 runs without --offloading")
     seeds = device_rng_seeds(args, len(prompts))
     policies = prompt_policies(args, len(prompts))
+    top_k = batch_top_k(args)
     if args.batch != 1 or args.refill:
         B = check_batch_args(args, len(prompts))
         target = GraphInferenceEngineTG(max_length=args.M, model_name_or_path=args.target, dtype=torch.float16,
@@ -393,7 +407,7 @@ def main(argv=None):
         grow_map = torch.load(path)
         assert args.M >= MAX_NEW_LEN + grow_map["size"], "--M must hold 256 tokens + the tree (README.md:47 of the reference)"
         res = simulation_batch(target, draft, prompts, grow_map, args.tree, args.T, args.P, args.M, B, stop=stop,
-                               refill=args.refill, seeds=seeds, policies=policies)
+                               refill=args.refill, seeds=seeds, policies=policies, top_k=top_k)
         print(json.dumps({k: (round(v, 5) if isinstance(v, float) else v) for k, v in res.items()}))
         return res
     target = (tcls(max_length=args.M, model_name_or_path=args.target, dtype=torch.float16, device=DEV)
