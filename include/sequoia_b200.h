@@ -40,6 +40,8 @@ extern "C" {
 #define SQ_ST_SKIPPED 7
 #define SQ_ST_M 8 /* host-written: length of tokens / position_ids (max_length); bounds the walk's epilogue writes */
 #define SQ_ST_FROZEN 9 /* host-written, batched calls only: nonzero = finished sequence, nothing of it is written */
+#define SQ_ST_FINISH 10 /* the *_batch_stop walks only: 0 = go on, 1 = a stop id ended the sequence, 2 = its length limit */
+#define SQ_ST_END 11    /* the *_batch_stop walks only: the sequence's final length when SQ_ST_FINISH != 0, else 0 */
 #define SQ_ST_WORDS 16
 
 typedef uint16_t sq_half;
@@ -420,6 +422,33 @@ int sq_accept_stochastic_batch_mixed(const sq_half* target_logits, int64_t ld_t,
                                      const int32_t* depth, int S, int V, const float* T, const int32_t* greedy,
                                      int64_t* tokens, int64_t* position_ids, int64_t ld_seq, int32_t* accept_idx,
                                      int64_t ld_acc, int32_t* state, int B, int max_target_seq, int policy, void* stream);
+/* Per-sequence stop ids and length limits (stop mode).  stop_ids: (B, SQ_MAX_STOP) int32 device array, sequence b's ids
+ * padded with -1 (an id < 0 never matches); end_limit: (B,) int32 device array, sequence b's absolute length limit E_b
+ * (prompt length + new-token budget), <= 0 = none.  greedy: as in the mixed forms, or NULL:
+ *   sq_accept_stochastic_batch_stop: sq_accept_stochastic_batch_per_seq (greedy NULL: every sequence samples) or
+ *     sq_accept_stochastic_batch_mixed (greedy set: only the sampling sequences walk);
+ *   sq_accept_greedy_batch_stop: sq_accept_greedy_batch (greedy NULL: every sequence walks) or
+ *     sq_accept_greedy_batch_mixed (greedy set: only the greedy sequences walk).
+ * Each walk runs without the fixed 0 / 2 end rule and commits exactly what that walk commits (tokens, position_ids,
+ * accept_idx, state words 0..9).  Then, with P = state[SQ_ST_P] at the start of the step and n = a + 1 (n = a when the
+ * NaN flag ended the walk, or no bonus token fitted the buffer), the committed tokens[P .. n) are scanned for the first
+ * stop id, at j: its end is j + 1; E_b counts too when E_b <= n.  SQ_ST_END = the smaller end, SQ_ST_FINISH = 1 when the
+ * stop id ends first or on a tie, 2 when E_b does; both 0 when neither applies.  The output of a stop-mode step is thus
+ * exactly tokens[:SQ_ST_END] of the step without a stop rule.  Refused with SQ_ERR_INVALID_ARG before any launch: a null
+ * stop_ids, end_limit (or T), and everything the per-sequence and mixed forms refuse. */
+#define SQ_MAX_STOP 8
+int sq_accept_stochastic_batch_stop(const sq_half* target_logits, int64_t ld_t, const sq_half* draft_logits,
+                                    int64_t ld_d, const int32_t* row_base, const int32_t* row_step, const sq_half* r,
+                                    const sq_half* noise, int64_t ld_noise, const int32_t* succ_off, const int32_t* succ,
+                                    const int32_t* depth, int S, int V, const float* T, const int32_t* greedy,
+                                    const int32_t* stop_ids, const int32_t* end_limit, int64_t* tokens,
+                                    int64_t* position_ids, int64_t ld_seq, int32_t* accept_idx, int64_t ld_acc,
+                                    int32_t* state, int B, int max_target_seq, int policy, void* stream);
+int sq_accept_greedy_batch_stop(const int64_t* target_token, const int32_t* succ_off, const int32_t* succ,
+                                const int32_t* depth, int S, int64_t* tokens, int64_t* position_ids, int64_t ld_seq,
+                                int32_t* accept_idx, int64_t ld_acc, int32_t* state, const int32_t* greedy,
+                                const int32_t* stop_ids, const int32_t* end_limit, int B, int max_target_seq,
+                                void* stream);
 
 /* ---- ragged batches: a forward over a chosen set of the B sequences, each with its own row count ----
  * A part list names the sequences to run.  Part j is n rows of sequence seq in that sequence's tree-relative addressing:

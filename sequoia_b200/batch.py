@@ -19,6 +19,13 @@ A sampled sequence draws from softmax(top_p(top_k(logits)) / T): the accept walk
 top_k best raw logits (0 = off), then to top_p, and speculative sampling stays exact for the filtered distribution.
 Each filter joins the captured graphs the first time a sampled sequence needs it (one recapture each); after that any
 values run in the same graphs.
+
+How a sequence ends: in default mode (every sequence with stop_tokens=None and max_new_tokens=None) the walks end it at
+an accepted 0 or 2, the reference's rule.  Stop mode starts the first time a sequence has a stop set (any list, [] too)
+or a token budget, and then stays on: the walks run without the fixed rule and then cut each sequence's committed tokens
+at the first of its stop ids, or at its length limit len(prompt) + max_new_tokens, on the device (state words
+SQ_ST_FINISH / SQ_ST_END).  The output is then exactly a prefix of the output without a stop rule.  finish_reason[b]
+says why slot b ended: "stop", "length", "nan" or "room" (None while it decodes).
 """
 from __future__ import annotations
 
@@ -33,7 +40,11 @@ from .tree import _Static, check_vocab
 
 F16 = torch.float16
 ST_P, ST_M, ST_FROZEN = 0, 8, 9
+ST_FINISH, ST_END = _lib.SQ_ST_FINISH, _lib.SQ_ST_END
+MAX_STOP = _lib.SQ_MAX_STOP
+INT32_MAX = (1 << 31) - 1
 POLICIES = ("spec", "greedy")
+_PREVIOUS = object()        # admit(): keep the slot's previous stop set / budget
 
 
 def draw_random(prompts: Sequence[torch.Tensor], M: int, S: int, V: int):
@@ -94,6 +105,69 @@ def _top_ks(top_k, B: int) -> List[int]:
     return [check_top_k(top_k)] * B
 
 
+def check_stop_tokens(stop_tokens, V: Optional[int] = None) -> Optional[tuple]:
+    """A stop set: None (no stop ids), or a collection of at most MAX_STOP distinct integer ids in [0, V) (the upper bound
+    is checked once V is given).  -> None or the sorted distinct ids."""
+    if stop_tokens is None:
+        return None
+    if isinstance(stop_tokens, (str, bytes)) or not isinstance(stop_tokens, (Sequence, set, frozenset)):
+        raise ValueError(f"stop_tokens must be None or a collection of token ids, got {stop_tokens!r}")
+    ids = set()
+    for t in stop_tokens:
+        if isinstance(t, bool) or not isinstance(t, numbers.Integral) or t < 0 or (V is not None and t >= V):
+            raise ValueError(f"stop_tokens: {t!r} is not a token id in [0, {V if V is not None else 'V'})")
+        ids.add(int(t))
+    if len(ids) > MAX_STOP:
+        raise ValueError(f"stop_tokens: {len(ids)} distinct ids, at most {MAX_STOP}")
+    return tuple(sorted(ids))
+
+
+def _is_collection(x) -> bool:
+    return isinstance(x, (Sequence, set, frozenset)) and not isinstance(x, (str, bytes))
+
+
+def _stop_sets(stop_tokens, B: int) -> List[Optional[tuple]]:
+    """One stop set (None or a collection of ids) for all B sequences, or a sequence of B of them (a non-empty sequence
+    whose entries are all None or collections)."""
+    if isinstance(stop_tokens, Sequence) and _is_collection(stop_tokens) and len(stop_tokens) > 0 \
+            and all(t is None or _is_collection(t) for t in stop_tokens):
+        sets = [check_stop_tokens(t) for t in stop_tokens]
+        if len(sets) != B:
+            raise ValueError(f"stop_tokens: {len(sets)} sets for {B} sequences")
+        return sets
+    return [check_stop_tokens(stop_tokens)] * B
+
+
+def check_max_new_tokens(max_new_tokens) -> Optional[int]:
+    """A token budget: None (no limit) or an integer >= 1."""
+    if max_new_tokens is None:
+        return None
+    if isinstance(max_new_tokens, bool) or not isinstance(max_new_tokens, numbers.Integral) or max_new_tokens < 1:
+        raise ValueError(f"max_new_tokens must be None or an integer >= 1, got {max_new_tokens!r}")
+    return int(max_new_tokens)
+
+
+def _budgets(max_new_tokens, B: int) -> List[Optional[int]]:
+    """One budget for all B sequences, or a sequence of B of them."""
+    if _is_collection(max_new_tokens):
+        ns = [check_max_new_tokens(n) for n in max_new_tokens]
+        if len(ns) != B:
+            raise ValueError(f"max_new_tokens: {len(ns)} values for {B} sequences")
+        return ns
+    return [check_max_new_tokens(max_new_tokens)] * B
+
+
+def _stop_row(ids: Optional[tuple]) -> List[int]:
+    """A stop set as its device row: the ids padded with -1 to MAX_STOP."""
+    ids = ids or ()
+    return list(ids) + [-1] * (MAX_STOP - len(ids))
+
+
+def _end_limit(prompt_len: int, budget: Optional[int]) -> int:
+    """The absolute length limit len(prompt) + max_new_tokens the device holds (0 = none; clamped to int32)."""
+    return 0 if budget is None else min(prompt_len + budget, INT32_MAX)
+
+
 def _per_seq(value, B: int, name: str) -> List[float]:
     """One value (a Python, numpy or 0-d tensor scalar) for all B sequences, or a sequence of B values."""
     if isinstance(value, numbers.Real) or (isinstance(value, torch.Tensor) and value.dim() == 0):
@@ -131,16 +205,23 @@ class BatchTree:
     seeds: None (r and rand drawn with torch's CPU generator as a lone SpecTree draws them, the bonus noise with torch's
     CUDA generator), or one integer in [0, 2^64) per prompt: each sequence then draws all its random numbers on the
     device from a Philox stream keyed by its seed, so its output does not depend on its slot or its neighbours ("greedy"
-    takes seeds and ignores them)."""
+    takes seeds and ignores them).
+    stop_tokens: None, or a collection of at most 8 distinct ids in [0, V), for all sequences; or one such value per
+    prompt.  max_new_tokens: None, or an integer >= 1, for all sequences or one per prompt.  Any stop set (an empty one
+    too) or budget turns on stop mode (module docstring): sequence b then ends at the first of its stop ids that it
+    commits, or when it holds len(prompt) + max_new_tokens tokens, whichever comes first, and verify() returns exactly
+    the tokens up to there with terminal True.  Both policies honour them."""
 
     def __init__(self, draft, target, prompts: Sequence[torch.Tensor], grow_map: dict,
                  policy: Union[str, Sequence[str]] = "spec",
                  temperature: Union[float, Sequence[float]] = 0.6, top_p: Union[float, Sequence[float]] = 1.0,
                  max_length: int = 256, max_target_seq: Optional[int] = None,
-                 seeds: Optional[Sequence[int]] = None, top_k: Union[int, Sequence[int]] = 0):
+                 seeds: Optional[Sequence[int]] = None, top_k: Union[int, Sequence[int]] = 0,
+                 stop_tokens=None, max_new_tokens: Union[None, int, Sequence[Optional[int]]] = None):
         B = len(prompts)
         policies = _policies(policy, B)
         top_ks = _top_ks(top_k, B)
+        stops, budgets = _stop_sets(stop_tokens, B), _budgets(max_new_tokens, B)
         temps, top_ps = _per_seq(temperature, B, "temperature"), _per_seq(top_p, B, "top_p")
         for t, p in zip(temps, top_ps):
             check_sampling(t, p)
@@ -170,6 +251,7 @@ class BatchTree:
         V = self.V = draft.engine.model_config.vocab_size
         for pol in set(policies):
             check_vocab(pol, V)
+        stops = [check_stop_tokens(t, V) for t in stops]
         M = max_length
         for p in prompts:
             if len(p) + S - 1 > M:
@@ -187,6 +269,14 @@ class BatchTree:
         self.top_k_dev = torch.tensor([0 if pol == "greedy" else min(k, V) for pol, k in zip(policies, top_ks)],
                                       dtype=torch.int32, device=dev)
         self.use_top_k = any(pol == "spec" and 0 < k < V for pol, k in zip(policies, top_ks))
+        # stop mode: each slot's stop ids (-1 padded) and absolute length limit (0 = none) on the device, read by the stop
+        # walks inside the captured graphs, which replace the walks the first time a slot has either (one recapture)
+        self.stop_tokens, self.max_new_tokens = stops, budgets
+        self.stop_ids_dev = torch.tensor([_stop_row(t) for t in stops], dtype=torch.int32, device=dev)
+        self.end_limit_dev = torch.tensor([_end_limit(len(p), n) for p, n in zip(prompts, budgets)], dtype=torch.int32,
+                                          device=dev)
+        self.use_stop = any(t is not None for t in stops) or any(n is not None for n in budgets)
+        self.finish_reason: List[Optional[str]] = [None] * B
         i64 = dict(dtype=torch.int64, device=dev)
         self.tokens = torch.zeros(B, M, **i64)
         self.position_ids = torch.zeros(B, M, **i64)
@@ -267,7 +357,8 @@ class BatchTree:
 
     @torch.inference_mode()
     def admit(self, b: int, prompt: torch.Tensor, temperature: Optional[float] = None, top_p: Optional[float] = None,
-              seed: Optional[int] = None, policy: Optional[str] = None, top_k: Optional[int] = None):
+              seed: Optional[int] = None, policy: Optional[str] = None, top_k: Optional[int] = None,
+              stop_tokens=_PREVIOUS, max_new_tokens=_PREVIOUS):
         """Start `prompt` in the frozen slot b (finished, out of room, or stopped with freeze), at its own policy,
         temperature, top_p and top_k (default: the slot's previous values).  The next verify() runs its first verify next
         to the steady sequences.  The slot draws r and rand as a lone SpecTree on the prompt would, and runs its draft
@@ -277,11 +368,18 @@ class BatchTree:
         The first admission that puts both policies in the batch starts mixed mode: the draft, steady and post graphs are
         captured once more, on their next use.  A tree built all-greedy allocates r and rand at its first "spec"
         admission.  The first "spec" admission with 0 < top_k < V (in a tree that had none) captures the steady and post
-        graphs once more: the top-k filter joins the accept step."""
+        graphs once more: the top-k filter joins the accept step.
+        stop_tokens / max_new_tokens: the prompt's stop set and token budget (default: the slot's previous ones; None is
+        none).  The budget counts from this prompt.  The first admission that brings a stop set or a budget to a tree in
+        default mode captures the steady and post graphs once more: the stop walks replace the walks."""
         if policy is not None:
             check_policy(policy)
         if top_k is not None:
             top_k = check_top_k(top_k)
+        if stop_tokens is not _PREVIOUS:
+            stop_tokens = check_stop_tokens(stop_tokens, self.V)
+        if max_new_tokens is not _PREVIOUS:
+            max_new_tokens = check_max_new_tokens(max_new_tokens)
         if not 0 <= b < self.B:
             raise IndexError(f"slot {b} out of range for a batch of {self.B}")
         if not self.frozen[b]:
@@ -300,6 +398,8 @@ class BatchTree:
             seed = check_seed(seed)
         pol = self.policies[b] if policy is None else policy
         k = self.top_ks[b] if top_k is None else top_k
+        stop = self.stop_tokens[b] if stop_tokens is _PREVIOUS else stop_tokens
+        budget = self.max_new_tokens[b] if max_new_tokens is _PREVIOUS else max_new_tokens
         # (every other slot holds the tree's one policy until then, so a different one means both are present; at B = 1
         # it is a switch, which the single-policy graphs do not serve either)
         enter_mixed = not self.mixed and pol != ("greedy" if self.greedy else "spec")
@@ -321,11 +421,19 @@ class BatchTree:
             self.use_top_k = True                  # the same for the top-k filter
             for name in ("steady", "post"):
                 self.graphs.pop(name, None)
+        self.stop_tokens[b], self.max_new_tokens[b] = stop, budget
+        self.stop_ids_dev[b] = torch.tensor(_stop_row(stop), dtype=torch.int32)
+        self.end_limit_dev[b] = _end_limit(P, budget)
+        if (stop is not None or budget is not None) and not self.use_stop:
+            self.use_stop = True                   # the stop walks replace the walks: capture steady and post once more
+            for name in ("steady", "post"):
+                self.graphs.pop(name, None)
         if pol == "spec" and self.r is None:       # the first sampling sequence of a tree built all-greedy
             self.r = torch.zeros(self.B, self.M, dtype=F16, device=self.device)
             self.rand = torch.zeros(self.B, self.S, self.V, dtype=F16, device=self.device)
         self._load_prompt(b, prompt)
         self.frozen[b] = False
+        self.finish_reason[b] = None
         self.last[b] = None
         self.ground_truth_len[b] = P
         self.target_kv_len[b] = 0
@@ -377,14 +485,24 @@ class BatchTree:
         st = self.st
         if self.greedy:
             ops.argmax_rows(self.target_logits, self.target_token)
+            if self.use_stop:
+                ops.accept_greedy_batch_stop(self.target_token, st.succ_off, st.succ, st.depth, self.S, None,
+                                             self.stop_ids_dev, self.end_limit_dev, self.tokens, self.position_ids,
+                                             self.accept_idx, self.state, self.max_target_seq)
+                return
             ops.accept_greedy_batch(self.target_token, st.succ_off, st.succ, st.depth, self.S, self.tokens,
                                     self.position_ids, self.accept_idx, self.state, self.max_target_seq)
             return
         if self.mixed:                             # the greedy sequences' walk; the sampling ones' follows below
             ops.argmax_rows(self.target_logits, self.target_token)
-            ops.accept_greedy_batch_mixed(self.target_token, st.succ_off, st.succ, st.depth, self.S, self.greedy_dev,
-                                          self.tokens, self.position_ids, self.accept_idx, self.state,
-                                          self.max_target_seq)
+            if self.use_stop:
+                ops.accept_greedy_batch_stop(self.target_token, st.succ_off, st.succ, st.depth, self.S, self.greedy_dev,
+                                             self.stop_ids_dev, self.end_limit_dev, self.tokens, self.position_ids,
+                                             self.accept_idx, self.state, self.max_target_seq)
+            else:
+                ops.accept_greedy_batch_mixed(self.target_token, st.succ_off, st.succ, st.depth, self.S, self.greedy_dev,
+                                              self.tokens, self.position_ids, self.accept_idx, self.state,
+                                              self.max_target_seq)
         if self.use_top_k:                         # top_k before top_p: top_p renormalises over the k survivors
             ops.top_k_filter_per_seq_(self.target_logits, self.top_k_dev, self.S)
         if self.use_top_p:
@@ -394,6 +512,13 @@ class BatchTree:
                 ops.rng_exponential_batch(self.noise, self.seeds, self.steps, self.state)
             else:
                 self.noise.exponential_(1.0)
+        if self.use_stop:
+            ops.accept_stochastic_batch_stop(self.target_logits, self.draft_logits, self.row_base, self.row_step, self.r,
+                                             self.noise, st.succ_off, st.succ, st.depth, self.S, self.T_dev,
+                                             self.greedy_dev if self.mixed else None, self.stop_ids_dev,
+                                             self.end_limit_dev, self.tokens, self.position_ids, self.accept_idx,
+                                             self.state, self.max_target_seq)
+            return
         if self.mixed:
             ops.accept_stochastic_batch_mixed(self.target_logits, self.draft_logits, self.row_base, self.row_step, self.r,
                                               self.noise, st.succ_off, st.succ, st.depth, self.S, self.T_dev,
@@ -514,10 +639,17 @@ class BatchTree:
                 out.append(self.last[b])
                 continue
             a, terminal, skipped = int(hs[b, 1]), bool(hs[b, 2]), bool(hs[b, 7])
-            if terminal:
+            finish = int(hs[b, ST_FINISH])          # (always 0 in default mode: only the stop walks write it)
+            if finish:
+                valid = self.tokens[b, :int(hs[b, ST_END])]
+                terminal = True
+                self.finish_reason[b] = "stop" if finish == 1 else "length"
+            elif terminal:
                 valid = self.tokens[b, :a]
+                self.finish_reason[b] = "nan" if bool(hs[b, 6]) else "stop"
             elif skipped:
                 valid = self.tokens[b, :min(a + 1, self.M)]
+                self.finish_reason[b] = "room"
             else:
                 valid = self.tokens[b, :a + 1]
                 self.ground_truth_len[b] = a + 1

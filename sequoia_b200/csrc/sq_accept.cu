@@ -197,14 +197,18 @@ __global__ void __launch_bounds__(ANT) accept_stochastic_kernel(
 
 // BATCH: grid (B), one walk per sequence; target_token rows of S per sequence, the rest as in BatchArgs.
 // MIXED (BATCH only): only the sequences with greedy[b] nonzero walk; the others' blocks exit as a frozen one does.
-template <bool BATCH, bool MIXED = false>
+// STOP (BATCH only): stop mode, as in accept_stochastic_cluster_kernel: no fixed 0 / 2 end rule, then stop_cut with the
+// rows of stop_ids / end_limit (nullptr in every other instance).
+template <bool BATCH, bool MIXED = false, bool STOP = false>
 __global__ void accept_greedy_kernel(const int64_t* __restrict__ target_token, const int32_t* __restrict__ succ_off,
                                      const int32_t* __restrict__ succ, const int32_t* __restrict__ depth, int S,
                                      int64_t* __restrict__ tokens, int64_t* __restrict__ position_ids,
                                      int32_t* __restrict__ accept_idx, int32_t* __restrict__ state,
                                      int max_target_seq, int64_t ld_seq, int64_t ld_acc,
-                                     const int32_t* __restrict__ greedy) {
+                                     const int32_t* __restrict__ greedy, const int32_t* __restrict__ stop_ids,
+                                     const int32_t* __restrict__ end_limit) {
   static_assert(BATCH || !MIXED, "a per-sequence policy needs the batched kernel");
+  static_assert(BATCH || !STOP, "stop mode needs the batched kernel");
   __shared__ int32_t sh_acc[1024];
   __shared__ int sh_n, sh_term;
   __shared__ long long sh_bonus;
@@ -218,6 +222,8 @@ __global__ void accept_greedy_kernel(const int64_t* __restrict__ target_token, c
     position_ids += b * ld_seq;
     accept_idx += b * ld_acc;
   }
+  __shared__ int32_t sh_stop[STOP ? SQ_MAX_STOP + 1 : 1];
+  if constexpr (STOP) stop_row_load(sh_stop, stop_ids, end_limit, b);
   const int P = state[ST_P];
   if (threadIdx.x == 0) {
     int cur = 0, n_new = 0, term = 0;
@@ -232,7 +238,7 @@ __global__ void accept_greedy_kernel(const int64_t* __restrict__ target_token, c
       const int slot = P - 1 + acc;
       sh_acc[n_new++] = slot;
       const int64_t t = tokens[slot];
-      if (t == 0 || t == 2) { term = 1; break; }
+      if (!STOP && (t == 0 || t == 2)) { term = 1; break; }
       cur = acc;
     }
     sh_n = n_new;
@@ -242,6 +248,7 @@ __global__ void accept_greedy_kernel(const int64_t* __restrict__ target_token, c
   __syncthreads();
   finish_verify(sh_acc, sh_n, P, sh_term != 0, false, (int64_t)sh_bonus, false, depth, S, tokens, position_ids,
                 accept_idx, state, max_target_seq);
+  if constexpr (STOP) stop_cut(sh_stop, sh_n, P, sh_term != 0, tokens, state, max_target_seq);
 }
 
 }  // namespace sq
@@ -280,27 +287,36 @@ extern "C" int sq_accept_greedy(const int64_t* target_token, const int32_t* succ
   SQ_CHECK_ARG(S >= 1 && S <= 1024, "sq_accept_greedy: S=%d unsupported", S);
   accept_greedy_kernel<false><<<1, 256, 0, (cudaStream_t)stream>>>(target_token, succ_off, succ, depth, S, tokens,
                                                                    position_ids, accept_idx, state, max_target_seq, 0, 0,
-                                                                   nullptr);
+                                                                   nullptr, nullptr, nullptr);
   SQ_CHECK_LAUNCH("sq_accept_greedy");
   return SQ_OK;
 }
 
-// sq_accept_greedy_batch (greedy == nullptr) and its mixed-policy form
+// sq_accept_greedy_batch (greedy == nullptr), its mixed-policy form and (stop_ids != nullptr) the stop forms
 static int accept_greedy_batch(const char* name, const int64_t* target_token, const int32_t* succ_off,
                                const int32_t* succ, const int32_t* depth, int S, int64_t* tokens, int64_t* position_ids,
                                int64_t ld_seq, int32_t* accept_idx, int64_t ld_acc, int32_t* state, int B,
-                               int max_target_seq, const int32_t* greedy, void* stream) {
+                               int max_target_seq, const int32_t* greedy, void* stream,
+                               const int32_t* stop_ids = nullptr, const int32_t* end_limit = nullptr) {
   SQ_CHECK_ARG(S >= 1 && S <= 1024, "%s: S=%d unsupported", name, S);
   SQ_CHECK_ARG(B >= 1 && B <= SQ_MAX_BATCH, "%s: B=%d (1..%d)", name, B, SQ_MAX_BATCH);
   SQ_CHECK_ARG(ld_acc >= S && ld_seq >= 1, "%s: accept_idx rows of %lld < S=%d", name, (long long)ld_acc, S);
-  if (greedy)
+  if (stop_ids && greedy)
+    accept_greedy_kernel<true, true, true><<<B, 256, 0, (cudaStream_t)stream>>>(
+        target_token, succ_off, succ, depth, S, tokens, position_ids, accept_idx, state, max_target_seq, ld_seq, ld_acc,
+        greedy, stop_ids, end_limit);
+  else if (stop_ids)
+    accept_greedy_kernel<true, false, true><<<B, 256, 0, (cudaStream_t)stream>>>(
+        target_token, succ_off, succ, depth, S, tokens, position_ids, accept_idx, state, max_target_seq, ld_seq, ld_acc,
+        nullptr, stop_ids, end_limit);
+  else if (greedy)
     accept_greedy_kernel<true, true><<<B, 256, 0, (cudaStream_t)stream>>>(
         target_token, succ_off, succ, depth, S, tokens, position_ids, accept_idx, state, max_target_seq, ld_seq, ld_acc,
-        greedy);
+        greedy, nullptr, nullptr);
   else
     accept_greedy_kernel<true><<<B, 256, 0, (cudaStream_t)stream>>>(target_token, succ_off, succ, depth, S, tokens,
                                                                     position_ids, accept_idx, state, max_target_seq,
-                                                                    ld_seq, ld_acc, nullptr);
+                                                                    ld_seq, ld_acc, nullptr, nullptr, nullptr);
   SQ_CHECK_LAUNCH(name);
   return SQ_OK;
 }
@@ -322,20 +338,22 @@ extern "C" int sq_accept_greedy_batch_mixed(const int64_t* target_token, const i
                              ld_seq, accept_idx, ld_acc, state, B, max_target_seq, greedy, stream);
 }
 
-// sq_accept_stochastic_batch (T_seq == nullptr), its per-sequence form and (greedy != nullptr) the mixed-policy form
+// sq_accept_stochastic_batch (T_seq == nullptr), its per-sequence form, (greedy != nullptr) the mixed-policy form and
+// (stop_ids != nullptr) the stop forms
 static int accept_stochastic_batch(const char* name, const sq_half* target_logits, int64_t ld_t,
                                    const sq_half* draft_logits, int64_t ld_d, const int32_t* row_base,
                                    const int32_t* row_step, const sq_half* r, const sq_half* noise, int64_t ld_noise,
                                    const int32_t* succ_off, const int32_t* succ, const int32_t* depth, int S, int V,
                                    float T, const float* T_seq, int64_t* tokens, int64_t* position_ids, int64_t ld_seq,
                                    int32_t* accept_idx, int64_t ld_acc, int32_t* state, int B, int max_target_seq,
-                                   int policy, void* stream, const int32_t* greedy = nullptr) {
+                                   int policy, void* stream, const int32_t* greedy = nullptr,
+                                   const int32_t* stop_ids = nullptr, const int32_t* end_limit = nullptr) {
   SQ_CHECK_ARG(S >= 1 && S <= 1024, "%s: S=%d unsupported", name, S);
   SQ_CHECK_ARG(B >= 1 && B <= SQ_MAX_BATCH, "%s: B=%d (1..%d)", name, B, SQ_MAX_BATCH);
   SQ_CHECK_ARG((policy & ~3) == 0, "%s: unknown policy bits %d", name, policy);
   SQ_CHECK_ARG(row_base && row_step, "%s: null draft-row table", name);
   SQ_CHECK_ARG(ld_acc >= S && ld_noise >= V, "%s: accept_idx / noise rows too short", name);
-  BatchArgs ba{B, ld_seq, ld_noise, ld_acc, row_base, row_step, greedy};
+  BatchArgs ba{B, ld_seq, ld_noise, ld_acc, row_base, row_step, greedy, stop_ids, end_limit};
   return sq::launch_accept_cluster(target_logits, ld_t, draft_logits, ld_d, r, noise, succ_off, succ, depth, S, V, T, tokens,
                                    position_ids, accept_idx, state, max_target_seq, policy, stream, &ba, T_seq);
 }
@@ -376,4 +394,30 @@ extern "C" int sq_accept_stochastic_batch_mixed(const sq_half* target_logits, in
   return accept_stochastic_batch("sq_accept_stochastic_batch_mixed", target_logits, ld_t, draft_logits, ld_d, row_base,
                                  row_step, r, noise, ld_noise, succ_off, succ, depth, S, V, 1.0f, T, tokens, position_ids,
                                  ld_seq, accept_idx, ld_acc, state, B, max_target_seq, policy, stream, greedy);
+}
+
+extern "C" int sq_accept_stochastic_batch_stop(const sq_half* target_logits, int64_t ld_t, const sq_half* draft_logits,
+                                               int64_t ld_d, const int32_t* row_base, const int32_t* row_step,
+                                               const sq_half* r, const sq_half* noise, int64_t ld_noise,
+                                               const int32_t* succ_off, const int32_t* succ, const int32_t* depth, int S,
+                                               int V, const float* T, const int32_t* greedy, const int32_t* stop_ids,
+                                               const int32_t* end_limit, int64_t* tokens, int64_t* position_ids,
+                                               int64_t ld_seq, int32_t* accept_idx, int64_t ld_acc, int32_t* state, int B,
+                                               int max_target_seq, int policy, void* stream) {
+  SQ_CHECK_ARG(T != nullptr, "sq_accept_stochastic_batch_stop: null temperature array");
+  SQ_CHECK_ARG(stop_ids != nullptr && end_limit != nullptr, "sq_accept_stochastic_batch_stop: null stop_ids or end_limit");
+  return accept_stochastic_batch("sq_accept_stochastic_batch_stop", target_logits, ld_t, draft_logits, ld_d, row_base,
+                                 row_step, r, noise, ld_noise, succ_off, succ, depth, S, V, 1.0f, T, tokens, position_ids,
+                                 ld_seq, accept_idx, ld_acc, state, B, max_target_seq, policy, stream, greedy, stop_ids,
+                                 end_limit);
+}
+
+extern "C" int sq_accept_greedy_batch_stop(const int64_t* target_token, const int32_t* succ_off, const int32_t* succ,
+                                           const int32_t* depth, int S, int64_t* tokens, int64_t* position_ids,
+                                           int64_t ld_seq, int32_t* accept_idx, int64_t ld_acc, int32_t* state,
+                                           const int32_t* greedy, const int32_t* stop_ids, const int32_t* end_limit, int B,
+                                           int max_target_seq, void* stream) {
+  SQ_CHECK_ARG(stop_ids != nullptr && end_limit != nullptr, "sq_accept_greedy_batch_stop: null stop_ids or end_limit");
+  return accept_greedy_batch("sq_accept_greedy_batch_stop", target_token, succ_off, succ, depth, S, tokens, position_ids,
+                             ld_seq, accept_idx, ld_acc, state, B, max_target_seq, greedy, stream, stop_ids, end_limit);
 }

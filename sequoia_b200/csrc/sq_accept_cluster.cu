@@ -79,7 +79,9 @@ struct ClusterCtx {
 // draft rows by 1/T[b]; otherwise `temp` is the scalar 1/T.
 // MIXED (PER_SEQ only): the cluster of a sequence with ba.greedy[b] nonzero exits where a frozen one does and writes
 // nothing (its walk is the greedy kernel's).
-template <bool BATCH, int NCH, bool PER_SEQ = false, bool MIXED = false>
+// STOP (PER_SEQ only): stop mode.  The fixed 0 / 2 end rule is compiled out; rank 0 then cuts the committed tokens at the
+// sequence's stop ids and length limit (ba.stop_ids / ba.end_limit, stop_cut) and writes ST_FINISH / ST_END.
+template <bool BATCH, int NCH, bool PER_SEQ = false, bool MIXED = false, bool STOP = false>
 __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(CNT) accept_stochastic_cluster_kernel(
     const __half* __restrict__ target_logits, int64_t ld_t, const __half* __restrict__ draft_logits, int64_t ld_d,
     const __half* __restrict__ r, const __half* __restrict__ noise, const int32_t* __restrict__ succ_off,
@@ -88,6 +90,7 @@ __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(CNT) accept_stochas
     int32_t* __restrict__ state, int max_target_seq, int policy, BatchArgs ba) {
   static_assert(BATCH || !PER_SEQ, "per-sequence parameters need the batched kernel");
   static_assert(PER_SEQ || !MIXED, "a per-sequence policy needs the per-sequence temperature");
+  static_assert(PER_SEQ || !STOP, "stop mode needs the per-sequence walk");
   __shared__ Xch xch;
   __shared__ float red[CNW];
   __shared__ int32_t sh_acc[1024];
@@ -105,6 +108,8 @@ __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(CNT) accept_stochas
     position_ids += b * ba.ld_seq;
     accept_idx += b * ba.ld_acc;
   }
+  __shared__ int32_t sh_stop[STOP ? SQ_MAX_STOP + 1 : 1];
+  if constexpr (STOP) stop_row_load(sh_stop, ba.stop_ids, ba.end_limit, b);
   const float inv_T = inv_temp(temp, b);
   ClusterCtx cx{cg::this_cluster(), &xch, 0, 0};
   cx.rank = (int)cx.cluster.block_rank();
@@ -243,7 +248,7 @@ __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(CNT) accept_stochas
     if (threadIdx.x == 0) sh_acc[n_new] = slot;
     ++n_new;
     const int64_t t = tokens[slot];
-    if (t == 0 || t == 2) { terminal = true; break; }        // (:208)
+    if (!STOP && (t == 0 || t == 2)) { terminal = true; break; }   // (:208)
     cur = accepted;
   }
   bool nan_flag = false;
@@ -291,6 +296,7 @@ __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(CNT) accept_stochas
   __syncthreads();
   finish_verify(sh_acc, n_new, P, terminal, nan_flag, bonus, true, depth, S, tokens, position_ids, accept_idx, state,
                 max_target_seq);
+  if constexpr (STOP) stop_cut(sh_stop, n_new, P, terminal, tokens, state, max_target_seq);
 }
 
 }  // namespace sq
@@ -303,6 +309,18 @@ static int launch_accept_nch(const sq_half* target_logits, int64_t ld_t, const s
                              const int32_t* depth, int S, int V, float T, int64_t* tokens, int64_t* position_ids,
                              int32_t* accept_idx, int32_t* state, int max_target_seq, int policy, void* stream,
                              const BatchArgs* batch, const float* T_seq) {
+  if (batch && T_seq && batch->stop_ids) {
+    if (batch->greedy)
+      accept_stochastic_cluster_kernel<true, NCH, true, true, true><<<dim3(CL, batch->B), CNT, 0, (cudaStream_t)stream>>>(
+          (const __half*)target_logits, ld_t, (const __half*)draft_logits, ld_d, (const __half*)r, (const __half*)noise,
+          succ_off, succ, depth, S, V, T_seq, tokens, position_ids, accept_idx, state, max_target_seq, policy, *batch);
+    else
+      accept_stochastic_cluster_kernel<true, NCH, true, false, true><<<dim3(CL, batch->B), CNT, 0, (cudaStream_t)stream>>>(
+          (const __half*)target_logits, ld_t, (const __half*)draft_logits, ld_d, (const __half*)r, (const __half*)noise,
+          succ_off, succ, depth, S, V, T_seq, tokens, position_ids, accept_idx, state, max_target_seq, policy, *batch);
+    SQ_CHECK_LAUNCH("sq_accept_stochastic_batch_stop");
+    return SQ_OK;
+  }
   if (batch && T_seq && batch->greedy) {
     accept_stochastic_cluster_kernel<true, NCH, true, true><<<dim3(CL, batch->B), CNT, 0, (cudaStream_t)stream>>>(
         (const __half*)target_logits, ld_t, (const __half*)draft_logits, ld_d, (const __half*)r, (const __half*)noise,

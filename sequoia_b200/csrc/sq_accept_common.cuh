@@ -7,13 +7,16 @@ namespace sq {
 // Per-sequence addressing of the batched walks (sequence b = blockIdx.y): tokens / position_ids / r rows of ld_seq
 // elements, noise rows of ld_noise, accept_idx rows of ld_acc, target logits (B*S, V), and the draft-logit row of node k
 // at row_base[k] + b * row_step[k].  greedy: the (B,) per-sequence policy of the mixed walks (nonzero = greedy), nullptr
-// for every other batched walk.
+// for every other batched walk.  stop_ids / end_limit: the stop walks' per-sequence stop ids and length limits
+// (StopRow), nullptr for every other walk.
 struct BatchArgs {
   int B;
   int64_t ld_seq, ld_noise, ld_acc;
   const int32_t* row_base;
   const int32_t* row_step;
   const int32_t* greedy = nullptr;
+  const int32_t* stop_ids = nullptr;
+  const int32_t* end_limit = nullptr;
   template <bool BATCH>
   __device__ __forceinline__ int64_t row(int node, int b) const {
     return BATCH ? (int64_t)row_base[node] + (int64_t)b * row_step[node] : node;
@@ -70,6 +73,39 @@ __device__ __forceinline__ void finish_verify(const int32_t* sh_acc, int n_new, 
   if (prepare) {
     for (int k = 1 + threadIdx.x; k < S; k += blockDim.x) position_ids[a + k] = (int64_t)depth[k] + a;
   }
+}
+
+// Stop mode (the STOP instances behind the *_batch_stop entry points).  Sequence b's stop row is staged in shared memory
+// once, after the kernel's PDL wait: words [0, SQ_MAX_STOP) its stop ids (-1 = unused), word SQ_MAX_STOP its absolute
+// length limit E_b (<= 0 = none).  A block barrier must separate the load from stop_cut.
+__device__ __forceinline__ void stop_row_load(int32_t* sh_stop, const int32_t* __restrict__ stop_ids,
+                                              const int32_t* __restrict__ end_limit, int b) {
+  if (threadIdx.x < SQ_MAX_STOP) sh_stop[threadIdx.x] = stop_ids[b * SQ_MAX_STOP + threadIdx.x];
+  else if (threadIdx.x == SQ_MAX_STOP) sh_stop[SQ_MAX_STOP] = end_limit[b];
+}
+
+// The cut, after finish_verify, by thread 0 (which wrote the committed tokens itself).  The walk ran without an end rule,
+// so its output is tokens[P .. n), n = a + 1 when finish_verify wrote the bonus token at a, else a (NaN, or no room).
+// The first stop id at j ends the sequence at j + 1; E_b ends it when E_b <= n; the earlier end wins, the stop id on a tie.
+__device__ __forceinline__ void stop_cut(const int32_t* sh_stop, int n_new, int P, bool terminal,
+                                         const int64_t* __restrict__ tokens, int32_t* __restrict__ state,
+                                         int max_target_seq) {
+  if (threadIdx.x != 0) return;
+  const int a = P + n_new;
+  const int M = state[ST_M] > 0 ? state[ST_M] : max_target_seq;
+  const int n = (!terminal && a < M) ? a + 1 : a;           // finish_verify's bonus_ok
+  int end = 0, finish = 0;
+  for (int j = P; j < n && finish == 0; ++j) {
+    const int64_t t = tokens[j];
+#pragma unroll
+    for (int k = 0; k < SQ_MAX_STOP; ++k)
+      if (t == sh_stop[k]) finish = 1;
+    if (finish) end = j + 1;
+  }
+  const int E = sh_stop[SQ_MAX_STOP];
+  if (E > 0 && E <= n && (finish == 0 || E < end)) { end = E; finish = 2; }
+  state[ST_FINISH] = finish;
+  state[ST_END] = end;
 }
 
 }  // namespace sq

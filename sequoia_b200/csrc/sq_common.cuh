@@ -66,6 +66,8 @@ enum StateWord : int {
   ST_SKIPPED = 7,    // prepare_for_next_iter was skipped (a + 1 > max_target_seq, or the tree would overrun the buffers)
   ST_M = 8,          // length of the tokens / position_ids buffers (max_length), written by the host once per prompt
   ST_FROZEN = 9,     // batched entry points only: nonzero = finished sequence, its tokens / state / KV rows are not written
+  ST_FINISH = 10,    // *_batch_stop walks only: 1 = a stop id ended the sequence, 2 = its length limit, 0 = neither
+  ST_END = 11,       // *_batch_stop walks only: the sequence's final length when ST_FINISH != 0, else 0
   ST_WORDS = 16
 };
 

@@ -670,3 +670,51 @@ def accept_stochastic_batch_mixed(target_logits, draft_logits, row_base, row_ste
         ptr(row_step), ptr(r), ptr(noise), _rows(noise, "noise"), ptr(succ_off), ptr(succ), ptr(depth), S, V, ptr(T),
         ptr(greedy), ptr(tokens), ptr(position_ids), ld, ptr(accept_idx), _rows(accept_idx, "accept_idx"), ptr(state), B,
         max_target_seq, policy, stream_ptr()), "sq_accept_stochastic_batch_mixed")
+
+
+# ---- stop mode: per-sequence stop ids and length limits, applied by the walks (include/sequoia_b200.h) -------------------
+def _stop_args(stop_ids, end_limit, B, name):
+    if stop_ids is None or stop_ids.dtype != torch.int32 or not stop_ids.is_cuda or stop_ids.dim() != 2 \
+            or stop_ids.shape[0] < B or stop_ids.shape[1] != _lib.SQ_MAX_STOP or not stop_ids.is_contiguous():
+        raise TypeError(f"{name}: stop_ids must be a contiguous ({B}, {_lib.SQ_MAX_STOP}) int32 CUDA tensor (-1 = unused)")
+    if end_limit is None or end_limit.dtype != torch.int32 or not end_limit.is_cuda or end_limit.dim() != 1 \
+            or end_limit.shape[0] < B or end_limit.stride(0) != 1:
+        raise TypeError(f"{name}: end_limit must be a contiguous ({B},) int32 CUDA tensor (<= 0 = no limit)")
+
+
+def accept_stochastic_batch_stop(target_logits, draft_logits, row_base, row_step, r, noise, succ_off, succ, depth, S, T,
+                                 greedy, stop_ids, end_limit, tokens, position_ids, accept_idx, state, max_target_seq,
+                                 policy=0):
+    """accept_stochastic_batch_per_seq (greedy None) or accept_stochastic_batch_mixed (greedy set) without the fixed 0 / 2
+    end rule; then each walked sequence's committed tokens are cut at its stop ids (stop_ids (B, 8) int32, -1 padded) and
+    its absolute length limit (end_limit (B,) int32, <= 0 = none): state words SQ_ST_FINISH / SQ_ST_END."""
+    B = state.shape[0]
+    _seq_params("accept_stochastic_batch_stop", B, T=T)
+    if greedy is not None:
+        _greedy_arg(greedy, B, "accept_stochastic_batch_stop")
+    _stop_args(stop_ids, end_limit, B, "accept_stochastic_batch_stop")
+    V = target_logits.shape[-1]
+    ld = _rows(tokens, "tokens")
+    assert _rows(position_ids, "position_ids") == ld and _rows(r, "r") == ld
+    check(_lib.load().sq_accept_stochastic_batch_stop(
+        ptr(target_logits), target_logits.stride(0), ptr(draft_logits), draft_logits.stride(0), ptr(row_base),
+        ptr(row_step), ptr(r), ptr(noise), _rows(noise, "noise"), ptr(succ_off), ptr(succ), ptr(depth), S, V, ptr(T),
+        ptr(greedy), ptr(stop_ids), ptr(end_limit), ptr(tokens), ptr(position_ids), ld, ptr(accept_idx),
+        _rows(accept_idx, "accept_idx"), ptr(state), B, max_target_seq, policy, stream_ptr()),
+        "sq_accept_stochastic_batch_stop")
+
+
+def accept_greedy_batch_stop(target_token, succ_off, succ, depth, S, greedy, stop_ids, end_limit, tokens, position_ids,
+                             accept_idx, state, max_target_seq):
+    """accept_greedy_batch (greedy None) or accept_greedy_batch_mixed (greedy set) with the stop rule of
+    accept_stochastic_batch_stop."""
+    B = state.shape[0]
+    if greedy is not None:
+        _greedy_arg(greedy, B, "accept_greedy_batch_stop")
+    _stop_args(stop_ids, end_limit, B, "accept_greedy_batch_stop")
+    ld = _rows(tokens, "tokens")
+    assert _rows(position_ids, "position_ids") == ld
+    check(_lib.load().sq_accept_greedy_batch_stop(ptr(target_token), ptr(succ_off), ptr(succ), ptr(depth), S, ptr(tokens),
+                                                  ptr(position_ids), ld, ptr(accept_idx), _rows(accept_idx, "accept_idx"),
+                                                  ptr(state), ptr(greedy), ptr(stop_ids), ptr(end_limit), B,
+                                                  max_target_seq, stream_ptr()), "sq_accept_greedy_batch_stop")

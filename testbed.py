@@ -188,13 +188,23 @@ def simulation_baseline(target, prompts, T, top_p, M, new_tokens: int = 32, stop
     return dict(decoded_tokens=decoded, seconds=total_time, latency=total_time / max(decoded, 1))
 
 
-def decode_refill(tree, prompts, limits, stop=DEFAULT_STOP, step_times=None, seeds=None, policies=None):
+def device_stop_settings(prompts, stop):
+    """--device-stop: prompt i's (stop_tokens, max_new_tokens) lists for BatchTree / admit: the stop ids of the target's
+    config, and the budget that ends it at MAX_NEW_LEN tokens, where the host loop stops it (at least 1)."""
+    ids = sorted(stop)
+    return [ids] * len(prompts), [max(1, MAX_NEW_LEN - len(p)) for p in prompts]
+
+
+def decode_refill(tree, prompts, limits, stop=DEFAULT_STOP, step_times=None, seeds=None, policies=None,
+                  device_stop=None):
     """Decode every prompt of a queue on a BatchTree whose B slots start with prompts[:B]: each slot that finishes (a stop
     token, its length limit `limits[i]`, or out of room) takes the next prompt, until the queue is empty.
     -> (outputs, decoded tokens, per-sequence target steps, admission order); outputs[i] = prompt i's committed tokens.
     step_times: a list that receives ("steady" | "admission", seconds) per step; an admission step is timed from the
     first admit() of the step to the end of its verify.  seeds: for a seeded tree, prompt i's seed is seeds[i].
-    policies: prompt i decodes with policies[i] ("spec" / "greedy"); None keeps each slot's policy."""
+    policies: prompt i decodes with policies[i] ("spec" / "greedy"); None keeps each slot's policy.
+    device_stop: (stop_tokens, max_new_tokens) per prompt (device_stop_settings), passed to each admission; None keeps
+    each slot's."""
     B = len(tree.frozen)
     slot = list(range(B))                        # prompt index decoding in each slot (None: the queue ran out)
     length = [len(p) for p in prompts[:B]]
@@ -209,6 +219,8 @@ def decode_refill(tree, prompts, limits, stop=DEFAULT_STOP, step_times=None, see
                 kw["seed"] = seeds[slot[b]]
             if policies is not None:
                 kw["policy"] = policies[slot[b]]
+            if device_stop is not None:
+                kw["stop_tokens"], kw["max_new_tokens"] = device_stop[0][slot[b]], device_stop[1][slot[b]]
             tree.admit(b, prompts[slot[b]], **kw)
         kind = "admission" if pending else "steady"
         pending = []
@@ -262,27 +274,32 @@ def decode_chunk(tree, chunk, limits, stop=DEFAULT_STOP):
 
 @torch.inference_mode()
 def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: int, stop=DEFAULT_STOP,
-                     refill: bool = False, seeds=None, policies=None, top_k: int = 0):
+                     refill: bool = False, seeds=None, policies=None, top_k: int = 0, device_stop: bool = False):
     """--batch B: the same metric loop with B prompts decoded together (sequoia_b200.batch.BatchTree).  Chunked: B
     prompts at a time, each chunk until its last sequence stops.  refill: one batch whose finished slots take the next
     prompt (BatchTree.admit).  seeds: one per prompt (--device-rng): each sequence draws its random numbers on the device
     from its own seed.  policies: one per prompt (--policies), in place of `policy` for all.  top_k: every sampled
-    prompt's top-k filter (--top-k, 0 = off)."""
+    prompt's top-k filter (--top-k, 0 = off).  device_stop: each sequence ends on the device at the stop ids and the
+    length limit the host loop applies (--device-stop), without overshoot."""
     from sequoia_b200.batch import BatchTree
     steps = decoded = 0                          # steps: target steps summed over sequences (per-sequence tokens / step)
     total_time = 0.0
     limits = [MAX_NEW_LEN] * len(prompts)
     prompts = [p.to(DEV) for p in prompts]
     chunks = [prompts[:B]] if refill else [prompts[i:i + B] for i in range(0, len(prompts), B)]
+    dstop = device_stop_settings(prompts, stop) if device_stop else None
     for c, chunk in enumerate(chunks):
         i0 = c * B
         pol = policy if policies is None else policies[i0:i0 + len(chunk)]
+        kw = {}
+        if dstop is not None:
+            kw = dict(stop_tokens=dstop[0][i0:i0 + len(chunk)], max_new_tokens=dstop[1][i0:i0 + len(chunk)])
         tree = BatchTree(draft, target, chunk, grow_map, policy=pol, temperature=T, top_p=top_p, max_length=M,
-                         max_target_seq=M, seeds=None if seeds is None else seeds[i0:i0 + len(chunk)], top_k=top_k)
+                         max_target_seq=M, seeds=None if seeds is None else seeds[i0:i0 + len(chunk)], top_k=top_k, **kw)
         torch.cuda.synchronize()
         t1 = time.time()
         if refill:
-            _, d, s, _ = decode_refill(tree, prompts, limits, stop, seeds=seeds, policies=policies)
+            _, d, s, _ = decode_refill(tree, prompts, limits, stop, seeds=seeds, policies=policies, device_stop=dstop)
         else:
             d, s = decode_chunk(tree, chunk, limits[:len(chunk)], stop)
         decoded += d
@@ -328,6 +345,9 @@ def build_parser():
                          "policies[i %% len], greedy and sampled prompts in one batch")
     ap.add_argument("--top-k", type=int, default=0,
                     help="with --batch: keep the K best target logits of each row before top_p (0 = off)")
+    ap.add_argument("--device-stop", action="store_true",
+                    help="with --batch: each sequence ends on the device at the target's stop ids (anywhere in an "
+                         "accepted path) and at the length limit, exactly, instead of after the step")
     ap.add_argument("--target-weights", type=str, default="fp16", choices=["fp16", "fp8"],
                     help="fp8: the target's layer projections quantized to E4M3 with per-channel scales at load")
     return ap
@@ -383,6 +403,13 @@ def batch_top_k(args) -> int:
     return args.top_k
 
 
+def batch_device_stop(args) -> bool:
+    """--device-stop: refused without --batch / --refill (the lone trees keep the reference's end rule)."""
+    if args.device_stop and args.batch == 1 and not args.refill:
+        raise SystemExit("--device-stop runs with --batch (the batched tree); the lone trees keep the reference's end rule")
+    return args.device_stop
+
+
 def main(argv=None):
     args = build_parser().parse_args(argv)
     print(args)
@@ -397,6 +424,7 @@ def main(argv=None):
     seeds = device_rng_seeds(args, len(prompts))
     policies = prompt_policies(args, len(prompts))
     top_k = batch_top_k(args)
+    device_stop = batch_device_stop(args)
     if args.batch != 1 or args.refill:
         B = check_batch_args(args, len(prompts))
         target = GraphInferenceEngineTG(max_length=args.M, model_name_or_path=args.target, dtype=torch.float16,
@@ -407,7 +435,8 @@ def main(argv=None):
         grow_map = torch.load(path)
         assert args.M >= MAX_NEW_LEN + grow_map["size"], "--M must hold 256 tokens + the tree (README.md:47 of the reference)"
         res = simulation_batch(target, draft, prompts, grow_map, args.tree, args.T, args.P, args.M, B, stop=stop,
-                               refill=args.refill, seeds=seeds, policies=policies, top_k=top_k)
+                               refill=args.refill, seeds=seeds, policies=policies, top_k=top_k,
+                               device_stop=device_stop)
         print(json.dumps({k: (round(v, 5) if isinstance(v, float) else v) for k, v in res.items()}))
         return res
     target = (tcls(max_length=args.M, model_name_or_path=args.target, dtype=torch.float16, device=DEV)
