@@ -449,6 +449,28 @@ int sq_accept_greedy_batch_stop(const int64_t* target_token, const int32_t* succ
                                 int32_t* accept_idx, int64_t ld_acc, int32_t* state, const int32_t* greedy,
                                 const int32_t* stop_ids, const int32_t* end_limit, int B, int max_target_seq,
                                 void* stream);
+/* Per-sequence repetition, frequency and presence penalties (csrc/sq_penalty.cu), in place on the (B*S, V) target rows
+ * (row b*S + k = node k of sequence b, row pitch ld >= V), before any filter or walk reads them.  rep, freq, pres: (B,)
+ * fp32 device arrays (rho_b, f_b, p_b); prompt_len: (B,) int32, L_b = the length of sequence b's prompt.
+ *   Context of row k: with P = state[b][SQ_ST_P], the committed tokens[b, 0 .. P) (slot P-1 is node 0), then the tokens
+ *   at slots P-1+j of the ancestors-or-self j >= 1 of node k (the bits of row k of tree_bits).  These are the tokens the
+ *   row's logits were computed from.  c_all(t) counts t in the context, c_out(t) only at slots >= L_b (path slots count
+ *   as output).  Ids outside [0, V) are ignored.
+ *   Once for each distinct id t of the context, if x = float(logit[row, t]) is finite (inf and NaN are left alone):
+ *     c_all > 0: x = x < 0 ? x * rho : x / rho;
+ *     c_out > 0: x = x - f * c_out, then x = x - p;
+ *   each operation one IEEE fp32 round-to-nearest operation (no FMA), then x is clamped to [-65504, 65504] and rounded
+ *   to fp16, so a finite logit stays finite.
+ * A sequence with SQ_ST_FROZEN set, or with rho = 1, f = 0 and p = 0, has its rows left untouched; rows from B*S on are
+ * never touched.  scratch: caller-owned int32 of at least B * (3 * ld_seq + 1) words, rewritten by every call before it
+ * is read.  Two PDL-chained launches.  Refused with SQ_ERR_INVALID_ARG before any launch: a null array, B outside
+ * 1..SQ_MAX_BATCH, V not a multiple of 8 in 8..131072, ld < V, S < 1 or tree_words != ceil(S/32) or tree_words > 32,
+ * ld_seq outside 1..SQ_PENALTY_MAX_LEN, and a scratch too small. */
+#define SQ_PENALTY_MAX_LEN 4096
+int sq_penalize_rows_batch(sq_half* logits, int64_t ld, int V, const int64_t* tokens, int64_t ld_seq,
+                           const int32_t* state, const int32_t* prompt_len, const uint32_t* tree_bits, int tree_words,
+                           int S, const float* rep, const float* freq, const float* pres, int32_t* scratch,
+                           int64_t scratch_words, int B, void* stream);
 
 /* ---- ragged batches: a forward over a chosen set of the B sequences, each with its own row count ----
  * A part list names the sequences to run.  Part j is n rows of sequence seq in that sequence's tree-relative addressing:

@@ -19,6 +19,8 @@ _lib = None
 # stop mode (include/sequoia_b200.h): stop ids per sequence, and the state words the *_batch_stop walks write
 SQ_MAX_STOP = 8
 SQ_ST_FINISH, SQ_ST_END = 10, 11
+# per-sequence penalties: the longest token row (ld_seq) sq_penalize_rows_batch counts
+SQ_PENALTY_MAX_LEN = 4096
 
 i32, i64, f32, vp = C.c_int, C.c_int64, C.c_float, C.c_void_p
 
@@ -112,6 +114,7 @@ _SIGNATURES = {
     "sq_accept_stochastic_batch_stop": (i32, [vp, i64, vp, i64, vp, vp, vp, vp, i64, vp, vp, vp, i32, i32, vp, vp, vp, vp,
                                               vp, vp, i64, vp, i64, vp, i32, i32, i32, vp]),
     "sq_accept_greedy_batch_stop": (i32, [vp, vp, vp, vp, i32, vp, vp, i64, vp, i64, vp, vp, vp, vp, i32, i32, vp]),
+    "sq_penalize_rows_batch": (i32, [vp, i64, i32, vp, i64, vp, vp, vp, i32, i32, vp, vp, vp, vp, i64, i32, vp]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

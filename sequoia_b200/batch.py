@@ -26,11 +26,19 @@ or a token budget, and then stays on: the walks run without the fixed rule and t
 at the first of its stop ids, or at its length limit len(prompt) + max_new_tokens, on the device (state words
 SQ_ST_FINISH / SQ_ST_END).  The output is then exactly a prefix of the output without a stop rule.  finish_reason[b]
 says why slot b ended: "stop", "length", "nan" or "room" (None while it decodes).
+
+Penalties: each sequence has a repetition_penalty (1 = off), frequency_penalty and presence_penalty (0 = off), vLLM's
+parameters.  Target row k of a sequence is penalised for the context it was computed from, the committed tokens plus the
+tokens on the tree path to node k, before the greedy walk and the filters read it (sq_penalize_rows_batch; the draft is
+not penalised, speculative sampling stays exact).  While every sequence is neutral nothing is launched; the first
+non-neutral setting, at construction or admission, captures the steady and post graphs once more, and the penalty
+kernels then stay in them.
 """
 from __future__ import annotations
 
 import math
 import numbers
+import struct
 from typing import Dict, List, Optional, Sequence, Union
 
 import torch
@@ -42,6 +50,8 @@ F16 = torch.float16
 ST_P, ST_M, ST_FROZEN = 0, 8, 9
 ST_FINISH, ST_END = _lib.SQ_ST_FINISH, _lib.SQ_ST_END
 MAX_STOP = _lib.SQ_MAX_STOP
+PENALTY_MAX_LEN = _lib.SQ_PENALTY_MAX_LEN
+FP16_MAX = 65504.0
 INT32_MAX = (1 << 31) - 1
 POLICIES = ("spec", "greedy")
 _PREVIOUS = object()        # admit(): keep the slot's previous stop set / budget
@@ -178,6 +188,40 @@ def _per_seq(value, B: int, name: str) -> List[float]:
     return vals
 
 
+def _fp32(x: float) -> float:
+    return struct.unpack("f", struct.pack("f", x))[0]
+
+
+def check_penalty(name: str, value) -> float:
+    """A repetition_penalty in (0, 65504], or a frequency_penalty / presence_penalty with |value| <= 65504: a finite real
+    number (not a bool).  -> the value rounded to fp32, as the device holds it (a repetition penalty that rounds to 0 is
+    refused).  The bounds keep f * count finite, so a penalised finite logit stays finite."""
+    if isinstance(value, bool) or not isinstance(value, numbers.Real) or not math.isfinite(value):
+        raise ValueError(f"{name} must be a finite number, got {value!r}")
+    v = _fp32(float(value)) if abs(float(value)) <= FP16_MAX else float(value)
+    if name == "repetition_penalty":
+        if not 0 < v <= FP16_MAX:
+            raise ValueError(f"repetition_penalty must be in (0, 65504], got {value!r}")
+    elif not abs(v) <= FP16_MAX:
+        raise ValueError(f"{name} must be in [-65504, 65504], got {value!r}")
+    return v
+
+
+def _penalties(name: str, value, B: int) -> List[float]:
+    """One penalty for all B sequences, or a sequence of B of them."""
+    if _is_collection(value):
+        vals = [check_penalty(name, v) for v in value]
+        if len(vals) != B:
+            raise ValueError(f"{name}: {len(vals)} values for {B} sequences")
+        return vals
+    return [check_penalty(name, value)] * B
+
+
+def is_neutral(rep: float, freq: float, pres: float) -> bool:
+    """The penalties that leave a row as it is: repetition 1, frequency 0, presence 0."""
+    return rep == 1.0 and freq == 0.0 and pres == 0.0
+
+
 def check_seed(seed) -> int:
     """A per-sequence seed: an integer in [0, 2^64)."""
     if isinstance(seed, bool) or not isinstance(seed, numbers.Integral):
@@ -210,16 +254,28 @@ class BatchTree:
     prompt.  max_new_tokens: None, or an integer >= 1, for all sequences or one per prompt.  Any stop set (an empty one
     too) or budget turns on stop mode (module docstring): sequence b then ends at the first of its stop ids that it
     commits, or when it holds len(prompt) + max_new_tokens tokens, whichever comes first, and verify() returns exactly
-    the tokens up to there with terminal True.  Both policies honour them."""
+    the tokens up to there with terminal True.  Both policies honour them.
+    repetition_penalty (in (0, 65504], 1 = off), frequency_penalty and presence_penalty (|value| <= 65504, 0 = off): one
+    value for all sequences or one per prompt, vLLM's meaning (module docstring, include/sequoia_b200.h).  Both policies
+    honour them.  Penalties count at most 4096 tokens: a tree with max_length > 4096 refuses a non-neutral setting."""
 
     def __init__(self, draft, target, prompts: Sequence[torch.Tensor], grow_map: dict,
                  policy: Union[str, Sequence[str]] = "spec",
                  temperature: Union[float, Sequence[float]] = 0.6, top_p: Union[float, Sequence[float]] = 1.0,
                  max_length: int = 256, max_target_seq: Optional[int] = None,
                  seeds: Optional[Sequence[int]] = None, top_k: Union[int, Sequence[int]] = 0,
-                 stop_tokens=None, max_new_tokens: Union[None, int, Sequence[Optional[int]]] = None):
+                 stop_tokens=None, max_new_tokens: Union[None, int, Sequence[Optional[int]]] = None,
+                 repetition_penalty: Union[float, Sequence[float]] = 1.0,
+                 frequency_penalty: Union[float, Sequence[float]] = 0.0,
+                 presence_penalty: Union[float, Sequence[float]] = 0.0):
         B = len(prompts)
         policies = _policies(policy, B)
+        reps = _penalties("repetition_penalty", repetition_penalty, B)
+        freqs = _penalties("frequency_penalty", frequency_penalty, B)
+        press = _penalties("presence_penalty", presence_penalty, B)
+        use_penalty = not all(is_neutral(*v) for v in zip(reps, freqs, press))
+        if use_penalty and max_length > PENALTY_MAX_LEN:
+            raise ValueError(f"penalties count at most {PENALTY_MAX_LEN} tokens; max_length={max_length}")
         top_ks = _top_ks(top_k, B)
         stops, budgets = _stop_sets(stop_tokens, B), _budgets(max_new_tokens, B)
         temps, top_ps = _per_seq(temperature, B, "temperature"), _per_seq(top_p, B, "top_p")
@@ -276,6 +332,17 @@ class BatchTree:
         self.end_limit_dev = torch.tensor([_end_limit(len(p), n) for p, n in zip(prompts, budgets)], dtype=torch.int32,
                                           device=dev)
         self.use_stop = any(t is not None for t in stops) or any(n is not None for n in budgets)
+        # penalties: each slot's values and prompt length on the device, read by sq_penalize_rows_batch inside the
+        # captured graphs, which it joins the first time a slot has a non-neutral setting (one recapture)
+        self.repetition_penalty, self.frequency_penalty, self.presence_penalty = reps, freqs, press
+        self.rep_dev = torch.tensor(reps, dtype=torch.float32, device=dev)
+        self.freq_dev = torch.tensor(freqs, dtype=torch.float32, device=dev)
+        self.pres_dev = torch.tensor(press, dtype=torch.float32, device=dev)
+        self.prompt_len_dev = torch.tensor([len(p) for p in prompts], dtype=torch.int32, device=dev)
+        self.use_penalty = False
+        self.pen_scratch: Optional[torch.Tensor] = None
+        if use_penalty:
+            self._start_penalties()
         self.finish_reason: List[Optional[str]] = [None] * B
         i64 = dict(dtype=torch.int64, device=dev)
         self.tokens = torch.zeros(B, M, **i64)
@@ -329,6 +396,12 @@ class BatchTree:
     def _mask_kw(self):
         return dict(tree_bits=self.st.tree_bits, tree_words=self.st.tree_words, tree_size=self.S)
 
+    def _start_penalties(self):
+        """The penalty kernels join op_accept, with their scratch: a distinct-id list per sequence, rewritten every step
+        before it is read, so not one of the captured buffers."""
+        self.use_penalty = True
+        self.pen_scratch = torch.zeros(ops.penalty_scratch_words(self.B, self.M), dtype=torch.int32, device=self.device)
+
     def _load_prompt(self, b: int, prompt: torch.Tensor):
         """Row b of tokens, position ids, state and accept_idx for a new prompt: nothing of an earlier occupant stays."""
         P, S, M = len(prompt), self.S, self.M
@@ -358,7 +431,8 @@ class BatchTree:
     @torch.inference_mode()
     def admit(self, b: int, prompt: torch.Tensor, temperature: Optional[float] = None, top_p: Optional[float] = None,
               seed: Optional[int] = None, policy: Optional[str] = None, top_k: Optional[int] = None,
-              stop_tokens=_PREVIOUS, max_new_tokens=_PREVIOUS):
+              stop_tokens=_PREVIOUS, max_new_tokens=_PREVIOUS, repetition_penalty: Optional[float] = None,
+              frequency_penalty: Optional[float] = None, presence_penalty: Optional[float] = None):
         """Start `prompt` in the frozen slot b (finished, out of room, or stopped with freeze), at its own policy,
         temperature, top_p and top_k (default: the slot's previous values).  The next verify() runs its first verify next
         to the steady sequences.  The slot draws r and rand as a lone SpecTree on the prompt would, and runs its draft
@@ -371,7 +445,10 @@ class BatchTree:
         graphs once more: the top-k filter joins the accept step.
         stop_tokens / max_new_tokens: the prompt's stop set and token budget (default: the slot's previous ones; None is
         none).  The budget counts from this prompt.  The first admission that brings a stop set or a budget to a tree in
-        default mode captures the steady and post graphs once more: the stop walks replace the walks."""
+        default mode captures the steady and post graphs once more: the stop walks replace the walks.
+        repetition_penalty / frequency_penalty / presence_penalty: the prompt's penalties (default: the slot's previous
+        ones); they count this prompt and its output only.  The first non-neutral setting in a tree without one captures
+        the steady and post graphs once more."""
         if policy is not None:
             check_policy(policy)
         if top_k is not None:
@@ -380,6 +457,9 @@ class BatchTree:
             stop_tokens = check_stop_tokens(stop_tokens, self.V)
         if max_new_tokens is not _PREVIOUS:
             max_new_tokens = check_max_new_tokens(max_new_tokens)
+        pens = [None if v is None else check_penalty(name, v) for name, v in
+                (("repetition_penalty", repetition_penalty), ("frequency_penalty", frequency_penalty),
+                 ("presence_penalty", presence_penalty))]
         if not 0 <= b < self.B:
             raise IndexError(f"slot {b} out of range for a batch of {self.B}")
         if not self.frozen[b]:
@@ -400,6 +480,10 @@ class BatchTree:
         k = self.top_ks[b] if top_k is None else top_k
         stop = self.stop_tokens[b] if stop_tokens is _PREVIOUS else stop_tokens
         budget = self.max_new_tokens[b] if max_new_tokens is _PREVIOUS else max_new_tokens
+        rep, freq, pres = (old[b] if v is None else v for v, old in
+                           zip(pens, (self.repetition_penalty, self.frequency_penalty, self.presence_penalty)))
+        if not is_neutral(rep, freq, pres) and self.M > PENALTY_MAX_LEN:
+            raise ValueError(f"penalties count at most {PENALTY_MAX_LEN} tokens; this tree's max_length={self.M}")
         # (every other slot holds the tree's one policy until then, so a different one means both are present; at B = 1
         # it is a switch, which the single-policy graphs do not serve either)
         enter_mixed = not self.mixed and pol != ("greedy" if self.greedy else "spec")
@@ -426,6 +510,13 @@ class BatchTree:
         self.end_limit_dev[b] = _end_limit(P, budget)
         if (stop is not None or budget is not None) and not self.use_stop:
             self.use_stop = True                   # the stop walks replace the walks: capture steady and post once more
+            for name in ("steady", "post"):
+                self.graphs.pop(name, None)
+        self.repetition_penalty[b], self.frequency_penalty[b], self.presence_penalty[b] = rep, freq, pres
+        self.rep_dev[b], self.freq_dev[b], self.pres_dev[b] = rep, freq, pres
+        self.prompt_len_dev[b] = P
+        if not is_neutral(rep, freq, pres) and not self.use_penalty:
+            self._start_penalties()                # the penalty kernels enter op_accept: capture steady and post once more
             for name in ("steady", "post"):
                 self.graphs.pop(name, None)
         if pol == "spec" and self.r is None:       # the first sampling sequence of a tree built all-greedy
@@ -483,6 +574,9 @@ class BatchTree:
 
     def op_accept(self):
         st = self.st
+        if self.use_penalty:                       # first: the greedy walk and the filters rank the penalised rows
+            ops.penalize_rows_batch_(self.target_logits, self.tokens, self.state, self.prompt_len_dev, st.tree_bits,
+                                     st.tree_words, self.S, self.rep_dev, self.freq_dev, self.pres_dev, self.pen_scratch)
         if self.greedy:
             ops.argmax_rows(self.target_logits, self.target_token)
             if self.use_stop:

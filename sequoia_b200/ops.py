@@ -718,3 +718,41 @@ def accept_greedy_batch_stop(target_token, succ_off, succ, depth, S, greedy, sto
                                                   ptr(position_ids), ld, ptr(accept_idx), _rows(accept_idx, "accept_idx"),
                                                   ptr(state), ptr(greedy), ptr(stop_ids), ptr(end_limit), B,
                                                   max_target_seq, stream_ptr()), "sq_accept_greedy_batch_stop")
+
+
+# ---- per-sequence repetition / frequency / presence penalties (csrc/sq_penalty.cu; semantics in include/sequoia_b200.h) --
+def penalty_scratch_words(B: int, ld_seq: int) -> int:
+    """int32 words of the scratch penalize_rows_batch_ needs: a distinct-id list of ld_seq entries per sequence."""
+    return B * (3 * ld_seq + 1)
+
+
+def penalize_rows_batch_(logits, tokens, state, prompt_len, tree_bits, tree_words: int, S: int, rep, freq, pres,
+                         scratch):
+    """Apply sequence b's repetition (rep[b]), frequency (freq[b]) and presence (pres[b]) penalties in place to its S
+    target rows b*S .. b*S+S-1 of the (>= B*S, V) fp16 logits: row b*S + k counts the committed tokens[b, :P] and the tokens
+    of node k's ancestors-or-self on the tree (tree_bits), output from slot prompt_len[b] on.  rep, freq, pres: (B,) float32
+    and prompt_len: (B,) int32 on the device; tokens (B, ld_seq) int64; scratch: int32 of penalty_scratch_words(B, ld_seq).
+    Frozen sequences and sequences with rep = 1, freq = 0, pres = 0 are left untouched."""
+    _need(logits, F16, "penalize_rows_batch_")
+    if logits.dim() != 2 or logits.stride(-1) != 1:
+        raise ValueError(f"penalize_rows_batch_: logits must be (rows, V) with contiguous rows, got {tuple(logits.shape)}")
+    B = state.shape[0]
+    if logits.shape[0] < B * S:
+        raise ValueError(f"penalize_rows_batch_: {logits.shape[0]} logit rows for {B} sequences of {S}")
+    _seq_params("penalize_rows_batch_", B, rep=rep, freq=freq, pres=pres)
+    if prompt_len is None or prompt_len.dtype != torch.int32 or not prompt_len.is_cuda or prompt_len.dim() != 1 \
+            or prompt_len.shape[0] < B or prompt_len.stride(0) != 1:
+        raise TypeError(f"penalize_rows_batch_: prompt_len must be a contiguous ({B},) int32 CUDA tensor")
+    _need(tokens, torch.int64, "penalize_rows_batch_")
+    _need(state, torch.int32, "penalize_rows_batch_")
+    _need(tree_bits, torch.int32, "penalize_rows_batch_")
+    _need(scratch, torch.int32, "penalize_rows_batch_")
+    if not tree_bits.is_contiguous() or not scratch.is_contiguous() or not state.is_contiguous():
+        raise ValueError("penalize_rows_batch_: tree_bits, scratch and state must be contiguous")
+    if tokens.shape[0] < B:
+        raise ValueError(f"penalize_rows_batch_: {tokens.shape[0]} token rows for {B} sequences")
+    check(_lib.load().sq_penalize_rows_batch(ptr(logits), logits.stride(0), logits.shape[1], ptr(tokens),
+                                             _rows(tokens, "tokens"), ptr(state), ptr(prompt_len), ptr(tree_bits),
+                                             tree_words, S, ptr(rep), ptr(freq), ptr(pres), ptr(scratch), scratch.numel(),
+                                             B, stream_ptr()), "sq_penalize_rows_batch")
+    return logits

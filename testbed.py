@@ -274,13 +274,16 @@ def decode_chunk(tree, chunk, limits, stop=DEFAULT_STOP):
 
 @torch.inference_mode()
 def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: int, stop=DEFAULT_STOP,
-                     refill: bool = False, seeds=None, policies=None, top_k: int = 0, device_stop: bool = False):
+                     refill: bool = False, seeds=None, policies=None, top_k: int = 0, device_stop: bool = False,
+                     penalties=None):
     """--batch B: the same metric loop with B prompts decoded together (sequoia_b200.batch.BatchTree).  Chunked: B
     prompts at a time, each chunk until its last sequence stops.  refill: one batch whose finished slots take the next
     prompt (BatchTree.admit).  seeds: one per prompt (--device-rng): each sequence draws its random numbers on the device
     from its own seed.  policies: one per prompt (--policies), in place of `policy` for all.  top_k: every sampled
     prompt's top-k filter (--top-k, 0 = off).  device_stop: each sequence ends on the device at the stop ids and the
-    length limit the host loop applies (--device-stop), without overshoot."""
+    length limit the host loop applies (--device-stop), without overshoot.  penalties: every prompt's
+    repetition_penalty / frequency_penalty / presence_penalty keywords (--repetition-penalty ..., batch_penalties); refill
+    admissions keep them."""
     from sequoia_b200.batch import BatchTree
     steps = decoded = 0                          # steps: target steps summed over sequences (per-sequence tokens / step)
     total_time = 0.0
@@ -291,9 +294,9 @@ def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: i
     for c, chunk in enumerate(chunks):
         i0 = c * B
         pol = policy if policies is None else policies[i0:i0 + len(chunk)]
-        kw = {}
+        kw = dict(penalties or {})
         if dstop is not None:
-            kw = dict(stop_tokens=dstop[0][i0:i0 + len(chunk)], max_new_tokens=dstop[1][i0:i0 + len(chunk)])
+            kw.update(stop_tokens=dstop[0][i0:i0 + len(chunk)], max_new_tokens=dstop[1][i0:i0 + len(chunk)])
         tree = BatchTree(draft, target, chunk, grow_map, policy=pol, temperature=T, top_p=top_p, max_length=M,
                          max_target_seq=M, seeds=None if seeds is None else seeds[i0:i0 + len(chunk)], top_k=top_k, **kw)
         torch.cuda.synchronize()
@@ -348,6 +351,12 @@ def build_parser():
     ap.add_argument("--device-stop", action="store_true",
                     help="with --batch: each sequence ends on the device at the target's stop ids (anywhere in an "
                          "accepted path) and at the length limit, exactly, instead of after the step")
+    ap.add_argument("--repetition-penalty", type=float, default=1.0,
+                    help="with --batch: HF's repetition penalty of every prompt (1 = off), on the target rows")
+    ap.add_argument("--frequency-penalty", type=float, default=0.0,
+                    help="with --batch: vLLM's frequency penalty of every prompt (0 = off), on the target rows")
+    ap.add_argument("--presence-penalty", type=float, default=0.0,
+                    help="with --batch: vLLM's presence penalty of every prompt (0 = off), on the target rows")
     ap.add_argument("--target-weights", type=str, default="fp16", choices=["fp16", "fp8"],
                     help="fp8: the target's layer projections quantized to E4M3 with per-channel scales at load")
     return ap
@@ -410,6 +419,25 @@ def batch_device_stop(args) -> bool:
     return args.device_stop
 
 
+def batch_penalties(args) -> dict:
+    """--repetition-penalty / --frequency-penalty / --presence-penalty: BatchTree's keywords for every prompt ({} when all
+    are off).  Refused outside the ranges BatchTree takes, and without --batch: the lone trees keep the reference's
+    sampling."""
+    from sequoia_b200.batch import check_penalty, is_neutral
+    vals = {}
+    for name in ("repetition_penalty", "frequency_penalty", "presence_penalty"):
+        try:
+            vals[name] = check_penalty(name, getattr(args, name))
+        except ValueError as e:
+            raise SystemExit(f"--{name.replace('_', '-')}: {e}")
+    if is_neutral(*vals.values()):
+        return {}
+    if args.batch == 1 and not args.refill:
+        raise SystemExit("--repetition-penalty / --frequency-penalty / --presence-penalty run with --batch (the batched "
+                         "tree); the lone trees keep the reference's sampling")
+    return vals
+
+
 def main(argv=None):
     args = build_parser().parse_args(argv)
     print(args)
@@ -425,6 +453,7 @@ def main(argv=None):
     policies = prompt_policies(args, len(prompts))
     top_k = batch_top_k(args)
     device_stop = batch_device_stop(args)
+    penalties = batch_penalties(args)
     if args.batch != 1 or args.refill:
         B = check_batch_args(args, len(prompts))
         target = GraphInferenceEngineTG(max_length=args.M, model_name_or_path=args.target, dtype=torch.float16,
@@ -436,7 +465,7 @@ def main(argv=None):
         assert args.M >= MAX_NEW_LEN + grow_map["size"], "--M must hold 256 tokens + the tree (README.md:47 of the reference)"
         res = simulation_batch(target, draft, prompts, grow_map, args.tree, args.T, args.P, args.M, B, stop=stop,
                                refill=args.refill, seeds=seeds, policies=policies, top_k=top_k,
-                               device_stop=device_stop)
+                               device_stop=device_stop, penalties=penalties)
         print(json.dumps({k: (round(v, 5) if isinstance(v, float) else v) for k, v in res.items()}))
         return res
     target = (tcls(max_length=args.M, model_name_or_path=args.target, dtype=torch.float16, device=DEV)
