@@ -471,6 +471,33 @@ int sq_penalize_rows_batch(sq_half* logits, int64_t ld, int V, const int64_t* to
                            const int32_t* state, const int32_t* prompt_len, const uint32_t* tree_bits, int tree_words,
                            int S, const float* rep, const float* freq, const float* pres, int32_t* scratch,
                            int64_t scratch_words, int B, void* stream);
+/* Per-sequence logprobs of the committed tokens (csrc/sq_logprobs.cu), after the walk, from the (B*S, V) target rows as the
+ * walk read them (penalised, top-k and top-p filtered; row pitch ld >= V, a multiple of 8).  With P = state[b][SQ_ST_P_OLD],
+ * n_new = state[b][SQ_ST_N_NEW], a = P + n_new and M = state[b][SQ_ST_M] (ld_seq when 0), the step committed position
+ * P + j for j < n_new (the accepted tokens) and for j = n_new when !state[b][SQ_ST_TERMINAL] && a < M (the bonus token).
+ *   Row of position P + j: node 0 (row b*S) for j = 0, else node k = accept_idx[b][j-1] - (P - 1) (row b*S + k): the row
+ *   the committed token was drawn from.  Token: tokens[b][P + j] as the walk left it.  SpecTree writes the bonus at slot a
+ *   before it gathers the accepted slots, so an accepted node living at slot a (accept_idx[b][j-1] == a) is committed as
+ *   the bonus token; that position still reads its path row.
+ *   Value: s_i = fp16(float(x_i) * (1.0f / T_b)), T_b = T[b] for a sampled sequence and 1 for a greedy one (greedy[b] != 0),
+ *   the values the walk's softmax reads; the fp32 log-softmax s_t - (m + log sum_i exp(s_i - m)), m = max s.
+ *   A filtered token (-inf) has logprob -inf.  A row holding a +inf or NaN scaled value, or only -inf, gives NaN for every
+ *   value.  At T = 1 with no filter or penalty this is the model's log-probability.
+ *   Top entries: n = min(n_top[b], SQ_MAX_LOGPROBS, V) ids of the row ranked as sq_top_k_filter ranks them (raw fp16 value
+ *   descending, equal values by ascending index, -0 equal to +0, NaN above +inf, -inf last; so the ids do not depend on T)
+ *   with their logprobs, which do not increase down the list.
+ * Output at absolute positions: lp_token (B, ld_seq) fp32 [b][P + j]; lp_ids (B, ld_seq, SQ_MAX_LOGPROBS) int32 and lp_top
+ * (same shape, fp32) entries [b][P + j][0 .. n).  Nothing else is written: not a frozen sequence (SQ_ST_FROZEN), not a
+ * sequence with n_top[b] < 0 (off), not a position the step did not commit, not entries from n on.  The token of an id
+ * outside [0, V) gets NaN.  One PDL-chained launch, grid (max_depth + 1, B) of one CTA per position; no state between
+ * calls.  Refused with SQ_ERR_INVALID_ARG before any launch: a null array, B outside 1..SQ_MAX_BATCH,
+ * V not a multiple of 8 in 8..131072, ld < V or not a multiple of 8, logits not 16-byte aligned, S < 1, max_depth outside
+ * 0..S-1, ld_seq < 1, ld_acc < max_depth. */
+#define SQ_MAX_LOGPROBS 20
+int sq_token_logprobs_batch(const sq_half* logits, int64_t ld, int V, int S, int max_depth, const int64_t* tokens,
+                            int64_t ld_seq, const int32_t* state, const int32_t* accept_idx, int64_t ld_acc,
+                            const float* T, const int32_t* greedy, const int32_t* n_top, float* lp_token,
+                            int32_t* lp_ids, float* lp_top, int B, void* stream);
 
 /* ---- ragged batches: a forward over a chosen set of the B sequences, each with its own row count ----
  * A part list names the sequences to run.  Part j is n rows of sequence seq in that sequence's tree-relative addressing:

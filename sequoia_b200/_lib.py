@@ -21,6 +21,8 @@ SQ_MAX_STOP = 8
 SQ_ST_FINISH, SQ_ST_END = 10, 11
 # per-sequence penalties: the longest token row (ld_seq) sq_penalize_rows_batch counts
 SQ_PENALTY_MAX_LEN = 4096
+# per-sequence logprobs: the most top alternatives sq_token_logprobs_batch returns per position (vLLM's and OpenAI's limit)
+SQ_MAX_LOGPROBS = 20
 
 i32, i64, f32, vp = C.c_int, C.c_int64, C.c_float, C.c_void_p
 
@@ -115,6 +117,7 @@ _SIGNATURES = {
                                               vp, vp, i64, vp, i64, vp, i32, i32, i32, vp]),
     "sq_accept_greedy_batch_stop": (i32, [vp, vp, vp, vp, i32, vp, vp, i64, vp, i64, vp, vp, vp, vp, i32, i32, vp]),
     "sq_penalize_rows_batch": (i32, [vp, i64, i32, vp, i64, vp, vp, vp, i32, i32, vp, vp, vp, vp, i64, i32, vp]),
+    "sq_token_logprobs_batch": (i32, [vp, i64, i32, i32, i32, vp, i64, vp, vp, i64, vp, vp, vp, vp, vp, vp, i32, vp]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

@@ -33,6 +33,14 @@ tokens on the tree path to node k, before the greedy walk and the filters read i
 not penalised, speculative sampling stays exact).  While every sequence is neutral nothing is launched; the first
 non-neutral setting, at construction or admission, captures the steady and post graphs once more, and the penalty
 kernels then stay in them.
+
+Logprobs: each sequence has logprobs None (off) or n in 0..20, vLLM's parameter.  After the walk, inside the captured
+graphs, sq_token_logprobs_batch writes the log-probability of every token the step committed and the n best ids of its
+target row with theirs, from the rows as the walk read them (penalised, filtered) at the sequence's temperature (1 for a
+greedy sequence), into (B, M) / (B, M, 20) device buffers at absolute positions; token_logprobs(b) copies slot b's
+generated part to the host.  With T = 1 and no filter or penalty the values are the model's own log-probabilities.
+While every sequence is off nothing is allocated or launched; the first sequence with logprobs on, at construction or
+admission, captures the steady and post graphs once more.
 """
 from __future__ import annotations
 
@@ -51,10 +59,11 @@ ST_P, ST_M, ST_FROZEN = 0, 8, 9
 ST_FINISH, ST_END = _lib.SQ_ST_FINISH, _lib.SQ_ST_END
 MAX_STOP = _lib.SQ_MAX_STOP
 PENALTY_MAX_LEN = _lib.SQ_PENALTY_MAX_LEN
+MAX_LOGPROBS = _lib.SQ_MAX_LOGPROBS
 FP16_MAX = 65504.0
 INT32_MAX = (1 << 31) - 1
 POLICIES = ("spec", "greedy")
-_PREVIOUS = object()        # admit(): keep the slot's previous stop set / budget
+_PREVIOUS = object()        # admit(): keep the slot's previous stop set / budget / logprobs
 
 
 def draw_random(prompts: Sequence[torch.Tensor], M: int, S: int, V: int):
@@ -222,6 +231,25 @@ def is_neutral(rep: float, freq: float, pres: float) -> bool:
     return rep == 1.0 and freq == 0.0 and pres == 0.0
 
 
+def check_logprobs(logprobs) -> Optional[int]:
+    """A logprobs setting: None (off) or an integer in 0..20, the number of top alternatives per generated token."""
+    if logprobs is None:
+        return None
+    if isinstance(logprobs, bool) or not isinstance(logprobs, numbers.Integral) or not 0 <= logprobs <= MAX_LOGPROBS:
+        raise ValueError(f"logprobs must be None or an integer in 0..{MAX_LOGPROBS}, got {logprobs!r}")
+    return int(logprobs)
+
+
+def _logprobs(logprobs, B: int) -> List[Optional[int]]:
+    """One logprobs setting for all B sequences, or a sequence of B of them."""
+    if _is_collection(logprobs):
+        vals = [check_logprobs(n) for n in logprobs]
+        if len(vals) != B:
+            raise ValueError(f"logprobs: {len(vals)} values for {B} sequences")
+        return vals
+    return [check_logprobs(logprobs)] * B
+
+
 def check_seed(seed) -> int:
     """A per-sequence seed: an integer in [0, 2^64)."""
     if isinstance(seed, bool) or not isinstance(seed, numbers.Integral):
@@ -257,7 +285,10 @@ class BatchTree:
     the tokens up to there with terminal True.  Both policies honour them.
     repetition_penalty (in (0, 65504], 1 = off), frequency_penalty and presence_penalty (|value| <= 65504, 0 = off): one
     value for all sequences or one per prompt, vLLM's meaning (module docstring, include/sequoia_b200.h).  Both policies
-    honour them.  Penalties count at most 4096 tokens: a tree with max_length > 4096 refuses a non-neutral setting."""
+    honour them.  Penalties count at most 4096 tokens: a tree with max_length > 4096 refuses a non-neutral setting.
+    logprobs: None (off) or an integer in 0..20, for all sequences or one per prompt: token_logprobs(b) then gives the
+    log-probability of each generated token and of the n best alternatives of its row (module docstring,
+    include/sequoia_b200.h).  Both policies honour it; verify() returns what it returns without it."""
 
     def __init__(self, draft, target, prompts: Sequence[torch.Tensor], grow_map: dict,
                  policy: Union[str, Sequence[str]] = "spec",
@@ -267,9 +298,11 @@ class BatchTree:
                  stop_tokens=None, max_new_tokens: Union[None, int, Sequence[Optional[int]]] = None,
                  repetition_penalty: Union[float, Sequence[float]] = 1.0,
                  frequency_penalty: Union[float, Sequence[float]] = 0.0,
-                 presence_penalty: Union[float, Sequence[float]] = 0.0):
+                 presence_penalty: Union[float, Sequence[float]] = 0.0,
+                 logprobs: Union[None, int, Sequence[Optional[int]]] = None):
         B = len(prompts)
         policies = _policies(policy, B)
+        lps = _logprobs(logprobs, B)
         reps = _penalties("repetition_penalty", repetition_penalty, B)
         freqs = _penalties("frequency_penalty", frequency_penalty, B)
         press = _penalties("presence_penalty", presence_penalty, B)
@@ -343,6 +376,13 @@ class BatchTree:
         self.pen_scratch: Optional[torch.Tensor] = None
         if use_penalty:
             self._start_penalties()
+        # logprobs: each slot's n on the device (-1 = off), read by sq_token_logprobs_batch inside the captured graphs,
+        # which it joins the first time a slot has logprobs on (one recapture); the prompt lengths bound token_logprobs
+        self.logprobs = lps
+        self.prompt_lens = [len(p) for p in prompts]
+        self.n_top_dev = torch.tensor([-1 if n is None else n for n in lps], dtype=torch.int32, device=dev)
+        self.use_logprobs = False
+        self.lp_token = self.lp_ids = self.lp_top = None
         self.finish_reason: List[Optional[str]] = [None] * B
         i64 = dict(dtype=torch.int64, device=dev)
         self.tokens = torch.zeros(B, M, **i64)
@@ -387,6 +427,8 @@ class BatchTree:
         else:
             r, rand = draw_random(prompts, M, S, V)
             self.r, self.rand = r.to(dev), rand.to(dev)
+        if any(n is not None for n in lps):
+            self._start_logprobs()
         for b, p in enumerate(prompts):
             self._load_prompt(b, p)
         with torch.inference_mode():
@@ -401,6 +443,15 @@ class BatchTree:
         before it is read, so not one of the captured buffers."""
         self.use_penalty = True
         self.pen_scratch = torch.zeros(ops.penalty_scratch_words(self.B, self.M), dtype=torch.int32, device=self.device)
+
+    def _start_logprobs(self):
+        """The logprobs kernel joins seq_post, with its (B, M) / (B, M, 20) output buffers (a position is written by the
+        step that commits it)."""
+        self.use_logprobs = True
+        B, M, dev = self.B, self.M, self.device
+        self.lp_token = torch.full((B, M), float("nan"), dtype=torch.float32, device=dev)
+        self.lp_ids = torch.full((B, M, MAX_LOGPROBS), -1, dtype=torch.int32, device=dev)
+        self.lp_top = torch.full((B, M, MAX_LOGPROBS), float("nan"), dtype=torch.float32, device=dev)
 
     def _load_prompt(self, b: int, prompt: torch.Tensor):
         """Row b of tokens, position ids, state and accept_idx for a new prompt: nothing of an earlier occupant stays."""
@@ -432,7 +483,8 @@ class BatchTree:
     def admit(self, b: int, prompt: torch.Tensor, temperature: Optional[float] = None, top_p: Optional[float] = None,
               seed: Optional[int] = None, policy: Optional[str] = None, top_k: Optional[int] = None,
               stop_tokens=_PREVIOUS, max_new_tokens=_PREVIOUS, repetition_penalty: Optional[float] = None,
-              frequency_penalty: Optional[float] = None, presence_penalty: Optional[float] = None):
+              frequency_penalty: Optional[float] = None, presence_penalty: Optional[float] = None,
+              logprobs=_PREVIOUS):
         """Start `prompt` in the frozen slot b (finished, out of room, or stopped with freeze), at its own policy,
         temperature, top_p and top_k (default: the slot's previous values).  The next verify() runs its first verify next
         to the steady sequences.  The slot draws r and rand as a lone SpecTree on the prompt would, and runs its draft
@@ -448,7 +500,9 @@ class BatchTree:
         default mode captures the steady and post graphs once more: the stop walks replace the walks.
         repetition_penalty / frequency_penalty / presence_penalty: the prompt's penalties (default: the slot's previous
         ones); they count this prompt and its output only.  The first non-neutral setting in a tree without one captures
-        the steady and post graphs once more."""
+        the steady and post graphs once more.
+        logprobs: the prompt's logprobs setting (default: the slot's previous one; None is off).  The first one that is
+        on, in a tree without one, captures the steady and post graphs once more."""
         if policy is not None:
             check_policy(policy)
         if top_k is not None:
@@ -460,6 +514,8 @@ class BatchTree:
         pens = [None if v is None else check_penalty(name, v) for name, v in
                 (("repetition_penalty", repetition_penalty), ("frequency_penalty", frequency_penalty),
                  ("presence_penalty", presence_penalty))]
+        if logprobs is not _PREVIOUS:
+            logprobs = check_logprobs(logprobs)
         if not 0 <= b < self.B:
             raise IndexError(f"slot {b} out of range for a batch of {self.B}")
         if not self.frozen[b]:
@@ -517,6 +573,14 @@ class BatchTree:
         self.prompt_len_dev[b] = P
         if not is_neutral(rep, freq, pres) and not self.use_penalty:
             self._start_penalties()                # the penalty kernels enter op_accept: capture steady and post once more
+            for name in ("steady", "post"):
+                self.graphs.pop(name, None)
+        n_lp = self.logprobs[b] if logprobs is _PREVIOUS else logprobs
+        self.logprobs[b] = n_lp
+        self.n_top_dev[b] = -1 if n_lp is None else n_lp
+        self.prompt_lens[b] = P
+        if n_lp is not None and not self.use_logprobs:
+            self._start_logprobs()                 # the logprobs kernel enters seq_post: capture steady and post once more
             for name in ("steady", "post"):
                 self.graphs.pop(name, None)
         if pol == "spec" and self.r is None:       # the first sampling sequence of a tree built all-greedy
@@ -638,8 +702,14 @@ class BatchTree:
             self.op_sample(i)
             self.op_draft_level(i)
 
+    def op_logprobs(self):
+        ops.token_logprobs_batch_(self.target_logits, self.S, self.st.max_depth, self.tokens, self.state, self.accept_idx,
+                                  self.T_dev, self.greedy_dev, self.n_top_dev, self.lp_token, self.lp_ids, self.lp_top)
+
     def seq_post(self):
         self.op_accept()
+        if self.use_logprobs:                      # the rows as the walk read them, before anything else writes them
+            self.op_logprobs()
         self.op_kv_gather()
         self.op_bonus_forward()
         self.host_state.copy_(self.state, non_blocking=True)
@@ -682,6 +752,8 @@ class BatchTree:
         """The device buffers a graph's warm-up run writes (the noise counters of a seeded tree included, so that a
         sequence's noise does not depend on when the graphs were captured)."""
         bufs = [self.tokens, self.position_ids, self.state, self.draft_logits, self.target_logits, self.noise]
+        if self.use_logprobs:
+            bufs += [self.lp_token, self.lp_ids, self.lp_top]
         return bufs + [self.steps] if self.seeded else bufs
 
     def _snapshot(self):
@@ -753,3 +825,19 @@ class BatchTree:
                 self.freeze(b)
             out.append(self.last[b])
         return out
+
+    def token_logprobs(self, b: int):
+        """Slot b's generated tokens so far (positions len(prompt) .. len(its last verify() tokens)), on the host:
+        -> (token_lp (n,) float32, top_ids (n, k) int64, top_lp (n, k) float32), k = the slot's logprobs setting (at most
+        V).  token_lp[i] is the log-probability of generated token i, top_ids[i] / top_lp[i] the k best ids of its row,
+        best first, and theirs.  Refused for a slot whose logprobs are off."""
+        if not 0 <= b < self.B:
+            raise IndexError(f"slot {b} out of range for a batch of {self.B}")
+        n_lp = self.logprobs[b]
+        if n_lp is None:
+            raise ValueError(f"slot {b} has logprobs off (logprobs=None)")
+        L = self.prompt_lens[b]
+        end = L if self.last[b] is None else max(L, len(self.last[b][0]))
+        k = min(n_lp, self.V)
+        return (self.lp_token[b, L:end].cpu(), self.lp_ids[b, L:end, :k].cpu().to(torch.int64),
+                self.lp_top[b, L:end, :k].cpu())

@@ -154,6 +154,20 @@ __device__ __forceinline__ float h2f(__half h) { return __half2float(h); }
 __device__ __forceinline__ __half f2h(float f) { return __float2half_rn(f); }
 __device__ __forceinline__ float rnd16(float f) { return __half2float(__float2half_rn(f)); }
 
+// fp16 bits -> uint16 whose unsigned order equals the float order (-inf lowest, +inf highest)
+__device__ __forceinline__ uint32_t ord16(__half h) {
+  const uint32_t b = __half_as_ushort(h);
+  return (b & 0x8000u) ? (~b & 0xFFFFu) : (b | 0x8000u);
+}
+
+// ord16 with the order torch.sort gives fp16 values: -0 equal to +0, NaN above +inf (the top-k filter's and the logprobs'
+// ranking key)
+__device__ __forceinline__ uint32_t topk_key(__half h) {
+  const uint32_t b = __half_as_ushort(h);
+  if ((b & 0x7FFFu) > 0x7C00u) return 0xFFFFu;
+  return b == 0x8000u ? 0x8000u : ord16(h);
+}
+
 union Pack8 {
   uint4 u;
   __half h[8];

@@ -76,12 +76,6 @@ __device__ __forceinline__ int64_t wide_index(uint64_t k) {
   return (int64_t)rank * SLICE + (int64_t)(0xFFFFu - (uint32_t)(k & 0xFFFFu));
 }
 
-// fp16 bits -> uint16 whose unsigned order equals the float order (-inf lowest, +inf highest)
-__device__ __forceinline__ uint32_t ord16(__half h) {
-  const uint32_t b = __half_as_ushort(h);
-  return (b & 0x8000u) ? (~b & 0xFFFFu) : (b | 0x8000u);
-}
-
 __device__ __forceinline__ uint32_t block_max_u32(uint32_t v, uint32_t* red) {
   v = __reduce_max_sync(0xffffffffu, v);
   const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
@@ -761,13 +755,6 @@ __global__ void __launch_bounds__(NT) top_p_filter_kernel(__half* __restrict__ l
 // left untouched (the whole cluster reads the same k).  Otherwise `top_k` is the scalar k, 0 < k < V.
 template <bool PER_SEQ>
 using SeqInt = typename std::conditional<PER_SEQ, const int32_t*, int>::type;
-
-// ord16 with the order torch.sort gives fp16 values: -0 equal to +0, NaN above +inf
-__device__ __forceinline__ uint32_t topk_key(__half h) {
-  const uint32_t b = __half_as_ushort(h);
-  if ((b & 0x7FFFu) > 0x7C00u) return 0xFFFFu;
-  return b == 0x8000u ? 0x8000u : ord16(h);
-}
 
 template <bool WIDE, bool PER_SEQ = false>
 __global__ void __launch_bounds__(NT) top_k_filter_kernel(__half* __restrict__ logits, int64_t ld, int V,

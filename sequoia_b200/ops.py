@@ -756,3 +756,44 @@ def penalize_rows_batch_(logits, tokens, state, prompt_len, tree_bits, tree_word
                                              tree_words, S, ptr(rep), ptr(freq), ptr(pres), ptr(scratch), scratch.numel(),
                                              B, stream_ptr()), "sq_penalize_rows_batch")
     return logits
+
+
+# ---- per-sequence logprobs of the committed tokens (csrc/sq_logprobs.cu; semantics in include/sequoia_b200.h) -----------
+def token_logprobs_batch_(target_logits, S: int, max_depth: int, tokens, state, accept_idx, T, greedy, n_top, lp_token,
+                          lp_ids, lp_top):
+    """After the walk: for each sequence b with n_top[b] >= 0 that is not frozen, the logprob of every token the step
+    committed (positions state[b, P_OLD] + j, j <= the path depth, the bonus included) into lp_token[b, pos], and the
+    min(n_top[b], 20) best ids of its target row with their logprobs into lp_ids / lp_top[b, pos, :n].  target_logits:
+    (>= B*S, V) fp16 as the walk read it (row b*S + k = node k of sequence b); T: (B,) float32, greedy / n_top: (B,) int32
+    on the device; tokens: (B, M) int64; accept_idx: (B, >= max_depth) int32; lp_token: (B, M) float32; lp_ids: (B, M, 20)
+    int32; lp_top: (B, M, 20) float32.  Nothing else of the outputs is written."""
+    name = "token_logprobs_batch_"
+    _need(target_logits, F16, name)
+    if target_logits.dim() != 2 or target_logits.stride(-1) != 1:
+        raise ValueError(f"{name}: target_logits must be (rows, V) with contiguous rows, got {tuple(target_logits.shape)}")
+    _need(tokens, torch.int64, name)
+    _need(state, torch.int32, name)
+    _need(accept_idx, torch.int32, name)
+    if not state.is_contiguous():
+        raise ValueError(f"{name}: state must be contiguous")
+    B = state.shape[0]
+    if target_logits.shape[0] < B * S:
+        raise ValueError(f"{name}: {target_logits.shape[0]} logit rows for {B} sequences of {S}")
+    _seq_params(name, B, T=T)
+    for k, t in (("greedy", greedy), ("n_top", n_top)):
+        if t is None or t.dtype != torch.int32 or not t.is_cuda or t.dim() != 1 or t.shape[0] < B or t.stride(0) != 1:
+            raise TypeError(f"{name}: {k} must be a contiguous ({B},) int32 CUDA tensor")
+    M = tokens.shape[1] if tokens.dim() == 2 else -1
+    if tokens.dim() != 2 or tokens.shape[0] < B or accept_idx.dim() != 2 or accept_idx.shape[0] < B:
+        raise ValueError(f"{name}: tokens and accept_idx must be (B, ...) with B = {B}")
+    for k, t, dt, shape in (("lp_token", lp_token, torch.float32, (B, M)),
+                            ("lp_ids", lp_ids, torch.int32, (B, M, _lib.SQ_MAX_LOGPROBS)),
+                            ("lp_top", lp_top, torch.float32, (B, M, _lib.SQ_MAX_LOGPROBS))):
+        _need(t, dt, name)
+        if tuple(t.shape) != shape or not t.is_contiguous():
+            raise ValueError(f"{name}: {k} must be a contiguous {shape} tensor, got {tuple(t.shape)}")
+    check(_lib.load().sq_token_logprobs_batch(ptr(target_logits), target_logits.stride(0), target_logits.shape[1], S,
+                                              max_depth, ptr(tokens), _rows(tokens, "tokens"), ptr(state), ptr(accept_idx),
+                                              _rows(accept_idx, "accept_idx"), ptr(T), ptr(greedy), ptr(n_top),
+                                              ptr(lp_token), ptr(lp_ids), ptr(lp_top), B, stream_ptr()),
+          "sq_token_logprobs_batch")

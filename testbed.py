@@ -195,8 +195,15 @@ def device_stop_settings(prompts, stop):
     return [ids] * len(prompts), [max(1, MAX_NEW_LEN - len(p)) for p in prompts]
 
 
+def _record_logprobs(tree, b: int, i: int, means):
+    """means[i] = the mean logprob of the tokens slot b generated for prompt i (a tree with logprobs; means None: off)."""
+    if means is not None:
+        lp = tree.token_logprobs(b)[0]
+        means[i] = float(lp.double().mean()) if len(lp) else float("nan")
+
+
 def decode_refill(tree, prompts, limits, stop=DEFAULT_STOP, step_times=None, seeds=None, policies=None,
-                  device_stop=None):
+                  device_stop=None, logprob_means=None):
     """Decode every prompt of a queue on a BatchTree whose B slots start with prompts[:B]: each slot that finishes (a stop
     token, its length limit `limits[i]`, or out of room) takes the next prompt, until the queue is empty.
     -> (outputs, decoded tokens, per-sequence target steps, admission order); outputs[i] = prompt i's committed tokens.
@@ -204,7 +211,7 @@ def decode_refill(tree, prompts, limits, stop=DEFAULT_STOP, step_times=None, see
     first admit() of the step to the end of its verify.  seeds: for a seeded tree, prompt i's seed is seeds[i].
     policies: prompt i decodes with policies[i] ("spec" / "greedy"); None keeps each slot's policy.
     device_stop: (stop_tokens, max_new_tokens) per prompt (device_stop_settings), passed to each admission; None keeps
-    each slot's."""
+    each slot's.  logprob_means: a list that receives prompt i's mean token logprob at index i (--logprobs)."""
     B = len(tree.frozen)
     slot = list(range(B))                        # prompt index decoding in each slot (None: the queue ran out)
     length = [len(p) for p in prompts[:B]]
@@ -239,6 +246,7 @@ def decode_refill(tree, prompts, limits, stop=DEFAULT_STOP, step_times=None, see
             # tree.frozen[b] without `terminate`: the tree stopped the slot itself (no room for another tree)
             if terminate or tree.frozen[b] or last in stop or length[b] >= limits[i]:
                 outputs[i] = valid.clone()           # the slot's token row is reused by the next prompt
+                _record_logprobs(tree, b, i, logprob_means)
                 if not tree.frozen[b]:
                     tree.freeze(b)
                 if nxt < len(prompts):
@@ -251,8 +259,9 @@ def decode_refill(tree, prompts, limits, stop=DEFAULT_STOP, step_times=None, see
     return outputs, decoded, steps, order
 
 
-def decode_chunk(tree, chunk, limits, stop=DEFAULT_STOP):
-    """Decode a BatchTree built on `chunk` until every sequence has finished.  -> (decoded tokens, per-sequence steps)"""
+def decode_chunk(tree, chunk, limits, stop=DEFAULT_STOP, logprob_means=None, i0: int = 0):
+    """Decode a BatchTree built on `chunk` until every sequence has finished.  -> (decoded tokens, per-sequence steps)
+    logprob_means: a list that receives the mean token logprob of chunk[b] at index i0 + b (--logprobs)."""
     length = [len(p) for p in chunk]
     done = set()
     decoded = steps = 0
@@ -267,6 +276,7 @@ def decode_chunk(tree, chunk, limits, stop=DEFAULT_STOP):
             last = int(valid[-1]) if valid.shape[0] else 0
             if terminate or tree.frozen[b] or last in stop or length[b] >= limits[b]:
                 done.add(b)
+                _record_logprobs(tree, b, i0 + b, logprob_means)
                 if not tree.frozen[b]:
                     tree.freeze(b)
     return decoded, steps
@@ -275,7 +285,7 @@ def decode_chunk(tree, chunk, limits, stop=DEFAULT_STOP):
 @torch.inference_mode()
 def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: int, stop=DEFAULT_STOP,
                      refill: bool = False, seeds=None, policies=None, top_k: int = 0, device_stop: bool = False,
-                     penalties=None):
+                     penalties=None, logprobs=None):
     """--batch B: the same metric loop with B prompts decoded together (sequoia_b200.batch.BatchTree).  Chunked: B
     prompts at a time, each chunk until its last sequence stops.  refill: one batch whose finished slots take the next
     prompt (BatchTree.admit).  seeds: one per prompt (--device-rng): each sequence draws its random numbers on the device
@@ -283,7 +293,8 @@ def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: i
     prompt's top-k filter (--top-k, 0 = off).  device_stop: each sequence ends on the device at the stop ids and the
     length limit the host loop applies (--device-stop), without overshoot.  penalties: every prompt's
     repetition_penalty / frequency_penalty / presence_penalty keywords (--repetition-penalty ..., batch_penalties); refill
-    admissions keep them."""
+    admissions keep them.  logprobs: every prompt's logprobs setting (--logprobs, None = off); the mean logprob of each
+    prompt's generated tokens is printed and returned."""
     from sequoia_b200.batch import BatchTree
     steps = decoded = 0                          # steps: target steps summed over sequences (per-sequence tokens / step)
     total_time = 0.0
@@ -291,10 +302,13 @@ def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: i
     prompts = [p.to(DEV) for p in prompts]
     chunks = [prompts[:B]] if refill else [prompts[i:i + B] for i in range(0, len(prompts), B)]
     dstop = device_stop_settings(prompts, stop) if device_stop else None
+    means = None if logprobs is None else [float("nan")] * len(prompts)
     for c, chunk in enumerate(chunks):
         i0 = c * B
         pol = policy if policies is None else policies[i0:i0 + len(chunk)]
         kw = dict(penalties or {})
+        if logprobs is not None:
+            kw["logprobs"] = logprobs
         if dstop is not None:
             kw.update(stop_tokens=dstop[0][i0:i0 + len(chunk)], max_new_tokens=dstop[1][i0:i0 + len(chunk)])
         tree = BatchTree(draft, target, chunk, grow_map, policy=pol, temperature=T, top_p=top_p, max_length=M,
@@ -302,9 +316,10 @@ def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: i
         torch.cuda.synchronize()
         t1 = time.time()
         if refill:
-            _, d, s, _ = decode_refill(tree, prompts, limits, stop, seeds=seeds, policies=policies, device_stop=dstop)
+            _, d, s, _ = decode_refill(tree, prompts, limits, stop, seeds=seeds, policies=policies, device_stop=dstop,
+                                       logprob_means=means)
         else:
-            d, s = decode_chunk(tree, chunk, limits[:len(chunk)], stop)
+            d, s = decode_chunk(tree, chunk, limits[:len(chunk)], stop, logprob_means=means, i0=i0)
         decoded += d
         steps += s
         torch.cuda.synchronize()
@@ -316,8 +331,13 @@ def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: i
         total_time, total_time / max(decoded, 1), decoded, steps, decoded / steps))
     print("batch {}{}: aggregate {:.2f} tokens/s".format(B, " (refill)" if refill else "",
                                                          decoded / total_time if total_time > 0 else 0.0))
-    return dict(decoded_tokens=decoded, target_steps=steps, tokens_per_step=decoded / steps, seconds=total_time,
-                tokens_per_second=decoded / total_time if total_time > 0 else 0.0, batch=B, refill=refill)
+    res = dict(decoded_tokens=decoded, target_steps=steps, tokens_per_step=decoded / steps, seconds=total_time,
+               tokens_per_second=decoded / total_time if total_time > 0 else 0.0, batch=B, refill=refill)
+    if means is not None:
+        for i, m in enumerate(means):
+            print(f"prompt {i}: mean token logprob {m:.4f}")
+        res["mean_token_logprob"] = means
+    return res
 
 
 def build_parser():
@@ -357,6 +377,8 @@ def build_parser():
                     help="with --batch: vLLM's frequency penalty of every prompt (0 = off), on the target rows")
     ap.add_argument("--presence-penalty", type=float, default=0.0,
                     help="with --batch: vLLM's presence penalty of every prompt (0 = off), on the target rows")
+    ap.add_argument("--logprobs", type=int, default=None,
+                    help="with --batch: the top alternatives per token (0..20); prints each prompt's mean token logprob")
     ap.add_argument("--target-weights", type=str, default="fp16", choices=["fp16", "fp8"],
                     help="fp8: the target's layer projections quantized to E4M3 with per-channel scales at load")
     return ap
@@ -438,6 +460,21 @@ def batch_penalties(args) -> dict:
     return vals
 
 
+def batch_logprobs(args):
+    """--logprobs N: every prompt's logprobs setting (None = off).  Refused outside 0..20, and without --batch: the lone
+    trees compute no logprobs."""
+    if args.logprobs is None:
+        return None
+    from sequoia_b200.batch import check_logprobs
+    try:
+        n = check_logprobs(args.logprobs)
+    except ValueError as e:
+        raise SystemExit(f"--logprobs: {e}")
+    if args.batch == 1 and not args.refill:
+        raise SystemExit("--logprobs runs with --batch (the batched tree); the lone trees compute no logprobs")
+    return n
+
+
 def main(argv=None):
     args = build_parser().parse_args(argv)
     print(args)
@@ -454,6 +491,7 @@ def main(argv=None):
     top_k = batch_top_k(args)
     device_stop = batch_device_stop(args)
     penalties = batch_penalties(args)
+    logprobs = batch_logprobs(args)
     if args.batch != 1 or args.refill:
         B = check_batch_args(args, len(prompts))
         target = GraphInferenceEngineTG(max_length=args.M, model_name_or_path=args.target, dtype=torch.float16,
@@ -465,7 +503,7 @@ def main(argv=None):
         assert args.M >= MAX_NEW_LEN + grow_map["size"], "--M must hold 256 tokens + the tree (README.md:47 of the reference)"
         res = simulation_batch(target, draft, prompts, grow_map, args.tree, args.T, args.P, args.M, B, stop=stop,
                                refill=args.refill, seeds=seeds, policies=policies, top_k=top_k,
-                               device_stop=device_stop, penalties=penalties)
+                               device_stop=device_stop, penalties=penalties, logprobs=logprobs)
         print(json.dumps({k: (round(v, 5) if isinstance(v, float) else v) for k, v in res.items()}))
         return res
     target = (tcls(max_length=args.M, model_name_or_path=args.target, dtype=torch.float16, device=DEV)
