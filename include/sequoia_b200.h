@@ -471,6 +471,26 @@ int sq_penalize_rows_batch(sq_half* logits, int64_t ld, int V, const int64_t* to
                            const int32_t* state, const int32_t* prompt_len, const uint32_t* tree_bits, int tree_words,
                            int S, const float* rep, const float* freq, const float* pres, int32_t* scratch,
                            int64_t scratch_words, int B, void* stream);
+/* Per-sequence allowed-token mask and logit bias (csrc/sq_logit_bias.cu), in place on the (B*S, V) target rows (row b*S + k
+ * = node k of sequence b, row pitch ld >= V), before the penalties, the walks and the filters read them.  The rule does not
+ * depend on the tree: every row of sequence b is processed alike.
+ *   allowed: (B, allowed_words) bitmask, id t allowed for sequence b when bit (t & 31) of word [b][t >> 5] is set
+ *   (allowed_words >= ceil(V/32); bits from V on are not read); has_mask: (B,) int32, nonzero = sequence b has an allowed
+ *   set.  bias_ids / bias_vals: (B, SQ_MAX_LOGIT_BIAS) int32 / fp32, the first n = min(n_bias[b], SQ_MAX_LOGIT_BIAS)
+ *   entries of row b with ids in ascending order; ids outside [0, V) are skipped.
+ *   1. Mask: when has_mask[b], every entry of the rows whose id is not allowed becomes -inf (0xFC00), NaN and +inf
+ *      included; allowed entries are not touched.
+ *   2. Bias: for each entry (t, beta) in order, if t is allowed (or there is no mask) and x = float(logit[row, t]) is
+ *      finite, the logit becomes fp16(clamp(x + beta, -65504, 65504)), the add one IEEE fp32 round-to-nearest operation.
+ *      Non-finite logits are left alone.
+ * A sequence with SQ_ST_FROZEN set, or with no mask and n_bias <= 0, has its rows left byte-identical; rows from B*S on
+ * are never touched.  One PDL-chained launch, grid (ceil(V/4096), S, B); no state, no scratch.  Refused with
+ * SQ_ERR_INVALID_ARG before any launch: a null array, B outside 1..SQ_MAX_BATCH, V not a multiple of 8 in 8..131072,
+ * ld < V, S < 1, allowed_words < ceil(V/32). */
+#define SQ_MAX_LOGIT_BIAS 1024
+int sq_logit_bias_rows_batch(sq_half* logits, int64_t ld, int V, int S, const int32_t* state, const uint32_t* allowed,
+                             int64_t allowed_words, const int32_t* has_mask, const int32_t* bias_ids,
+                             const float* bias_vals, const int32_t* n_bias, int B, void* stream);
 /* Per-sequence logprobs of the committed tokens (csrc/sq_logprobs.cu), after the walk, from the (B*S, V) target rows as the
  * walk read them (penalised, top-k and top-p filtered; row pitch ld >= V, a multiple of 8).  With P = state[b][SQ_ST_P_OLD],
  * n_new = state[b][SQ_ST_N_NEW], a = P + n_new and M = state[b][SQ_ST_M] (ld_seq when 0), the step committed position
@@ -482,7 +502,7 @@ int sq_penalize_rows_batch(sq_half* logits, int64_t ld, int V, const int64_t* to
  *   Value: s_i = fp16(float(x_i) * (1.0f / T_b)), T_b = T[b] for a sampled sequence and 1 for a greedy one (greedy[b] != 0),
  *   the values the walk's softmax reads; the fp32 log-softmax s_t - (m + log sum_i exp(s_i - m)), m = max s.
  *   A filtered token (-inf) has logprob -inf.  A row holding a +inf or NaN scaled value, or only -inf, gives NaN for every
- *   value.  At T = 1 with no filter or penalty this is the model's log-probability.
+ *   value.  At T = 1 with no filter, penalty, logit bias or allowed set this is the model's log-probability.
  *   Top entries: n = min(n_top[b], SQ_MAX_LOGPROBS, V) ids of the row ranked as sq_top_k_filter ranks them (raw fp16 value
  *   descending, equal values by ascending index, -0 equal to +0, NaN above +inf, -inf last; so the ids do not depend on T)
  *   with their logprobs, which do not increase down the list.

@@ -23,6 +23,8 @@ SQ_ST_FINISH, SQ_ST_END = 10, 11
 SQ_PENALTY_MAX_LEN = 4096
 # per-sequence logprobs: the most top alternatives sq_token_logprobs_batch returns per position (vLLM's and OpenAI's limit)
 SQ_MAX_LOGPROBS = 20
+# per-sequence logit bias: the most (id, bias) entries sq_logit_bias_rows_batch holds per sequence
+SQ_MAX_LOGIT_BIAS = 1024
 
 i32, i64, f32, vp = C.c_int, C.c_int64, C.c_float, C.c_void_p
 
@@ -118,6 +120,7 @@ _SIGNATURES = {
     "sq_accept_greedy_batch_stop": (i32, [vp, vp, vp, vp, i32, vp, vp, i64, vp, i64, vp, vp, vp, vp, i32, i32, vp]),
     "sq_penalize_rows_batch": (i32, [vp, i64, i32, vp, i64, vp, vp, vp, i32, i32, vp, vp, vp, vp, i64, i32, vp]),
     "sq_token_logprobs_batch": (i32, [vp, i64, i32, i32, i32, vp, i64, vp, vp, i64, vp, vp, vp, vp, vp, vp, i32, vp]),
+    "sq_logit_bias_rows_batch": (i32, [vp, i64, i32, i32, vp, vp, i64, vp, vp, vp, vp, i32, vp]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

@@ -38,16 +38,24 @@ Logprobs: each sequence has logprobs None (off) or n in 0..20, vLLM's parameter.
 graphs, sq_token_logprobs_batch writes the log-probability of every token the step committed and the n best ids of its
 target row with theirs, from the rows as the walk read them (penalised, filtered) at the sequence's temperature (1 for a
 greedy sequence), into (B, M) / (B, M, 20) device buffers at absolute positions; token_logprobs(b) copies slot b's
-generated part to the host.  With T = 1 and no filter or penalty the values are the model's own log-probabilities.
-While every sequence is off nothing is allocated or launched; the first sequence with logprobs on, at construction or
-admission, captures the steady and post graphs once more.
+generated part to the host.  With T = 1 and no filter, penalty, logit bias or allowed set the values are the model's own
+log-probabilities.  While every sequence is off nothing is allocated or launched; the first sequence with logprobs on, at
+construction or admission, captures the steady and post graphs once more.
+
+Logit bias and allowed tokens: each sequence has a logit_bias {id: bias} and an allowed_token_ids set, vLLM's parameters.
+Every target row of the sequence is processed alike, first of all in the accept step (sq_logit_bias_rows_batch): ids
+outside the allowed set become -inf, then each bias is added to its finite logit; the penalties, the greedy walk and the
+filters then read the processed rows (the draft is not processed, speculative sampling stays exact).  A stop id outside
+the allowed set can never be generated, so it never ends the sequence.  While every sequence is neutral (no bias entries,
+no allowed set) nothing is allocated or launched; the first non-neutral setting, at construction or admission, captures
+the steady and post graphs once more, and the kernel then stays in them.
 """
 from __future__ import annotations
 
 import math
 import numbers
 import struct
-from typing import Dict, List, Optional, Sequence, Union
+from typing import Dict, List, Mapping, Optional, Sequence, Union
 
 import torch
 
@@ -60,10 +68,12 @@ ST_FINISH, ST_END = _lib.SQ_ST_FINISH, _lib.SQ_ST_END
 MAX_STOP = _lib.SQ_MAX_STOP
 PENALTY_MAX_LEN = _lib.SQ_PENALTY_MAX_LEN
 MAX_LOGPROBS = _lib.SQ_MAX_LOGPROBS
+MAX_LOGIT_BIAS = _lib.SQ_MAX_LOGIT_BIAS
+LOGIT_BIAS_MAX = 100.0
 FP16_MAX = 65504.0
 INT32_MAX = (1 << 31) - 1
 POLICIES = ("spec", "greedy")
-_PREVIOUS = object()        # admit(): keep the slot's previous stop set / budget / logprobs
+_PREVIOUS = object()        # admit(): keep the slot's previous stop set / budget / logprobs / logit bias / allowed set
 
 
 def draw_random(prompts: Sequence[torch.Tensor], M: int, S: int, V: int):
@@ -250,6 +260,78 @@ def _logprobs(logprobs, B: int) -> List[Optional[int]]:
     return [check_logprobs(logprobs)] * B
 
 
+def check_logit_bias(logit_bias, V: Optional[int] = None) -> Optional[tuple]:
+    """A logit bias: None, or a mapping {id: bias} of at most MAX_LOGIT_BIAS entries, each id an integer in [0, V) (the
+    upper bound is checked once V is given) and each bias a finite real number in [-100, 100] (not a bool).  -> None, or
+    the sorted tuple of (id, bias rounded to fp32, as the device holds it) without the entries whose bias is 0 (so {} and
+    {5: 0.0} are both neutral: ())."""
+    if logit_bias is None:
+        return None
+    if not isinstance(logit_bias, Mapping):
+        raise ValueError(f"logit_bias must be None or a mapping {{token id: bias}}, got {logit_bias!r}")
+    out = []
+    for t, v in logit_bias.items():
+        if isinstance(t, bool) or not isinstance(t, numbers.Integral) or t < 0 or (V is not None and t >= V):
+            raise ValueError(f"logit_bias: {t!r} is not a token id in [0, {V if V is not None else 'V'})")
+        if isinstance(v, bool) or not isinstance(v, numbers.Real) or not math.isfinite(v) \
+                or not abs(float(v)) <= LOGIT_BIAS_MAX:
+            raise ValueError(f"logit_bias: the bias of {int(t)} must be a finite number in [-100, 100], got {v!r}")
+        v = _fp32(float(v))
+        if v != 0.0:
+            out.append((int(t), v))
+    if len(out) > MAX_LOGIT_BIAS:
+        raise ValueError(f"logit_bias: {len(out)} entries, at most {MAX_LOGIT_BIAS}")
+    return tuple(sorted(out))
+
+
+def _logit_biases(logit_bias, B: int) -> List[Optional[tuple]]:
+    """One logit bias (None or a mapping) for all B sequences, or a sequence of B of them."""
+    if _is_collection(logit_bias) and not isinstance(logit_bias, Mapping):
+        vals = [check_logit_bias(v) for v in logit_bias]
+        if len(vals) != B:
+            raise ValueError(f"logit_bias: {len(vals)} values for {B} sequences")
+        return vals
+    return [check_logit_bias(logit_bias)] * B
+
+
+def check_allowed_token_ids(allowed_token_ids, V: Optional[int] = None) -> Optional[tuple]:
+    """An allowed set: None (every id), or a non-empty collection of distinct integer ids in [0, V) (the upper bound is
+    checked once V is given).  -> None or the sorted ids; a set that covers all of [0, V) is None."""
+    if allowed_token_ids is None:
+        return None
+    if not _is_collection(allowed_token_ids):
+        raise ValueError(f"allowed_token_ids must be None or a collection of token ids, got {allowed_token_ids!r}")
+    ids = set()
+    for t in allowed_token_ids:
+        if isinstance(t, bool) or not isinstance(t, numbers.Integral) or t < 0 or (V is not None and t >= V):
+            raise ValueError(f"allowed_token_ids: {t!r} is not a token id in [0, {V if V is not None else 'V'})")
+        if int(t) in ids:
+            raise ValueError(f"allowed_token_ids: {int(t)} is listed twice")
+        ids.add(int(t))
+    if not ids:
+        raise ValueError("allowed_token_ids must not be empty (None allows every id)")
+    if V is not None and len(ids) == V:
+        return None
+    return tuple(sorted(ids))
+
+
+def _allowed_sets(allowed_token_ids, B: int) -> List[Optional[tuple]]:
+    """One allowed set (None or a collection of ids) for all B sequences, or a sequence of B of them (a non-empty sequence
+    whose entries are all None or collections)."""
+    if isinstance(allowed_token_ids, Sequence) and _is_collection(allowed_token_ids) and len(allowed_token_ids) > 0 \
+            and all(t is None or _is_collection(t) for t in allowed_token_ids):
+        sets = [check_allowed_token_ids(t) for t in allowed_token_ids]
+        if len(sets) != B:
+            raise ValueError(f"allowed_token_ids: {len(sets)} sets for {B} sequences")
+        return sets
+    return [check_allowed_token_ids(allowed_token_ids)] * B
+
+
+def is_neutral_bias(logit_bias: Optional[tuple], allowed_token_ids: Optional[tuple]) -> bool:
+    """The checked settings that leave a row as it is: no bias entries and no allowed set."""
+    return not logit_bias and allowed_token_ids is None
+
+
 def check_seed(seed) -> int:
     """A per-sequence seed: an integer in [0, 2^64)."""
     if isinstance(seed, bool) or not isinstance(seed, numbers.Integral):
@@ -288,7 +370,11 @@ class BatchTree:
     honour them.  Penalties count at most 4096 tokens: a tree with max_length > 4096 refuses a non-neutral setting.
     logprobs: None (off) or an integer in 0..20, for all sequences or one per prompt: token_logprobs(b) then gives the
     log-probability of each generated token and of the n best alternatives of its row (module docstring,
-    include/sequoia_b200.h).  Both policies honour it; verify() returns what it returns without it."""
+    include/sequoia_b200.h).  Both policies honour it; verify() returns what it returns without it.
+    logit_bias: None or a mapping {id: bias} of at most 1024 ids in [0, V) with biases in [-100, 100] (-100 bans an id in
+    practice), for all sequences or one per prompt.  allowed_token_ids: None or a non-empty collection of distinct ids in
+    [0, V), for all sequences or one per prompt: every other id is -inf in the sequence's target rows.  Both policies
+    honour both; a greedy sequence takes the argmax of the processed row (module docstring, include/sequoia_b200.h)."""
 
     def __init__(self, draft, target, prompts: Sequence[torch.Tensor], grow_map: dict,
                  policy: Union[str, Sequence[str]] = "spec",
@@ -299,9 +385,11 @@ class BatchTree:
                  repetition_penalty: Union[float, Sequence[float]] = 1.0,
                  frequency_penalty: Union[float, Sequence[float]] = 0.0,
                  presence_penalty: Union[float, Sequence[float]] = 0.0,
-                 logprobs: Union[None, int, Sequence[Optional[int]]] = None):
+                 logprobs: Union[None, int, Sequence[Optional[int]]] = None,
+                 logit_bias=None, allowed_token_ids=None):
         B = len(prompts)
         policies = _policies(policy, B)
+        biases, alloweds = _logit_biases(logit_bias, B), _allowed_sets(allowed_token_ids, B)
         lps = _logprobs(logprobs, B)
         reps = _penalties("repetition_penalty", repetition_penalty, B)
         freqs = _penalties("frequency_penalty", frequency_penalty, B)
@@ -341,6 +429,8 @@ class BatchTree:
         for pol in set(policies):
             check_vocab(pol, V)
         stops = [check_stop_tokens(t, V) for t in stops]
+        biases = [check_logit_bias(None if t is None else dict(t), V) for t in biases]
+        alloweds = [check_allowed_token_ids(t, V) for t in alloweds]
         M = max_length
         for p in prompts:
             if len(p) + S - 1 > M:
@@ -383,6 +473,13 @@ class BatchTree:
         self.n_top_dev = torch.tensor([-1 if n is None else n for n in lps], dtype=torch.int32, device=dev)
         self.use_logprobs = False
         self.lp_token = self.lp_ids = self.lp_top = None
+        # logit bias and allowed sets: each slot's bitmask row and sorted (id, bias) entries on the device, read by
+        # sq_logit_bias_rows_batch inside the captured graphs, which it joins the first time a slot is non-neutral
+        self.logit_bias, self.allowed_token_ids = biases, alloweds
+        self.use_logit_bias = False
+        self.allowed_dev = self.has_mask_dev = self.bias_ids_dev = self.bias_vals_dev = self.n_bias_dev = None
+        if not all(is_neutral_bias(*v) for v in zip(biases, alloweds)):
+            self._start_logit_bias()
         self.finish_reason: List[Optional[str]] = [None] * B
         i64 = dict(dtype=torch.int64, device=dev)
         self.tokens = torch.zeros(B, M, **i64)
@@ -453,6 +550,36 @@ class BatchTree:
         self.lp_ids = torch.full((B, M, MAX_LOGPROBS), -1, dtype=torch.int32, device=dev)
         self.lp_top = torch.full((B, M, MAX_LOGPROBS), float("nan"), dtype=torch.float32, device=dev)
 
+    def _start_logit_bias(self):
+        """The mask-and-bias kernel joins op_accept, with every slot's device rows; it writes no scratch, so nothing joins
+        the captured buffers."""
+        self.use_logit_bias = True
+        B, dev = self.B, self.device
+        i32 = dict(dtype=torch.int32, device=dev)
+        self.allowed_dev = torch.zeros(B, ops.mask_words(self.V), **i32)
+        self.has_mask_dev = torch.zeros(B, **i32)
+        self.n_bias_dev = torch.zeros(B, **i32)
+        self.bias_ids_dev = torch.zeros(B, MAX_LOGIT_BIAS, **i32)
+        self.bias_vals_dev = torch.zeros(B, MAX_LOGIT_BIAS, dtype=torch.float32, device=dev)
+        for b in range(B):
+            self._write_logit_bias(b)
+
+    def _write_logit_bias(self, b: int):
+        """Slot b's device rows from its host settings: the bitmask (zeros without a set) and the entries (zero padded)."""
+        bias, allowed = self.logit_bias[b] or (), self.allowed_token_ids[b]
+        mask = ops.pack_token_mask(allowed, self.V) if allowed is not None else torch.zeros(ops.mask_words(self.V),
+                                                                                             dtype=torch.int32)
+        ids = torch.zeros(MAX_LOGIT_BIAS, dtype=torch.int32)
+        vals = torch.zeros(MAX_LOGIT_BIAS, dtype=torch.float32)
+        if bias:
+            ids[:len(bias)] = torch.tensor([t for t, _ in bias], dtype=torch.int32)
+            vals[:len(bias)] = torch.tensor([v for _, v in bias], dtype=torch.float32)
+        self.allowed_dev[b].copy_(_h2d(mask), non_blocking=True)
+        self.bias_ids_dev[b].copy_(_h2d(ids), non_blocking=True)
+        self.bias_vals_dev[b].copy_(_h2d(vals), non_blocking=True)
+        self.has_mask_dev[b] = 0 if allowed is None else 1
+        self.n_bias_dev[b] = len(bias)
+
     def _load_prompt(self, b: int, prompt: torch.Tensor):
         """Row b of tokens, position ids, state and accept_idx for a new prompt: nothing of an earlier occupant stays."""
         P, S, M = len(prompt), self.S, self.M
@@ -484,7 +611,7 @@ class BatchTree:
               seed: Optional[int] = None, policy: Optional[str] = None, top_k: Optional[int] = None,
               stop_tokens=_PREVIOUS, max_new_tokens=_PREVIOUS, repetition_penalty: Optional[float] = None,
               frequency_penalty: Optional[float] = None, presence_penalty: Optional[float] = None,
-              logprobs=_PREVIOUS):
+              logprobs=_PREVIOUS, logit_bias=_PREVIOUS, allowed_token_ids=_PREVIOUS):
         """Start `prompt` in the frozen slot b (finished, out of room, or stopped with freeze), at its own policy,
         temperature, top_p and top_k (default: the slot's previous values).  The next verify() runs its first verify next
         to the steady sequences.  The slot draws r and rand as a lone SpecTree on the prompt would, and runs its draft
@@ -502,7 +629,9 @@ class BatchTree:
         ones); they count this prompt and its output only.  The first non-neutral setting in a tree without one captures
         the steady and post graphs once more.
         logprobs: the prompt's logprobs setting (default: the slot's previous one; None is off).  The first one that is
-        on, in a tree without one, captures the steady and post graphs once more."""
+        on, in a tree without one, captures the steady and post graphs once more.
+        logit_bias / allowed_token_ids: the prompt's logit bias and allowed set (default: the slot's previous ones; None is
+        none).  The first non-neutral one, in a tree without one, captures the steady and post graphs once more."""
         if policy is not None:
             check_policy(policy)
         if top_k is not None:
@@ -516,6 +645,10 @@ class BatchTree:
                  ("presence_penalty", presence_penalty))]
         if logprobs is not _PREVIOUS:
             logprobs = check_logprobs(logprobs)
+        if logit_bias is not _PREVIOUS:
+            logit_bias = check_logit_bias(logit_bias, self.V)
+        if allowed_token_ids is not _PREVIOUS:
+            allowed_token_ids = check_allowed_token_ids(allowed_token_ids, self.V)
         if not 0 <= b < self.B:
             raise IndexError(f"slot {b} out of range for a batch of {self.B}")
         if not self.frozen[b]:
@@ -583,6 +716,16 @@ class BatchTree:
             self._start_logprobs()                 # the logprobs kernel enters seq_post: capture steady and post once more
             for name in ("steady", "post"):
                 self.graphs.pop(name, None)
+        if logit_bias is not _PREVIOUS:
+            self.logit_bias[b] = logit_bias
+        if allowed_token_ids is not _PREVIOUS:
+            self.allowed_token_ids[b] = allowed_token_ids
+        if self.use_logit_bias:
+            self._write_logit_bias(b)
+        elif not is_neutral_bias(self.logit_bias[b], self.allowed_token_ids[b]):
+            self._start_logit_bias()               # the bias kernel enters op_accept: capture steady and post once more
+            for name in ("steady", "post"):
+                self.graphs.pop(name, None)
         if pol == "spec" and self.r is None:       # the first sampling sequence of a tree built all-greedy
             self.r = torch.zeros(self.B, self.M, dtype=F16, device=self.device)
             self.rand = torch.zeros(self.B, self.S, self.V, dtype=F16, device=self.device)
@@ -638,6 +781,9 @@ class BatchTree:
 
     def op_accept(self):
         st = self.st
+        if self.use_logit_bias:                    # first: a bias is in logit space, the penalties then scale it
+            ops.logit_bias_rows_batch_(self.target_logits, self.S, self.state, self.allowed_dev, self.has_mask_dev,
+                                       self.bias_ids_dev, self.bias_vals_dev, self.n_bias_dev)
         if self.use_penalty:                       # first: the greedy walk and the filters rank the penalised rows
             ops.penalize_rows_batch_(self.target_logits, self.tokens, self.state, self.prompt_len_dev, st.tree_bits,
                                      st.tree_words, self.S, self.rep_dev, self.freq_dev, self.pres_dev, self.pen_scratch)

@@ -797,3 +797,51 @@ def token_logprobs_batch_(target_logits, S: int, max_depth: int, tokens, state, 
                                               _rows(accept_idx, "accept_idx"), ptr(T), ptr(greedy), ptr(n_top),
                                               ptr(lp_token), ptr(lp_ids), ptr(lp_top), B, stream_ptr()),
           "sq_token_logprobs_batch")
+
+
+# ---- per-sequence allowed-token mask and logit bias (csrc/sq_logit_bias.cu; semantics in include/sequoia_b200.h) ----------
+def mask_words(V: int) -> int:
+    """int32 words of one allowed-token bitmask row: ceil(V / 32)."""
+    return (V + 31) // 32
+
+
+def pack_token_mask(ids, V: int) -> torch.Tensor:
+    """The (mask_words(V),) int32 bitmask of a collection of ids in [0, V) on the host: bit t & 31 of word t >> 5 set for
+    every id t; the padding bits from V on are clear."""
+    words = mask_words(V)
+    bits = torch.zeros(words * 32, dtype=torch.bool)
+    bits[torch.as_tensor(list(ids), dtype=torch.int64)] = True
+    w = (bits.view(words, 32).to(torch.int64) << torch.arange(32, dtype=torch.int64)).sum(1)
+    return torch.where(w >= 1 << 31, w - (1 << 32), w).to(torch.int32)
+
+
+def logit_bias_rows_batch_(logits, S: int, state, allowed, has_mask, bias_ids, bias_vals, n_bias):
+    """Apply sequence b's allowed-token mask (when has_mask[b]) and then its logit bias entries in place to its S target
+    rows b*S .. b*S+S-1 of the (>= B*S, V) fp16 logits.  allowed: (B, >= mask_words(V)) int32 bitmask rows; has_mask,
+    n_bias: (B,) int32; bias_ids / bias_vals: (B, SQ_MAX_LOGIT_BIAS) int32 / float32, each row's first n_bias[b] ids
+    ascending; all on the device.  Frozen sequences and sequences with no mask and no entries are left untouched."""
+    name = "logit_bias_rows_batch_"
+    _need(logits, F16, name)
+    if logits.dim() != 2 or logits.stride(-1) != 1:
+        raise ValueError(f"{name}: logits must be (rows, V) with contiguous rows, got {tuple(logits.shape)}")
+    _need(state, torch.int32, name)
+    if not state.is_contiguous():
+        raise ValueError(f"{name}: state must be contiguous")
+    B = state.shape[0]
+    if logits.shape[0] < B * S:
+        raise ValueError(f"{name}: {logits.shape[0]} logit rows for {B} sequences of {S}")
+    for k, t in (("has_mask", has_mask), ("n_bias", n_bias)):
+        if t is None or t.dtype != torch.int32 or not t.is_cuda or t.dim() != 1 or t.shape[0] < B or t.stride(0) != 1:
+            raise TypeError(f"{name}: {k} must be a contiguous ({B},) int32 CUDA tensor")
+    nmax = _lib.SQ_MAX_LOGIT_BIAS
+    for k, t, dt, cols in (("allowed", allowed, torch.int32, mask_words(logits.shape[1])),
+                           ("bias_ids", bias_ids, torch.int32, nmax), ("bias_vals", bias_vals, torch.float32, nmax)):
+        _need(t, dt, name)
+        if t.dim() != 2 or t.shape[0] < B or t.shape[1] < cols or not t.is_contiguous():
+            raise ValueError(f"{name}: {k} must be a contiguous ({B}, >= {cols}) tensor, got {tuple(t.shape)}")
+    if bias_ids.shape[1] != nmax or bias_vals.shape[1] != nmax:
+        raise ValueError(f"{name}: bias_ids and bias_vals must have {nmax} columns")
+    check(_lib.load().sq_logit_bias_rows_batch(ptr(logits), logits.stride(0), logits.shape[1], S, ptr(state), ptr(allowed),
+                                               allowed.shape[1], ptr(has_mask), ptr(bias_ids), ptr(bias_vals),
+                                               ptr(n_bias), B, stream_ptr()), "sq_logit_bias_rows_batch")
+    return logits

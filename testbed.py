@@ -285,7 +285,7 @@ def decode_chunk(tree, chunk, limits, stop=DEFAULT_STOP, logprob_means=None, i0:
 @torch.inference_mode()
 def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: int, stop=DEFAULT_STOP,
                      refill: bool = False, seeds=None, policies=None, top_k: int = 0, device_stop: bool = False,
-                     penalties=None, logprobs=None):
+                     penalties=None, logprobs=None, logit_bias=None):
     """--batch B: the same metric loop with B prompts decoded together (sequoia_b200.batch.BatchTree).  Chunked: B
     prompts at a time, each chunk until its last sequence stops.  refill: one batch whose finished slots take the next
     prompt (BatchTree.admit).  seeds: one per prompt (--device-rng): each sequence draws its random numbers on the device
@@ -294,7 +294,8 @@ def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: i
     length limit the host loop applies (--device-stop), without overshoot.  penalties: every prompt's
     repetition_penalty / frequency_penalty / presence_penalty keywords (--repetition-penalty ..., batch_penalties); refill
     admissions keep them.  logprobs: every prompt's logprobs setting (--logprobs, None = off); the mean logprob of each
-    prompt's generated tokens is printed and returned."""
+    prompt's generated tokens is printed and returned.  logit_bias: every prompt's logit_bias / allowed_token_ids keywords
+    (--logit-bias / --allowed-token-ids, batch_logit_bias); refill admissions keep them."""
     from sequoia_b200.batch import BatchTree
     steps = decoded = 0                          # steps: target steps summed over sequences (per-sequence tokens / step)
     total_time = 0.0
@@ -307,6 +308,7 @@ def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: i
         i0 = c * B
         pol = policy if policies is None else policies[i0:i0 + len(chunk)]
         kw = dict(penalties or {})
+        kw.update(logit_bias or {})
         if logprobs is not None:
             kw["logprobs"] = logprobs
         if dstop is not None:
@@ -379,6 +381,10 @@ def build_parser():
                     help="with --batch: vLLM's presence penalty of every prompt (0 = off), on the target rows")
     ap.add_argument("--logprobs", type=int, default=None,
                     help="with --batch: the top alternatives per token (0..20); prints each prompt's mean token logprob")
+    ap.add_argument("--logit-bias", type=str, default=None,
+                    help="with --batch: ID:BIAS[,ID:BIAS...], added to every prompt's target logits (bias in [-100, 100])")
+    ap.add_argument("--allowed-token-ids", type=str, default=None,
+                    help="with --batch: LO-HI|ID[,...] (ranges inclusive), the only ids every prompt may generate")
     ap.add_argument("--target-weights", type=str, default="fp16", choices=["fp16", "fp8"],
                     help="fp8: the target's layer projections quantized to E4M3 with per-channel scales at load")
     return ap
@@ -475,6 +481,47 @@ def batch_logprobs(args):
     return n
 
 
+def _parse_logit_bias(text: str) -> dict:
+    out = {}
+    for item in text.split(","):
+        t, sep, v = item.partition(":")
+        if not sep:
+            raise ValueError(f"{item!r} is not ID:BIAS")
+        out[int(t)] = float(v)
+    return out
+
+
+def _parse_token_ids(text: str) -> list:
+    out = []
+    for item in text.split(","):
+        lo, sep, hi = item.strip().partition("-")
+        out.extend(range(int(lo), int(hi) + 1) if sep else [int(lo)])
+    return out
+
+
+def batch_logit_bias(args) -> dict:
+    """--logit-bias ID:BIAS[,...] / --allowed-token-ids LO-HI|ID[,...]: BatchTree's logit_bias / allowed_token_ids for
+    every prompt ({} when neither is given).  Refused when malformed or outside what BatchTree takes (ids are checked
+    against the vocabulary when the tree is built), and without --batch: the lone trees keep the reference's sampling."""
+    from sequoia_b200.batch import check_allowed_token_ids, check_logit_bias
+    kw = {}
+    for flag, attr, parse, check in (("--logit-bias", "logit_bias", _parse_logit_bias, check_logit_bias),
+                                     ("--allowed-token-ids", "allowed_token_ids", _parse_token_ids,
+                                      check_allowed_token_ids)):
+        text = getattr(args, attr)
+        if text is None:
+            continue
+        try:
+            val = check(parse(text))
+        except ValueError as e:
+            raise SystemExit(f"{flag}: {e}")
+        kw[attr] = dict(val) if attr == "logit_bias" else val     # (a mapping: a sequence would be one per prompt)
+    if kw and args.batch == 1 and not args.refill:
+        raise SystemExit("--logit-bias / --allowed-token-ids run with --batch (the batched tree); the lone trees keep the "
+                         "reference's sampling")
+    return kw
+
+
 def main(argv=None):
     args = build_parser().parse_args(argv)
     print(args)
@@ -492,6 +539,7 @@ def main(argv=None):
     device_stop = batch_device_stop(args)
     penalties = batch_penalties(args)
     logprobs = batch_logprobs(args)
+    logit_bias = batch_logit_bias(args)
     if args.batch != 1 or args.refill:
         B = check_batch_args(args, len(prompts))
         target = GraphInferenceEngineTG(max_length=args.M, model_name_or_path=args.target, dtype=torch.float16,
@@ -503,7 +551,8 @@ def main(argv=None):
         assert args.M >= MAX_NEW_LEN + grow_map["size"], "--M must hold 256 tokens + the tree (README.md:47 of the reference)"
         res = simulation_batch(target, draft, prompts, grow_map, args.tree, args.T, args.P, args.M, B, stop=stop,
                                refill=args.refill, seeds=seeds, policies=policies, top_k=top_k,
-                               device_stop=device_stop, penalties=penalties, logprobs=logprobs)
+                               device_stop=device_stop, penalties=penalties, logprobs=logprobs,
+                               logit_bias=logit_bias)
         print(json.dumps({k: (round(v, 5) if isinstance(v, float) else v) for k, v in res.items()}))
         return res
     target = (tcls(max_length=args.M, model_name_or_path=args.target, dtype=torch.float16, device=DEV)
