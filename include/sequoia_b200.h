@@ -394,6 +394,19 @@ int sq_top_p_filter_per_seq(sq_half* logits, int64_t ld, int n, int V, const flo
  * bit for bit what the scalar call computes.  A null array is refused with SQ_ERR_INVALID_ARG. */
 int sq_top_k_filter_per_seq(sq_half* logits, int64_t ld, int n, int V, const int32_t* top_k, int rows_per_seq,
                             void* stream);
+/* Min-p filter, in place on n rows; row r belongs to sequence b = r / rows_per_seq (rows_per_seq must divide n), whose
+ * fp32 ln(min_p) and temperature are log_min_p[b] and T[b], (B,) float32 device arrays; log_min_p[b] = -inf is off and
+ * leaves the rows untouched.  vLLM's rule, softmax(x / T)_i >= min_p * max softmax(x / T), decided in logit space: with
+ * x_i the fp32 value of the fp16 logit, m the row max over its non-NaN entries and thr = fp32(T[b] * log_min_p[b]) (one
+ * round-to-nearest multiply), token i keeps its logit when x_i is NaN, x_i == m or fp32(x_i - m) >= thr, and becomes -inf
+ * otherwise.  So NaN stays (the walk's NaN flag still ends the sequence), a +inf entry stays and drops every finite entry
+ * of its row, -inf stays, min_p = 1 (ln 1 = 0) keeps only the ties with the max, and a -inf threshold keeps everything.
+ * Min-p and top-k both keep an upper set of the value order that contains the max, so on NaN-free rows they commute bit
+ * for bit; run before sq_top_p_filter_per_seq, which then renormalises over the survivors.  Deterministic (no atomics).
+ * A null array, a rows_per_seq that does not divide n and a bad V are refused with SQ_ERR_INVALID_ARG; n == 0 is a
+ * no-op. */
+int sq_min_p_filter_per_seq(sq_half* logits, int64_t ld, int n, int V, const float* log_min_p, const float* T,
+                            int rows_per_seq, void* stream);
 /* target_token (B*S) int64 */
 int sq_accept_greedy_batch(const int64_t* target_token, const int32_t* succ_off, const int32_t* succ, const int32_t* depth,
                            int S, int64_t* tokens, int64_t* position_ids, int64_t ld_seq, int32_t* accept_idx,

@@ -103,6 +103,7 @@ _SIGNATURES = {
     "sq_top_p_filter_per_seq": (i32, [vp, i64, i32, i32, vp, vp, i32, vp]),
     "sq_top_k_filter": (i32, [vp, i64, i32, i32, i32, vp]),
     "sq_top_k_filter_per_seq": (i32, [vp, i64, i32, i32, vp, i32, vp]),
+    "sq_min_p_filter_per_seq": (i32, [vp, i64, i32, i32, vp, vp, i32, vp]),
     "sq_ragged_layout": (i32, [vp, i32, i32, i32, i32, vp, vp]),
     "sq_embed_rows_ragged": (i32, [vp, vp, i64, vp, vp, i32, i32, i32, i32, vp, vp]),
     "sq_rope_kv_append_ragged": (i32, [vp, i32, i32, i32, i32, vp, vp, vp, vp, i64, vp, vp, i32, i32, i32, vp, vp, i32,

@@ -3,9 +3,9 @@
 A steady step is the same two graph replays and one host sync as a single-sequence tree (sequoia_b200.tree), for all B
 sequences together: every per-sequence kernel is one launch for the batch, the row-wise kernels and the GEMMs see B*n
 rows.  Sequence b's device data: row b of state (B, 16), tokens / position_ids / storage_ids / r (B, M), rand (B, S, V),
-noise (B, V), accept_idx (B, S), its temperature and top_p (B,) and top_k (B,) int32; rows b*S .. b*S+S-1 of the target
-logits (B*S, V); the draft logits of node k at row_base[k] + b*row_step[k] (each tree level of all sequences is one
-block, written by one lm_head GEMM).
+noise (B, V), accept_idx (B, S), its temperature, top_p and log_min_p (B,) and top_k (B,) int32; rows b*S .. b*S+S-1 of
+the target logits (B*S, V); the draft logits of node k at row_base[k] + b*row_step[k] (each tree level of all sequences
+is one block, written by one lm_head GEMM).
 
 A sequence that is terminal, or has no room for another tree in max_length, is frozen: its state word SQ_ST_FROZEN is
 set and every batched kernel leaves its tokens, state and KV rows alone.  A frozen slot can take a new prompt with
@@ -15,7 +15,8 @@ Each sequence has its own policy, "spec" or "greedy".  While all are equal the t
 once both are present (mixed mode, which then stays on) the sampler and the two walks are the *_mixed forms, which read
 the (B,) int32 device array greedy_dev, and every sequence decodes as it would in a tree of its own policy.
 
-A sampled sequence draws from softmax(top_p(top_k(logits)) / T): the accept walk filters the target rows first to the
+A sampled sequence draws from softmax(top_p(top_k(min_p(logits))) / T): the accept walk filters the target rows first
+to the tokens whose probability at T is at least min_p times the row's largest (0 = off, vLLM's min_p), then to the
 top_k best raw logits (0 = off), then to top_p, and speculative sampling stays exact for the filtered distribution.
 Each filter joins the captured graphs the first time a sampled sequence needs it (one recapture each); after that any
 values run in the same graphs.
@@ -132,6 +133,29 @@ def _top_ks(top_k, B: int) -> List[int]:
             raise ValueError(f"top_k: {len(ks)} values for {B} sequences")
         return ks
     return [check_top_k(top_k)] * B
+
+
+def check_min_p(min_p) -> float:
+    """A min_p: a finite real number in [0, 1] (not a bool); 0 is off, 1 keeps only the tokens tied with the row's max."""
+    if isinstance(min_p, bool) or not isinstance(min_p, numbers.Real) or not 0 <= min_p <= 1:
+        raise ValueError(f"min_p must be a number in [0, 1] (0 = off), got {min_p!r}")
+    return float(min_p)
+
+
+def _min_ps(min_p, B: int) -> List[float]:
+    """One min_p for all B sequences, or a sequence of B of them."""
+    if _is_collection(min_p):
+        vals = [check_min_p(v) for v in min_p]
+        if len(vals) != B:
+            raise ValueError(f"min_p: {len(vals)} values for {B} sequences")
+        return vals
+    return [check_min_p(min_p)] * B
+
+
+def _log_min_p(policy: str, min_p: float) -> float:
+    """A slot's device value: fp32(ln min_p) (ln in double precision), or -inf when the filter is off for it (min_p 0, or
+    a greedy sequence)."""
+    return float("-inf") if policy == "greedy" or min_p == 0.0 else _fp32(math.log(min_p))
 
 
 def check_stop_tokens(stop_tokens, V: Optional[int] = None) -> Optional[tuple]:
@@ -356,6 +380,9 @@ class BatchTree:
     top_k: one integer >= 0 for all sequences, or one per sequence: a sampled sequence keeps the top_k best target logits
     of each row (raw value descending, equal values by ascending index) before top_p and its softmax; 0, and any value
     >= the vocabulary size, is off.  "greedy" sequences ignore it.
+    min_p: one number in [0, 1] for all sequences, or one per sequence: a sampled sequence keeps the target tokens whose
+    probability at its temperature is at least min_p times the row's largest, before top_k, top_p and the softmax
+    (vLLM's min_p; 0 is off).  "greedy" sequences ignore it.
     seeds: None (r and rand drawn with torch's CPU generator as a lone SpecTree draws them, the bonus noise with torch's
     CUDA generator), or one integer in [0, 2^64) per prompt: each sequence then draws all its random numbers on the
     device from a Philox stream keyed by its seed, so its output does not depend on its slot or its neighbours ("greedy"
@@ -386,9 +413,10 @@ class BatchTree:
                  frequency_penalty: Union[float, Sequence[float]] = 0.0,
                  presence_penalty: Union[float, Sequence[float]] = 0.0,
                  logprobs: Union[None, int, Sequence[Optional[int]]] = None,
-                 logit_bias=None, allowed_token_ids=None):
+                 logit_bias=None, allowed_token_ids=None, min_p: Union[float, Sequence[float]] = 0.0):
         B = len(prompts)
         policies = _policies(policy, B)
+        min_ps = _min_ps(min_p, B)
         biases, alloweds = _logit_biases(logit_bias, B), _allowed_sets(allowed_token_ids, B)
         lps = _logprobs(logprobs, B)
         reps = _penalties("repetition_penalty", repetition_penalty, B)
@@ -448,6 +476,11 @@ class BatchTree:
         self.top_k_dev = torch.tensor([0 if pol == "greedy" else min(k, V) for pol, k in zip(policies, top_ks)],
                                       dtype=torch.int32, device=dev)
         self.use_top_k = any(pol == "spec" and 0 < k < V for pol, k in zip(policies, top_ks))
+        # the same for min_p, held as fp32(ln min_p) (-inf = off, and for a greedy sequence)
+        self.min_ps = min_ps
+        self.log_min_p_dev = torch.tensor([_log_min_p(pol, p) for pol, p in zip(policies, min_ps)], dtype=torch.float32,
+                                          device=dev)
+        self.use_min_p = any(pol == "spec" and p > 0.0 for pol, p in zip(policies, min_ps))
         # stop mode: each slot's stop ids (-1 padded) and absolute length limit (0 = none) on the device, read by the stop
         # walks inside the captured graphs, which replace the walks the first time a slot has either (one recapture)
         self.stop_tokens, self.max_new_tokens = stops, budgets
@@ -611,7 +644,7 @@ class BatchTree:
               seed: Optional[int] = None, policy: Optional[str] = None, top_k: Optional[int] = None,
               stop_tokens=_PREVIOUS, max_new_tokens=_PREVIOUS, repetition_penalty: Optional[float] = None,
               frequency_penalty: Optional[float] = None, presence_penalty: Optional[float] = None,
-              logprobs=_PREVIOUS, logit_bias=_PREVIOUS, allowed_token_ids=_PREVIOUS):
+              logprobs=_PREVIOUS, logit_bias=_PREVIOUS, allowed_token_ids=_PREVIOUS, min_p: Optional[float] = None):
         """Start `prompt` in the frozen slot b (finished, out of room, or stopped with freeze), at its own policy,
         temperature, top_p and top_k (default: the slot's previous values).  The next verify() runs its first verify next
         to the steady sequences.  The slot draws r and rand as a lone SpecTree on the prompt would, and runs its draft
@@ -622,6 +655,8 @@ class BatchTree:
         captured once more, on their next use.  A tree built all-greedy allocates r and rand at its first "spec"
         admission.  The first "spec" admission with 0 < top_k < V (in a tree that had none) captures the steady and post
         graphs once more: the top-k filter joins the accept step.
+        min_p: the prompt's min_p (default: the slot's previous one).  The first "spec" admission with min_p > 0, in a tree
+        that had none, captures the steady and post graphs once more: the min-p filter joins the accept step.
         stop_tokens / max_new_tokens: the prompt's stop set and token budget (default: the slot's previous ones; None is
         none).  The budget counts from this prompt.  The first admission that brings a stop set or a budget to a tree in
         default mode captures the steady and post graphs once more: the stop walks replace the walks.
@@ -636,6 +671,8 @@ class BatchTree:
             check_policy(policy)
         if top_k is not None:
             top_k = check_top_k(top_k)
+        if min_p is not None:
+            min_p = check_min_p(min_p)
         if stop_tokens is not _PREVIOUS:
             stop_tokens = check_stop_tokens(stop_tokens, self.V)
         if max_new_tokens is not _PREVIOUS:
@@ -667,6 +704,7 @@ class BatchTree:
             seed = check_seed(seed)
         pol = self.policies[b] if policy is None else policy
         k = self.top_ks[b] if top_k is None else top_k
+        mp = self.min_ps[b] if min_p is None else min_p
         stop = self.stop_tokens[b] if stop_tokens is _PREVIOUS else stop_tokens
         budget = self.max_new_tokens[b] if max_new_tokens is _PREVIOUS else max_new_tokens
         rep, freq, pres = (old[b] if v is None else v for v, old in
@@ -692,6 +730,12 @@ class BatchTree:
                 self.graphs.pop(name, None)
         if 0 < k < self.V and pol == "spec" and not self.use_top_k:
             self.use_top_k = True                  # the same for the top-k filter
+            for name in ("steady", "post"):
+                self.graphs.pop(name, None)
+        self.min_ps[b] = mp
+        self.log_min_p_dev[b] = _log_min_p(pol, mp)
+        if mp > 0.0 and pol == "spec" and not self.use_min_p:
+            self.use_min_p = True                  # the same for the min-p filter
             for name in ("steady", "post"):
                 self.graphs.pop(name, None)
         self.stop_tokens[b], self.max_new_tokens[b] = stop, budget
@@ -807,6 +851,8 @@ class BatchTree:
                 ops.accept_greedy_batch_mixed(self.target_token, st.succ_off, st.succ, st.depth, self.S, self.greedy_dev,
                                               self.tokens, self.position_ids, self.accept_idx, self.state,
                                               self.max_target_seq)
+        if self.use_min_p:                         # vLLM's order: min_p, top_k, top_p (min_p and top_k commute)
+            ops.min_p_filter_per_seq_(self.target_logits, self.log_min_p_dev, self.T_dev, self.S)
         if self.use_top_k:                         # top_k before top_p: top_p renormalises over the k survivors
             ops.top_k_filter_per_seq_(self.target_logits, self.top_k_dev, self.S)
         if self.use_top_p:

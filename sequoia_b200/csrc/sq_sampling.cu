@@ -908,6 +908,64 @@ __global__ void __launch_bounds__(NT) top_k_filter_kernel(__half* __restrict__ l
   }
 }
 
+// ---------------------------------------------------------------------------------------------
+// Min-p filter, in place: token i keeps its logit when softmax(x / T)_i >= min_p * max_j softmax(x / T)_j, else becomes
+// -inf.  Decided in logit space, exp((x_i - m) / T) >= min_p <=> x_i - m >= T * ln(min_p), so neither side needs an exp or
+// a log: with m the NaN-ignoring row max (fmaxf) and thr = fp32(T) * fp32(ln min_p) (one round-to-nearest multiply; the
+// host supplies ln min_p), token i stays when it is NaN, equals m, or fp32(x_i - m) >= thr.  NaN stays NaN (the walk's
+// NaN flag still ends the sequence), a +inf entry stays and drops every finite one, -inf stays -inf.  Only 16-byte packs
+// holding a dropped finite entry are written.  One read of the row, one block max (WIDE: plus one cluster max), no
+// histogram, no atomics.  Row r belongs to sequence r / rows_per_seq; a row whose log_min_p is -inf (off) returns after
+// griddepcontrol.wait without touching memory (the whole cluster reads the same value).
+template <bool WIDE>
+__global__ void __launch_bounds__(NT) min_p_filter_kernel(__half* __restrict__ logits, int64_t ld, int V,
+                                                           const float* __restrict__ log_min_p,
+                                                           const float* __restrict__ T, int rows_per_seq) {
+  __shared__ float red[NW];
+  pdl_wait();
+  Slice sl{};
+  if constexpr (WIDE) sl = slice_of(V);
+  const int seq = (WIDE ? sl.row : (int)blockIdx.x) / rows_per_seq;
+  const float lmp = log_min_p[seq];
+  if (lmp == -INFINITY) return;
+  const float thr = __fmul_rn(T[seq], lmp);
+  __half* row;
+  if constexpr (WIDE) {
+    row = logits + sl.row * ld + sl.base;
+    V = sl.V;
+  } else {
+    row = logits + blockIdx.x * ld;
+  }
+  const int nvec = V / 8;
+  Pack8 x[CH];
+  load_row(row, V, x);
+  float m = -INFINITY;
+#pragma unroll
+  for (int i = 0; i < CH; ++i)
+#pragma unroll
+    for (int e = 0; e < 8; ++e) m = fmaxf(m, h2f(x[i].h[e]));      // (padding chunks are -inf)
+  m = block_max<NW>(m, red);
+  if constexpr (WIDE) {
+    __shared__ float xs[MAX_SLICES];
+    m = cl_max(m, xs, sl);
+  }
+#pragma unroll
+  for (int i = 0; i < CH; ++i) {
+    const int c = i * NT + threadIdx.x;
+    if (c >= nvec) continue;
+    bool any = false;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      const float v = h2f(x[i].h[e]);
+      // (v > -inf is false for NaN and -inf, which stay as they are)
+      const bool drop = v > -INFINITY && v != m && !(__fsub_rn(v, m) >= thr);
+      if (drop) x[i].h[e] = __ushort_as_half((unsigned short)0xFC00u);     // -inf
+      any |= drop;
+    }
+    if (any) reinterpret_cast<uint4*>(row)[c] = x[i].u;
+  }
+}
+
 }  // namespace sq
 
 using namespace sq;
@@ -1154,5 +1212,22 @@ extern "C" int sq_top_k_filter_per_seq(sq_half* logits, int64_t ld, int n, int V
   }
   top_k_filter_kernel<false, true><<<n, NT, 0, (cudaStream_t)stream>>>((__half*)logits, ld, V, top_k, rows_per_seq);
   SQ_CHECK_LAUNCH("sq_top_k_filter_per_seq");
+  return SQ_OK;
+}
+
+extern "C" int sq_min_p_filter_per_seq(sq_half* logits, int64_t ld, int n, int V, const float* log_min_p, const float* T,
+                                       int rows_per_seq, void* stream) {
+  SQ_CHECK_V_WIDE(V);
+  SQ_CHECK_ARG(log_min_p != nullptr && T != nullptr, "sq_min_p_filter_per_seq: null log_min_p or temperature array");
+  SQ_CHECK_ARG(rows_per_seq >= 1 && n >= 0 && n % rows_per_seq == 0,
+               "sq_min_p_filter_per_seq: rows_per_seq=%d does not divide n=%d", rows_per_seq, n);
+  if (n == 0) return SQ_OK;
+  if (V > SLICE) {
+    SQ_CHECK_WIDE_LAUNCH(launch_wide(min_p_filter_kernel<true>, n, 1, V, (cudaStream_t)stream, (__half*)logits, ld, V,
+                                     log_min_p, T, rows_per_seq), "sq_min_p_filter_per_seq");
+    return SQ_OK;
+  }
+  min_p_filter_kernel<false><<<n, NT, 0, (cudaStream_t)stream>>>((__half*)logits, ld, V, log_min_p, T, rows_per_seq);
+  SQ_CHECK_LAUNCH("sq_min_p_filter_per_seq");
   return SQ_OK;
 }

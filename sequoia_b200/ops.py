@@ -571,6 +571,20 @@ def top_k_filter_per_seq_(logits, top_k, rows_per_seq: int):
     return logits
 
 
+def min_p_filter_per_seq_(logits, log_min_p, T, rows_per_seq: int):
+    """Min-p filter in place on (n, V) fp16 logits whose row r belongs to sequence b = r // rows_per_seq: a token keeps its
+    logit when its probability at T[b] is at least min_p times the row's largest, else it becomes -inf (the exact rule in
+    include/sequoia_b200.h).  log_min_p and T are (B,) float32 on the device, log_min_p[b] = fp32(ln min_p) or -inf (off:
+    the rows are left untouched)."""
+    _need(logits, F16, "min_p_filter_per_seq_")
+    n, V = logits.shape
+    B = n // rows_per_seq if rows_per_seq > 0 else 0
+    _seq_params("min_p_filter_per_seq_", B, log_min_p=log_min_p, T=T)
+    check(_lib.load().sq_min_p_filter_per_seq(ptr(logits), logits.stride(0), n, V, ptr(log_min_p), ptr(T), rows_per_seq,
+                                              stream_ptr()), "sq_min_p_filter_per_seq")
+    return logits
+
+
 # ---- per-sequence counter-based random numbers (csrc/sq_rng.cu; stream layout in include/sequoia_b200.h) -------------------
 RNG_R, RNG_RAND, RNG_NOISE = 0, 1, 2     # purposes: r (M), rand (S*V, node-major), bonus noise (V, one step per verify)
 

@@ -285,7 +285,7 @@ def decode_chunk(tree, chunk, limits, stop=DEFAULT_STOP, logprob_means=None, i0:
 @torch.inference_mode()
 def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: int, stop=DEFAULT_STOP,
                      refill: bool = False, seeds=None, policies=None, top_k: int = 0, device_stop: bool = False,
-                     penalties=None, logprobs=None, logit_bias=None):
+                     penalties=None, logprobs=None, logit_bias=None, min_p: float = 0.0):
     """--batch B: the same metric loop with B prompts decoded together (sequoia_b200.batch.BatchTree).  Chunked: B
     prompts at a time, each chunk until its last sequence stops.  refill: one batch whose finished slots take the next
     prompt (BatchTree.admit).  seeds: one per prompt (--device-rng): each sequence draws its random numbers on the device
@@ -295,7 +295,8 @@ def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: i
     repetition_penalty / frequency_penalty / presence_penalty keywords (--repetition-penalty ..., batch_penalties); refill
     admissions keep them.  logprobs: every prompt's logprobs setting (--logprobs, None = off); the mean logprob of each
     prompt's generated tokens is printed and returned.  logit_bias: every prompt's logit_bias / allowed_token_ids keywords
-    (--logit-bias / --allowed-token-ids, batch_logit_bias); refill admissions keep them."""
+    (--logit-bias / --allowed-token-ids, batch_logit_bias); refill admissions keep them.  min_p: every sampled prompt's
+    min-p filter (--min-p, 0 = off); refill admissions keep it."""
     from sequoia_b200.batch import BatchTree
     steps = decoded = 0                          # steps: target steps summed over sequences (per-sequence tokens / step)
     total_time = 0.0
@@ -314,7 +315,8 @@ def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: i
         if dstop is not None:
             kw.update(stop_tokens=dstop[0][i0:i0 + len(chunk)], max_new_tokens=dstop[1][i0:i0 + len(chunk)])
         tree = BatchTree(draft, target, chunk, grow_map, policy=pol, temperature=T, top_p=top_p, max_length=M,
-                         max_target_seq=M, seeds=None if seeds is None else seeds[i0:i0 + len(chunk)], top_k=top_k, **kw)
+                         max_target_seq=M, seeds=None if seeds is None else seeds[i0:i0 + len(chunk)], top_k=top_k, min_p=min_p,
+                         **kw)
         torch.cuda.synchronize()
         t1 = time.time()
         if refill:
@@ -370,6 +372,9 @@ def build_parser():
                          "policies[i %% len], greedy and sampled prompts in one batch")
     ap.add_argument("--top-k", type=int, default=0,
                     help="with --batch: keep the K best target logits of each row before top_p (0 = off)")
+    ap.add_argument("--min-p", type=float, default=0.0,
+                    help="with --batch: keep the target tokens whose probability is at least P times the row's largest, "
+                         "before top_k and top_p (0 = off)")
     ap.add_argument("--device-stop", action="store_true",
                     help="with --batch: each sequence ends on the device at the target's stop ids (anywhere in an "
                          "accepted path) and at the length limit, exactly, instead of after the step")
@@ -438,6 +443,16 @@ def batch_top_k(args) -> int:
     if args.top_k and args.batch == 1 and not args.refill:
         raise SystemExit("--top-k runs with --batch (the batched tree); the lone trees keep the reference's sampling")
     return args.top_k
+
+
+def batch_min_p(args) -> float:
+    """--min-p: every prompt's min_p (0 = off).  Refused outside [0, 1], and without --batch: the lone trees keep the
+    reference's sampling."""
+    if not 0.0 <= args.min_p <= 1.0:
+        raise SystemExit(f"--min-p must be in [0, 1], got {args.min_p}")
+    if args.min_p and args.batch == 1 and not args.refill:
+        raise SystemExit("--min-p runs with --batch (the batched tree); the lone trees keep the reference's sampling")
+    return args.min_p
 
 
 def batch_device_stop(args) -> bool:
@@ -536,6 +551,7 @@ def main(argv=None):
     seeds = device_rng_seeds(args, len(prompts))
     policies = prompt_policies(args, len(prompts))
     top_k = batch_top_k(args)
+    min_p = batch_min_p(args)
     device_stop = batch_device_stop(args)
     penalties = batch_penalties(args)
     logprobs = batch_logprobs(args)
@@ -552,7 +568,7 @@ def main(argv=None):
         res = simulation_batch(target, draft, prompts, grow_map, args.tree, args.T, args.P, args.M, B, stop=stop,
                                refill=args.refill, seeds=seeds, policies=policies, top_k=top_k,
                                device_stop=device_stop, penalties=penalties, logprobs=logprobs,
-                               logit_bias=logit_bias)
+                               logit_bias=logit_bias, min_p=min_p)
         print(json.dumps({k: (round(v, 5) if isinstance(v, float) else v) for k, v in res.items()}))
         return res
     target = (tcls(max_length=args.M, model_name_or_path=args.target, dtype=torch.float16, device=DEV)
