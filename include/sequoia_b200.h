@@ -504,6 +504,34 @@ int sq_penalize_rows_batch(sq_half* logits, int64_t ld, int V, const int64_t* to
 int sq_logit_bias_rows_batch(sq_half* logits, int64_t ld, int V, int S, const int32_t* state, const uint32_t* allowed,
                              int64_t allowed_words, const int32_t* has_mask, const int32_t* bias_ids,
                              const float* bias_vals, const int32_t* n_bias, int B, void* stream);
+/* Per-sequence bad words and min_tokens (csrc/sq_ban.cu), in place on the (B*S, V) target rows (row b*S + k = node k of
+ * sequence b, row pitch ld >= V), right after sq_logit_bias_rows_batch and before the penalties, the walks and the
+ * filters read them.  Each row gets a small set of banned ids that become -inf; the set depends on the tree path.
+ *   Context of row k: with P = state[b][SQ_ST_P], the committed tokens[b, 0 .. P) at positions 0 .. P-1, then the path
+ *   tokens at slots P-1+j of the ancestors-or-self j >= 1 of node k (the bits of row k of tree_bits), at positions
+ *   P .. P+d-1 in slot order, d = depth[k] (node indices increase along every path).  The row's token lands at position
+ *   P + d.  The generated context is the part at positions >= L = prompt_len[b].  A context token outside [0, V) matches
+ *   no word id.
+ *   Bad words (vLLM v1's rule, on output tokens only): words (B, SQ_MAX_BAD_WORDS, SQ_MAX_BAD_WORD_LEN) int32, word w of
+ *   sequence b at [b][w][0 .. n), n = word_len[b][w]; the first min(n_words[b], SQ_MAX_BAD_WORDS) words are read.  When
+ *   the generated context has at least n - 1 tokens and its last n - 1 equal w[0 .. n-2], id w[n-1] is banned (a
+ *   one-token word in every row; a prefix that would reach into the prompt does not match).  A word with n outside
+ *   1..SQ_MAX_BAD_WORD_LEN, or whose last id is outside [0, V), bans nothing.
+ *   min_tokens: min_end (B,) int32, the absolute limit L + min_tokens (0 = off).  When P + d < min_end[b], every id of
+ *   row b of end_ids (B, SQ_MAX_STOP) int32 in [0, V) is banned (-1 pads the row).
+ *   A banned entry becomes -inf (0xFC00) unconditionally, NaN and +inf included; nothing else of the row is touched.
+ * A sequence with SQ_ST_FROZEN set, or with n_words <= 0 and min_end <= 0, has its rows left byte-identical (its CTAs
+ * return right after the PDL wait); rows from B*S on are never touched.  One PDL-chained launch, grid (S, B) of 128
+ * threads; no state, no scratch.  Refused with SQ_ERR_INVALID_ARG before any launch: a null array, B outside
+ * 1..SQ_MAX_BATCH, V not a multiple of 8 in 8..131072, ld < V, S < 1 or tree_words != ceil(S/32) or tree_words > 32,
+ * ld_seq < 1. */
+#define SQ_MAX_BAD_WORDS 128
+#define SQ_MAX_BAD_WORD_LEN 16
+int sq_ban_tokens_rows_batch(sq_half* logits, int64_t ld, int V, const int64_t* tokens, int64_t ld_seq,
+                             const int32_t* state, const int32_t* prompt_len, const int32_t* depth,
+                             const uint32_t* tree_bits, int tree_words, int S, const int32_t* words,
+                             const int32_t* word_len, const int32_t* n_words, const int32_t* min_end,
+                             const int32_t* end_ids, int B, void* stream);
 /* Per-sequence logprobs of the committed tokens (csrc/sq_logprobs.cu), after the walk, from the (B*S, V) target rows as the
  * walk read them (penalised, top-k and top-p filtered; row pitch ld >= V, a multiple of 8).  With P = state[b][SQ_ST_P_OLD],
  * n_new = state[b][SQ_ST_N_NEW], a = P + n_new and M = state[b][SQ_ST_M] (ld_seq when 0), the step committed position

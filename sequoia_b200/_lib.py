@@ -25,6 +25,8 @@ SQ_PENALTY_MAX_LEN = 4096
 SQ_MAX_LOGPROBS = 20
 # per-sequence logit bias: the most (id, bias) entries sq_logit_bias_rows_batch holds per sequence
 SQ_MAX_LOGIT_BIAS = 1024
+# per-sequence bad words: the most words sq_ban_tokens_rows_batch holds per sequence, and the most ids per word
+SQ_MAX_BAD_WORDS, SQ_MAX_BAD_WORD_LEN = 128, 16
 
 i32, i64, f32, vp = C.c_int, C.c_int64, C.c_float, C.c_void_p
 
@@ -122,6 +124,7 @@ _SIGNATURES = {
     "sq_penalize_rows_batch": (i32, [vp, i64, i32, vp, i64, vp, vp, vp, i32, i32, vp, vp, vp, vp, i64, i32, vp]),
     "sq_token_logprobs_batch": (i32, [vp, i64, i32, i32, i32, vp, i64, vp, vp, i64, vp, vp, vp, vp, vp, vp, i32, vp]),
     "sq_logit_bias_rows_batch": (i32, [vp, i64, i32, i32, vp, vp, i64, vp, vp, vp, vp, i32, vp]),
+    "sq_ban_tokens_rows_batch": (i32, [vp, i64, i32, vp, i64, vp, vp, vp, vp, i32, i32, vp, vp, vp, vp, vp, i32, vp]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

@@ -50,6 +50,19 @@ filters then read the processed rows (the draft is not processed, speculative sa
 the allowed set can never be generated, so it never ends the sequence.  While every sequence is neutral (no bias entries,
 no allowed set) nothing is allocated or launched; the first non-neutral setting, at construction or admission, captures
 the steady and post graphs once more, and the kernel then stays in them.
+
+Bad words and min_tokens: each sequence has bad_words (token sequences its output must never contain) and min_tokens
+(the tokens it must generate before it may end), vLLM's parameters.  Right after the logit bias, sq_ban_tokens_rows_batch
+sets a few ids of each target row to -inf, for the context the row was computed from (the committed tokens plus the
+tree path to its node): the last id of every word whose other ids end the row's generated context, and, while the row's
+token would land before len(prompt) + min_tokens, the sequence's end ids (its stop ids in stop mode, 0 and 2 in default
+mode).  The draft is not processed; speculative sampling stays exact, so no walk draws a banned id from the row that
+bans it (on a branching tree the stochastic walk's bonus_first quirk can still commit the bonus token at an accepted
+node's position, whose row did not draw it; DESIGN.md §3a).  A row can still lose every finite entry on some path
+(settings that do so in every row are refused): a sampled sequence then ends by the walk's NaN flag (finish_reason
+"nan"), a greedy one commits id 0, the argmax of an all -inf row.  While every sequence is neutral (no words,
+min_tokens 0) nothing is allocated or launched; the first non-neutral setting, at construction or admission, captures
+the steady and post graphs once more, and the kernel then stays in them.
 """
 from __future__ import annotations
 
@@ -71,10 +84,13 @@ PENALTY_MAX_LEN = _lib.SQ_PENALTY_MAX_LEN
 MAX_LOGPROBS = _lib.SQ_MAX_LOGPROBS
 MAX_LOGIT_BIAS = _lib.SQ_MAX_LOGIT_BIAS
 LOGIT_BIAS_MAX = 100.0
+MAX_BAD_WORDS, MAX_BAD_WORD_LEN = _lib.SQ_MAX_BAD_WORDS, _lib.SQ_MAX_BAD_WORD_LEN
+DEFAULT_END_IDS = (0, 2)    # the ids the walks end a sequence on in default mode (the reference's fixed rule)
 FP16_MAX = 65504.0
 INT32_MAX = (1 << 31) - 1
 POLICIES = ("spec", "greedy")
-_PREVIOUS = object()        # admit(): keep the slot's previous stop set / budget / logprobs / logit bias / allowed set
+_PREVIOUS = object()        # admit(): keep the slot's previous stop set / budget / logprobs / logit bias / allowed set /
+                            # bad words / min_tokens
 
 
 def draw_random(prompts: Sequence[torch.Tensor], M: int, S: int, V: int):
@@ -356,6 +372,94 @@ def is_neutral_bias(logit_bias: Optional[tuple], allowed_token_ids: Optional[tup
     return not logit_bias and allowed_token_ids is None
 
 
+def check_bad_words(bad_words, V: Optional[int] = None) -> Optional[tuple]:
+    """Bad words: None, or a collection of words, each a non-empty sequence of at most MAX_BAD_WORD_LEN integer ids in
+    [0, V) (not bools; the upper bound is checked once V is given), at most MAX_BAD_WORDS distinct words.  -> None, or the
+    distinct words as tuples in first-seen order (duplicates dropped; an empty collection is ())."""
+    if bad_words is None:
+        return None
+    if not _is_collection(bad_words):
+        raise ValueError(f"bad_words must be None or a collection of words (sequences of token ids), got {bad_words!r}")
+    out = {}
+    for w in bad_words:
+        if not isinstance(w, Sequence) or isinstance(w, (str, bytes)) or not 1 <= len(w) <= MAX_BAD_WORD_LEN:
+            raise ValueError(f"bad_words: a word is a sequence of 1..{MAX_BAD_WORD_LEN} token ids, got {w!r}")
+        for t in w:
+            if isinstance(t, bool) or not isinstance(t, numbers.Integral) or t < 0 or (V is not None and t >= V):
+                raise ValueError(f"bad_words: {t!r} is not a token id in [0, {V if V is not None else 'V'})")
+        out.setdefault(tuple(int(t) for t in w), None)
+    if len(out) > MAX_BAD_WORDS:
+        raise ValueError(f"bad_words: {len(out)} distinct words, at most {MAX_BAD_WORDS}")
+    return tuple(out)
+
+
+def _is_word_set(x) -> bool:
+    """None, or a collection whose entries are all collections: one prompt's set of words in the per-prompt form."""
+    return x is None or (_is_collection(x) and all(_is_collection(w) for w in x))
+
+
+def _bad_words(bad_words, B: int) -> List[Optional[tuple]]:
+    """One set of words for all B sequences, or one per sequence.  The per-prompt form is a non-empty sequence whose every
+    entry is None or a collection of collections (three levels of nesting: [None, [[2, 3]]]); anything else is one set
+    for all prompts (two levels: [[1], [2, 3]] is one set of two words).  So [[], []] gives two prompts no words each."""
+    if isinstance(bad_words, Sequence) and _is_collection(bad_words) and len(bad_words) > 0 \
+            and all(_is_word_set(e) for e in bad_words):
+        sets = [check_bad_words(e) for e in bad_words]
+        if len(sets) != B:
+            raise ValueError(f"bad_words: {len(sets)} sets for {B} sequences")
+        return sets
+    return [check_bad_words(bad_words)] * B
+
+
+def check_min_tokens(min_tokens, max_new_tokens: Optional[int] = None) -> int:
+    """A min_tokens: an integer >= 0 (not a bool; 0 = off), at most the sequence's max_new_tokens when it has one (vLLM
+    refuses min_tokens > max_tokens)."""
+    if isinstance(min_tokens, bool) or not isinstance(min_tokens, numbers.Integral) or min_tokens < 0:
+        raise ValueError(f"min_tokens must be an integer >= 0 (0 = off), got {min_tokens!r}")
+    if max_new_tokens is not None and min_tokens > max_new_tokens:
+        raise ValueError(f"min_tokens={int(min_tokens)} exceeds max_new_tokens={max_new_tokens}")
+    return int(min_tokens)
+
+
+def _min_tokens(min_tokens, B: int) -> List[int]:
+    """One min_tokens for all B sequences, or a sequence of B of them."""
+    if _is_collection(min_tokens):
+        vals = [check_min_tokens(m) for m in min_tokens]
+        if len(vals) != B:
+            raise ValueError(f"min_tokens: {len(vals)} values for {B} sequences")
+        return vals
+    return [check_min_tokens(min_tokens)] * B
+
+
+def _min_end(prompt_len: int, min_tokens: int) -> int:
+    """The absolute limit len(prompt) + min_tokens the device holds (0 = off; clamped to int32)."""
+    return 0 if min_tokens == 0 else min(prompt_len + min_tokens, INT32_MAX)
+
+
+def end_ids(stop_tokens: Optional[tuple], stop_mode: bool) -> tuple:
+    """The ids that end a sequence, which min_tokens bans: its stop ids in stop mode (none without a stop set), else
+    DEFAULT_END_IDS, the reference's fixed rule."""
+    return (stop_tokens or ()) if stop_mode else DEFAULT_END_IDS
+
+
+def check_bannable(V: int, bad_words: Optional[tuple], allowed_token_ids: Optional[tuple], min_tokens: int,
+                   ends: tuple):
+    """Refuse settings that ban every id a sequence may generate in every row: its one-token words, plus its end ids
+    when min_tokens > 0, cover the vocabulary or its allowed set."""
+    banned = {w[0] for w in bad_words or () if len(w) == 1}
+    if min_tokens > 0:
+        banned.update(ends)
+    candidates = range(V) if allowed_token_ids is None else allowed_token_ids
+    if len(banned) >= len(candidates) and all(t in banned for t in candidates):
+        raise ValueError("bad_words" + (" and min_tokens" if min_tokens > 0 else "") + " ban every token id the "
+                         "sequence may generate" + (" (its allowed_token_ids)" if allowed_token_ids is not None else ""))
+
+
+def is_neutral_ban(bad_words: Optional[tuple], min_tokens: int) -> bool:
+    """The checked settings that ban nothing: no words and min_tokens 0."""
+    return not bad_words and min_tokens == 0
+
+
 def check_seed(seed) -> int:
     """A per-sequence seed: an integer in [0, 2^64)."""
     if isinstance(seed, bool) or not isinstance(seed, numbers.Integral):
@@ -401,7 +505,13 @@ class BatchTree:
     logit_bias: None or a mapping {id: bias} of at most 1024 ids in [0, V) with biases in [-100, 100] (-100 bans an id in
     practice), for all sequences or one per prompt.  allowed_token_ids: None or a non-empty collection of distinct ids in
     [0, V), for all sequences or one per prompt: every other id is -inf in the sequence's target rows.  Both policies
-    honour both; a greedy sequence takes the argmax of the processed row (module docstring, include/sequoia_b200.h)."""
+    honour both; a greedy sequence takes the argmax of the processed row (module docstring, include/sequoia_b200.h).
+    bad_words: None, or a collection of at most 128 words, each a sequence of 1..16 ids in [0, V), for all sequences
+    ([[1], [2, 3]]: two words); or one such value (or None) per prompt ([None, [[2, 3]]]: three levels of nesting).  The
+    output then never contains a word: its last id is banned wherever its other ids end the generated tokens (a one-token
+    word everywhere; a word never matches across the prompt).  min_tokens: an integer >= 0 (at most max_new_tokens), for
+    all sequences or one per prompt: the sequence's end ids are banned until it has generated that many tokens.  Both
+    policies honour both (module docstring, include/sequoia_b200.h)."""
 
     def __init__(self, draft, target, prompts: Sequence[torch.Tensor], grow_map: dict,
                  policy: Union[str, Sequence[str]] = "spec",
@@ -413,10 +523,12 @@ class BatchTree:
                  frequency_penalty: Union[float, Sequence[float]] = 0.0,
                  presence_penalty: Union[float, Sequence[float]] = 0.0,
                  logprobs: Union[None, int, Sequence[Optional[int]]] = None,
-                 logit_bias=None, allowed_token_ids=None, min_p: Union[float, Sequence[float]] = 0.0):
+                 logit_bias=None, allowed_token_ids=None, min_p: Union[float, Sequence[float]] = 0.0,
+                 bad_words=None, min_tokens: Union[int, Sequence[int]] = 0):
         B = len(prompts)
         policies = _policies(policy, B)
         min_ps = _min_ps(min_p, B)
+        words, min_toks = _bad_words(bad_words, B), _min_tokens(min_tokens, B)
         biases, alloweds = _logit_biases(logit_bias, B), _allowed_sets(allowed_token_ids, B)
         lps = _logprobs(logprobs, B)
         reps = _penalties("repetition_penalty", repetition_penalty, B)
@@ -459,6 +571,11 @@ class BatchTree:
         stops = [check_stop_tokens(t, V) for t in stops]
         biases = [check_logit_bias(None if t is None else dict(t), V) for t in biases]
         alloweds = [check_allowed_token_ids(t, V) for t in alloweds]
+        words = [check_bad_words(w, V) for w in words]
+        stop_mode = any(t is not None for t in stops) or any(n is not None for n in budgets)
+        for b in range(B):
+            check_min_tokens(min_toks[b], budgets[b])
+            check_bannable(V, words[b], alloweds[b], min_toks[b], end_ids(stops[b], stop_mode))
         M = max_length
         for p in prompts:
             if len(p) + S - 1 > M:
@@ -487,7 +604,7 @@ class BatchTree:
         self.stop_ids_dev = torch.tensor([_stop_row(t) for t in stops], dtype=torch.int32, device=dev)
         self.end_limit_dev = torch.tensor([_end_limit(len(p), n) for p, n in zip(prompts, budgets)], dtype=torch.int32,
                                           device=dev)
-        self.use_stop = any(t is not None for t in stops) or any(n is not None for n in budgets)
+        self.use_stop = stop_mode
         # penalties: each slot's values and prompt length on the device, read by sq_penalize_rows_batch inside the
         # captured graphs, which it joins the first time a slot has a non-neutral setting (one recapture)
         self.repetition_penalty, self.frequency_penalty, self.presence_penalty = reps, freqs, press
@@ -506,6 +623,13 @@ class BatchTree:
         self.n_top_dev = torch.tensor([-1 if n is None else n for n in lps], dtype=torch.int32, device=dev)
         self.use_logprobs = False
         self.lp_token = self.lp_ids = self.lp_top = None
+        # bad words and min_tokens: each slot's word table and absolute limit L + min_tokens on the device, read by
+        # sq_ban_tokens_rows_batch inside the captured graphs, which it joins the first time a slot is non-neutral
+        self.bad_words, self.min_tokens = words, min_toks
+        self.use_ban = False
+        self.words_dev = self.word_len_dev = self.n_words_dev = self.min_end_dev = self.default_end_dev = None
+        if not all(is_neutral_ban(*v) for v in zip(words, min_toks)):
+            self._start_ban()
         # logit bias and allowed sets: each slot's bitmask row and sorted (id, bias) entries on the device, read by
         # sq_logit_bias_rows_batch inside the captured graphs, which it joins the first time a slot is non-neutral
         self.logit_bias, self.allowed_token_ids = biases, alloweds
@@ -613,6 +737,39 @@ class BatchTree:
         self.has_mask_dev[b] = 0 if allowed is None else 1
         self.n_bias_dev[b] = len(bias)
 
+    def _start_ban(self):
+        """The ban kernel joins op_accept, with every slot's device rows; it writes no scratch, so nothing joins the
+        captured buffers."""
+        self.use_ban = True
+        B, dev = self.B, self.device
+        i32 = dict(dtype=torch.int32, device=dev)
+        self.words_dev = torch.zeros(B, MAX_BAD_WORDS, MAX_BAD_WORD_LEN, **i32)
+        self.word_len_dev = torch.zeros(B, MAX_BAD_WORDS, **i32)
+        self.n_words_dev = torch.zeros(B, **i32)
+        self.min_end_dev = torch.zeros(B, **i32)
+        self.default_end_dev = torch.tensor([_stop_row(DEFAULT_END_IDS)] * B, **i32)
+        for b in range(B):
+            self._write_ban(b)
+
+    def _write_ban(self, b: int):
+        """Slot b's device rows from its host settings: the words (zero padded), their lengths and L + min_tokens."""
+        words = self.bad_words[b] or ()
+        table = torch.zeros(MAX_BAD_WORDS, MAX_BAD_WORD_LEN, dtype=torch.int32)
+        lens = torch.zeros(MAX_BAD_WORDS, dtype=torch.int32)
+        for i, w in enumerate(words):
+            table[i, :len(w)] = torch.tensor(w, dtype=torch.int32)
+            lens[i] = len(w)
+        self.words_dev[b].copy_(_h2d(table), non_blocking=True)
+        self.word_len_dev[b].copy_(_h2d(lens), non_blocking=True)
+        self.n_words_dev[b] = len(words)
+        self.min_end_dev[b] = _min_end(self.prompt_lens[b], self.min_tokens[b])
+
+    def _ban_end_ids(self) -> torch.Tensor:
+        """The (B, MAX_STOP) end-id rows the ban kernel reads: in stop mode the stop walks' own stop_ids_dev, so a slot's
+        end ids are its stop ids with no copy to keep in step; in default mode DEFAULT_END_IDS for every slot.  Stop mode
+        starts with a recapture, which takes the new array into the graphs."""
+        return self.stop_ids_dev if self.use_stop else self.default_end_dev
+
     def _load_prompt(self, b: int, prompt: torch.Tensor):
         """Row b of tokens, position ids, state and accept_idx for a new prompt: nothing of an earlier occupant stays."""
         P, S, M = len(prompt), self.S, self.M
@@ -644,7 +801,8 @@ class BatchTree:
               seed: Optional[int] = None, policy: Optional[str] = None, top_k: Optional[int] = None,
               stop_tokens=_PREVIOUS, max_new_tokens=_PREVIOUS, repetition_penalty: Optional[float] = None,
               frequency_penalty: Optional[float] = None, presence_penalty: Optional[float] = None,
-              logprobs=_PREVIOUS, logit_bias=_PREVIOUS, allowed_token_ids=_PREVIOUS, min_p: Optional[float] = None):
+              logprobs=_PREVIOUS, logit_bias=_PREVIOUS, allowed_token_ids=_PREVIOUS, min_p: Optional[float] = None,
+              bad_words=_PREVIOUS, min_tokens=_PREVIOUS):
         """Start `prompt` in the frozen slot b (finished, out of room, or stopped with freeze), at its own policy,
         temperature, top_p and top_k (default: the slot's previous values).  The next verify() runs its first verify next
         to the steady sequences.  The slot draws r and rand as a lone SpecTree on the prompt would, and runs its draft
@@ -666,7 +824,10 @@ class BatchTree:
         logprobs: the prompt's logprobs setting (default: the slot's previous one; None is off).  The first one that is
         on, in a tree without one, captures the steady and post graphs once more.
         logit_bias / allowed_token_ids: the prompt's logit bias and allowed set (default: the slot's previous ones; None is
-        none).  The first non-neutral one, in a tree without one, captures the steady and post graphs once more."""
+        none).  The first non-neutral one, in a tree without one, captures the steady and post graphs once more.
+        bad_words / min_tokens: the prompt's bad words (None is none) and min_tokens (default: the slot's previous ones);
+        min_tokens counts from this prompt.  The first non-neutral one, in a tree without one, captures the steady and post
+        graphs once more."""
         if policy is not None:
             check_policy(policy)
         if top_k is not None:
@@ -686,6 +847,10 @@ class BatchTree:
             logit_bias = check_logit_bias(logit_bias, self.V)
         if allowed_token_ids is not _PREVIOUS:
             allowed_token_ids = check_allowed_token_ids(allowed_token_ids, self.V)
+        if bad_words is not _PREVIOUS:
+            bad_words = check_bad_words(bad_words, self.V)
+        if min_tokens is not _PREVIOUS:
+            min_tokens = check_min_tokens(min_tokens)
         if not 0 <= b < self.B:
             raise IndexError(f"slot {b} out of range for a batch of {self.B}")
         if not self.frozen[b]:
@@ -711,6 +876,11 @@ class BatchTree:
                            zip(pens, (self.repetition_penalty, self.frequency_penalty, self.presence_penalty)))
         if not is_neutral(rep, freq, pres) and self.M > PENALTY_MAX_LEN:
             raise ValueError(f"penalties count at most {PENALTY_MAX_LEN} tokens; this tree's max_length={self.M}")
+        words = self.bad_words[b] if bad_words is _PREVIOUS else bad_words
+        m = self.min_tokens[b] if min_tokens is _PREVIOUS else min_tokens
+        check_min_tokens(m, budget)
+        check_bannable(self.V, words, self.allowed_token_ids[b] if allowed_token_ids is _PREVIOUS else allowed_token_ids,
+                       m, end_ids(stop, self.use_stop or stop is not None or budget is not None))
         # (every other slot holds the tree's one policy until then, so a different one means both are present; at B = 1
         # it is a switch, which the single-policy graphs do not serve either)
         enter_mixed = not self.mixed and pol != ("greedy" if self.greedy else "spec")
@@ -768,6 +938,13 @@ class BatchTree:
             self._write_logit_bias(b)
         elif not is_neutral_bias(self.logit_bias[b], self.allowed_token_ids[b]):
             self._start_logit_bias()               # the bias kernel enters op_accept: capture steady and post once more
+            for name in ("steady", "post"):
+                self.graphs.pop(name, None)
+        self.bad_words[b], self.min_tokens[b] = words, m
+        if self.use_ban:
+            self._write_ban(b)
+        elif not is_neutral_ban(words, m):
+            self._start_ban()                      # the ban kernel enters op_accept: capture steady and post once more
             for name in ("steady", "post"):
                 self.graphs.pop(name, None)
         if pol == "spec" and self.r is None:       # the first sampling sequence of a tree built all-greedy
@@ -828,6 +1005,10 @@ class BatchTree:
         if self.use_logit_bias:                    # first: a bias is in logit space, the penalties then scale it
             ops.logit_bias_rows_batch_(self.target_logits, self.S, self.state, self.allowed_dev, self.has_mask_dev,
                                        self.bias_ids_dev, self.bias_vals_dev, self.n_bias_dev)
+        if self.use_ban:                           # -inf whatever the bias; the penalties leave -inf alone
+            ops.ban_tokens_rows_batch_(self.target_logits, self.tokens, self.state, self.prompt_len_dev, st.depth,
+                                       st.tree_bits, st.tree_words, self.S, self.words_dev, self.word_len_dev,
+                                       self.n_words_dev, self.min_end_dev, self._ban_end_ids())
         if self.use_penalty:                       # first: the greedy walk and the filters rank the penalised rows
             ops.penalize_rows_batch_(self.target_logits, self.tokens, self.state, self.prompt_len_dev, st.tree_bits,
                                      st.tree_words, self.S, self.rep_dev, self.freq_dev, self.pres_dev, self.pen_scratch)

@@ -859,3 +859,42 @@ def logit_bias_rows_batch_(logits, S: int, state, allowed, has_mask, bias_ids, b
                                                allowed.shape[1], ptr(has_mask), ptr(bias_ids), ptr(bias_vals),
                                                ptr(n_bias), B, stream_ptr()), "sq_logit_bias_rows_batch")
     return logits
+
+
+# ---- per-sequence bad words and min_tokens (csrc/sq_ban.cu; semantics in include/sequoia_b200.h) ---------------------
+def ban_tokens_rows_batch_(logits, tokens, state, prompt_len, depth, tree_bits, tree_words: int, S: int, words, word_len,
+                           n_words, min_end, end_ids):
+    """Write -inf in place at the banned ids of sequence b's S target rows b*S .. b*S+S-1 of the (>= B*S, V) fp16 logits:
+    the last id of each bad word whose prefix ends the row's generated context (the committed tokens from slot
+    prompt_len[b] on, then node k's path on the tree), and the end ids while the row's position P + depth[k] is below
+    min_end[b].  words: (B, SQ_MAX_BAD_WORDS, SQ_MAX_BAD_WORD_LEN) int32; word_len: (B, SQ_MAX_BAD_WORDS) int32; n_words,
+    min_end, prompt_len: (B,) int32; end_ids: (B, SQ_MAX_STOP) int32, -1 padded; depth: (S,) int32; all on the device.
+    Frozen sequences and sequences with no words and min_end 0 are left untouched."""
+    name = "ban_tokens_rows_batch_"
+    _need(logits, F16, name)
+    if logits.dim() != 2 or logits.stride(-1) != 1:
+        raise ValueError(f"{name}: logits must be (rows, V) with contiguous rows, got {tuple(logits.shape)}")
+    _need(state, torch.int32, name)
+    _need(tokens, torch.int64, name)
+    _need(tree_bits, torch.int32, name)
+    if not state.is_contiguous() or not tree_bits.is_contiguous():
+        raise ValueError(f"{name}: state and tree_bits must be contiguous")
+    B = state.shape[0]
+    if logits.shape[0] < B * S:
+        raise ValueError(f"{name}: {logits.shape[0]} logit rows for {B} sequences of {S}")
+    if tokens.shape[0] < B:
+        raise ValueError(f"{name}: {tokens.shape[0]} token rows for {B} sequences")
+    for k, t, n in (("prompt_len", prompt_len, B), ("n_words", n_words, B), ("min_end", min_end, B), ("depth", depth, S)):
+        if t is None or t.dtype != torch.int32 or not t.is_cuda or t.dim() != 1 or t.shape[0] < n or t.stride(0) != 1:
+            raise TypeError(f"{name}: {k} must be a contiguous ({n},) int32 CUDA tensor")
+    nw, wl, ns = _lib.SQ_MAX_BAD_WORDS, _lib.SQ_MAX_BAD_WORD_LEN, _lib.SQ_MAX_STOP
+    for k, t, shape in (("words", words, (nw, wl)), ("word_len", word_len, (nw,)), ("end_ids", end_ids, (ns,))):
+        _need(t, torch.int32, name)
+        if tuple(t.shape[1:]) != shape or t.shape[0] < B or not t.is_contiguous():
+            raise ValueError(f"{name}: {k} must be a contiguous ({B}, {', '.join(map(str, shape))}) tensor, got "
+                             f"{tuple(t.shape)}")
+    check(_lib.load().sq_ban_tokens_rows_batch(ptr(logits), logits.stride(0), logits.shape[1], ptr(tokens),
+                                               _rows(tokens, "tokens"), ptr(state), ptr(prompt_len), ptr(depth),
+                                               ptr(tree_bits), tree_words, S, ptr(words), ptr(word_len), ptr(n_words),
+                                               ptr(min_end), ptr(end_ids), B, stream_ptr()), "sq_ban_tokens_rows_batch")
+    return logits

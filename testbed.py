@@ -285,7 +285,7 @@ def decode_chunk(tree, chunk, limits, stop=DEFAULT_STOP, logprob_means=None, i0:
 @torch.inference_mode()
 def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: int, stop=DEFAULT_STOP,
                      refill: bool = False, seeds=None, policies=None, top_k: int = 0, device_stop: bool = False,
-                     penalties=None, logprobs=None, logit_bias=None, min_p: float = 0.0):
+                     penalties=None, logprobs=None, logit_bias=None, min_p: float = 0.0, bad_words=None):
     """--batch B: the same metric loop with B prompts decoded together (sequoia_b200.batch.BatchTree).  Chunked: B
     prompts at a time, each chunk until its last sequence stops.  refill: one batch whose finished slots take the next
     prompt (BatchTree.admit).  seeds: one per prompt (--device-rng): each sequence draws its random numbers on the device
@@ -296,7 +296,8 @@ def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: i
     admissions keep them.  logprobs: every prompt's logprobs setting (--logprobs, None = off); the mean logprob of each
     prompt's generated tokens is printed and returned.  logit_bias: every prompt's logit_bias / allowed_token_ids keywords
     (--logit-bias / --allowed-token-ids, batch_logit_bias); refill admissions keep them.  min_p: every sampled prompt's
-    min-p filter (--min-p, 0 = off); refill admissions keep it."""
+    min-p filter (--min-p, 0 = off); refill admissions keep it.  bad_words: every prompt's bad_words / min_tokens
+    keywords (--bad-words / --min-tokens, batch_bad_words); refill admissions keep them."""
     from sequoia_b200.batch import BatchTree
     steps = decoded = 0                          # steps: target steps summed over sequences (per-sequence tokens / step)
     total_time = 0.0
@@ -310,6 +311,7 @@ def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: i
         pol = policy if policies is None else policies[i0:i0 + len(chunk)]
         kw = dict(penalties or {})
         kw.update(logit_bias or {})
+        kw.update(bad_words or {})
         if logprobs is not None:
             kw["logprobs"] = logprobs
         if dstop is not None:
@@ -372,6 +374,10 @@ def build_parser():
                          "policies[i %% len], greedy and sampled prompts in one batch")
     ap.add_argument("--top-k", type=int, default=0,
                     help="with --batch: keep the K best target logits of each row before top_p (0 = off)")
+    ap.add_argument("--bad-words", type=str, default=None,
+                    help="with --batch: ID,ID,...;ID;... token sequences no prompt's output may contain")
+    ap.add_argument("--min-tokens", type=int, default=None,
+                    help="with --batch: the tokens every prompt generates before a stop id (or 0 / 2) may end it")
     ap.add_argument("--min-p", type=float, default=0.0,
                     help="with --batch: keep the target tokens whose probability is at least P times the row's largest, "
                          "before top_k and top_p (0 = off)")
@@ -537,6 +543,30 @@ def batch_logit_bias(args) -> dict:
     return kw
 
 
+def batch_bad_words(args) -> dict:
+    """--bad-words ID,ID,...;ID;... / --min-tokens N: BatchTree's bad_words / min_tokens for every prompt ({} when
+    neither is given).  Refused when malformed or outside what BatchTree takes (ids are checked against the vocabulary
+    when the tree is built), and without --batch: the lone trees keep the reference's sampling."""
+    from sequoia_b200.batch import check_bad_words, check_min_tokens
+    kw = {}
+    try:
+        if args.bad_words is not None:
+            words = [[int(t) for t in w.split(",")] for w in args.bad_words.split(";")]
+            check_bad_words(words)
+            kw["bad_words"] = words
+    except ValueError as e:
+        raise SystemExit(f"--bad-words: {e}")
+    try:
+        if args.min_tokens is not None:
+            kw["min_tokens"] = check_min_tokens(args.min_tokens)
+    except ValueError as e:
+        raise SystemExit(f"--min-tokens: {e}")
+    if kw and args.batch == 1 and not args.refill:
+        raise SystemExit("--bad-words / --min-tokens run with --batch (the batched tree); the lone trees keep the "
+                         "reference's sampling")
+    return kw
+
+
 def main(argv=None):
     args = build_parser().parse_args(argv)
     print(args)
@@ -556,6 +586,7 @@ def main(argv=None):
     penalties = batch_penalties(args)
     logprobs = batch_logprobs(args)
     logit_bias = batch_logit_bias(args)
+    bad_words = batch_bad_words(args)
     if args.batch != 1 or args.refill:
         B = check_batch_args(args, len(prompts))
         target = GraphInferenceEngineTG(max_length=args.M, model_name_or_path=args.target, dtype=torch.float16,
@@ -568,7 +599,7 @@ def main(argv=None):
         res = simulation_batch(target, draft, prompts, grow_map, args.tree, args.T, args.P, args.M, B, stop=stop,
                                refill=args.refill, seeds=seeds, policies=policies, top_k=top_k,
                                device_stop=device_stop, penalties=penalties, logprobs=logprobs,
-                               logit_bias=logit_bias, min_p=min_p)
+                               logit_bias=logit_bias, min_p=min_p, bad_words=bad_words)
         print(json.dumps({k: (round(v, 5) if isinstance(v, float) else v) for k, v in res.items()}))
         return res
     target = (tcls(max_length=args.M, model_name_or_path=args.target, dtype=torch.float16, device=DEV)
