@@ -42,6 +42,9 @@ extern "C" {
 #define SQ_ST_FROZEN 9 /* host-written, batched calls only: nonzero = finished sequence, nothing of it is written */
 #define SQ_ST_FINISH 10 /* the *_batch_stop walks only: 0 = go on, 1 = a stop id ended the sequence, 2 = its length limit */
 #define SQ_ST_END 11    /* the *_batch_stop walks only: the sequence's final length when SQ_ST_FINISH != 0, else 0 */
+#define SQ_ST_GUIDED 12 /* host-written, batched calls only: nonzero = the sequence follows a token guide (sq_guide_*) */
+#define SQ_ST_GUIDE_STATE 13 /* guided sequences: the guide state after the committed tokens, -1 = dead */
+#define SQ_ST_GUIDE_POS 14   /* guided sequences: the position up to which the guide has consumed the tokens */
 #define SQ_ST_WORDS 16
 
 typedef uint16_t sq_half;
@@ -363,7 +366,10 @@ int sq_sample_level_batch(const sq_half* logits, int64_t ld_logits, const int32_
                           const sq_half* rand, int64_t ld_rand, int64_t ld_rand_seq, const int32_t* parent_rows,
                           const int32_t* child_first, const int32_t* n_branch, int n_parents, int k_max, int V, float T,
                           int mode, int64_t* tokens, int64_t ld_seq, const int32_t* state, int B, void* stream);
-/* one walk (one 8-CTA cluster) per sequence; target_logits (B*S, V) */
+/* one walk (one 8-CTA cluster) per sequence; target_logits (B*S, V).  Every batched stochastic walk (this one and its
+ * _per_seq, _mixed and _stop forms) writes the bonus token at slot a before it gathers the accepted slots, as SpecTree
+ * does, except for a sequence whose SQ_ST_GUIDED word is nonzero: that one gathers first and then writes the bonus, as
+ * GreedyTree does, so every committed token is the token its own row drew. */
 int sq_accept_stochastic_batch(const sq_half* target_logits, int64_t ld_t, const sq_half* draft_logits, int64_t ld_d,
                                const int32_t* row_base, const int32_t* row_step, const sq_half* r, const sq_half* noise,
                                int64_t ld_noise, const int32_t* succ_off, const int32_t* succ, const int32_t* depth, int S,
@@ -532,6 +538,51 @@ int sq_ban_tokens_rows_batch(sq_half* logits, int64_t ld, int V, const int64_t* 
                              const uint32_t* tree_bits, int tree_words, int S, const int32_t* words,
                              const int32_t* word_len, const int32_t* n_words, const int32_t* min_end,
                              const int32_t* end_ids, int B, void* stream);
+/* Guided decoding (csrc/sq_guide.cu): a per-sequence token automaton that constrains every target row along its tree path.
+ *   Guide blob: one int32 array per guided sequence, at the address guide_table[b] ((B,) int64 device table, 0 = none):
+ *     [0] n = n_states (1..SQ_MAX_GUIDE_STATES), [1] W = ceil(V/32), [2] E = n_edges (<= SQ_MAX_GUIDE_EDGES), [3] V;
+ *     default_next[n] at word SQ_GUIDE_HEADER (-1 = none); edge_off[n + 1] (edge_off[0] = 0, edge_off[n] = E); edge_id[E],
+ *     ascending within each state's range [edge_off[s], edge_off[s+1]); edge_next[E]; then one allowed bitmask of W words
+ *     per state (id t allowed in state s when bit t & 31 of mask word [s][t >> 5] is set; sq_logit_bias_rows_batch's
+ *     layout).  The blob is consistent: the mask of s is exactly its edge ids, plus, when default_next[s] >= 0, the ids
+ *     with no edge that the guide's default allows; every next state is in [0, n).  Masks dominate the size:
+ *     n * W * 4 bytes, 16 KB per state at V = 128256.
+ *   step(s, t): -1 when s < 0, t is outside [0, V) or the mask of s does not allow t; else edge_next of t's edge in s
+ *   when t has one, else default_next[s].
+ *   State words of a guided sequence (SQ_ST_GUIDED nonzero): SQ_ST_GUIDE_STATE = the state after the committed tokens
+ *   (the guide's start for a new prompt), SQ_ST_GUIDE_POS = the position of the first token not yet consumed (the
+ *   prompt length for a new prompt).
+ * A sequence that is frozen, or whose SQ_ST_GUIDED word is 0 or guide_table[b] is 0, is left alone by all three calls.
+ * Each is one PDL-chained launch; bad arguments are refused with SQ_ERR_INVALID_ARG before any launch (a null array, B
+ * outside 1..SQ_MAX_BATCH, V not a multiple of 8 in 8..131072, and the checks named below).
+ *
+ * sq_guide_states_batch: node_state[b*S + k] (int32, (B, S)) = the state of node k of sequence b: the walk of step()
+ * from state[b][SQ_ST_GUIDE_STATE] (node 0, the root) through the tokens at slots P-1+j of node k's ancestors-or-self
+ * j >= 1 (the bits of row k of tree_bits, in slot order), P = state[b][SQ_ST_P]; -1 from the first disallowed id on.
+ * depth: (S,) int32, node indices increasing along every path.  Grid (B).  Refused also: S outside 1..1024, tree_words !=
+ * ceil(S/32), ld_seq < 1.
+ *
+ * sq_guide_mask_rows_batch: in place on the (B*S, V) target rows (row b*S + k = node k, pitch ld >= V), right after
+ * sq_ban_tokens_rows_batch: with s = node_state[b*S + k], every entry whose id state s does not allow becomes -inf
+ * (0xFC00), NaN and +inf included, and every entry of the row when s < 0; allowed entries stay bit-identical.  Rows from
+ * B*S on are never touched.  Grid (ceil(V/4096), S, B).  Refused also: ld < V, S < 1.
+ *
+ * sq_guide_advance_batch: after the walk, moves state[b][SQ_ST_GUIDE_STATE] by step() through tokens[b][pos .. n), pos
+ * = state[b][SQ_ST_GUIDE_POS], n = the step's committed length (a + 1 when !SQ_ST_TERMINAL and a < M, else a; a =
+ * SQ_ST_ACCEPT_LEN, M = SQ_ST_M or ld_seq when 0; SQ_ST_END when SQ_ST_FINISH is set), then sets SQ_ST_GUIDE_POS = n.  On
+ * a disallowed id at position q it sets SQ_ST_GUIDE_STATE = -1 and SQ_ST_GUIDE_POS = q: tokens[b][:q] is the longest
+ * prefix the guide accepts.  A dead sequence (SQ_ST_GUIDE_STATE < 0) is left alone.  Grid (B) of one warp.  Refused
+ * also: ld_seq < 1. */
+#define SQ_MAX_GUIDE_STATES 4096
+#define SQ_MAX_GUIDE_EDGES (1 << 20)
+#define SQ_GUIDE_HEADER 4
+int sq_guide_states_batch(const int64_t* guide_table, const int64_t* tokens, int64_t ld_seq, const int32_t* state,
+                          const int32_t* depth, const uint32_t* tree_bits, int tree_words, int S, int V,
+                          int32_t* node_state, int B, void* stream);
+int sq_guide_mask_rows_batch(sq_half* logits, int64_t ld, int V, int S, const int32_t* state,
+                             const int64_t* guide_table, const int32_t* node_state, int B, void* stream);
+int sq_guide_advance_batch(const int64_t* guide_table, const int64_t* tokens, int64_t ld_seq, int32_t* state, int V,
+                           int B, void* stream);
 /* Per-sequence logprobs of the committed tokens (csrc/sq_logprobs.cu), after the walk, from the (B*S, V) target rows as the
  * walk read them (penalised, top-k and top-p filtered; row pitch ld >= V, a multiple of 8).  With P = state[b][SQ_ST_P_OLD],
  * n_new = state[b][SQ_ST_N_NEW], a = P + n_new and M = state[b][SQ_ST_M] (ld_seq when 0), the step committed position

@@ -27,6 +27,10 @@ SQ_MAX_LOGPROBS = 20
 SQ_MAX_LOGIT_BIAS = 1024
 # per-sequence bad words: the most words sq_ban_tokens_rows_batch holds per sequence, and the most ids per word
 SQ_MAX_BAD_WORDS, SQ_MAX_BAD_WORD_LEN = 128, 16
+# guided decoding: the state words of a guided sequence, the largest guide, and the guide blob's header words
+SQ_ST_GUIDED, SQ_ST_GUIDE_STATE, SQ_ST_GUIDE_POS = 12, 13, 14
+SQ_MAX_GUIDE_STATES, SQ_MAX_GUIDE_EDGES = 4096, 1 << 20
+SQ_GUIDE_HEADER = 4
 
 i32, i64, f32, vp = C.c_int, C.c_int64, C.c_float, C.c_void_p
 
@@ -125,6 +129,9 @@ _SIGNATURES = {
     "sq_token_logprobs_batch": (i32, [vp, i64, i32, i32, i32, vp, i64, vp, vp, i64, vp, vp, vp, vp, vp, vp, i32, vp]),
     "sq_logit_bias_rows_batch": (i32, [vp, i64, i32, i32, vp, vp, i64, vp, vp, vp, vp, i32, vp]),
     "sq_ban_tokens_rows_batch": (i32, [vp, i64, i32, vp, i64, vp, vp, vp, vp, i32, i32, vp, vp, vp, vp, vp, i32, vp]),
+    "sq_guide_states_batch": (i32, [vp, vp, i64, vp, vp, vp, i32, i32, i32, vp, i32, vp]),
+    "sq_guide_mask_rows_batch": (i32, [vp, i64, i32, i32, vp, vp, vp, i32, vp]),
+    "sq_guide_advance_batch": (i32, [vp, vp, i64, vp, i32, i32, vp]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

@@ -63,6 +63,17 @@ node's position, whose row did not draw it; DESIGN.md §3a).  A row can still lo
 "nan"), a greedy one commits id 0, the argmax of an all -inf row.  While every sequence is neutral (no words,
 min_tokens 0) nothing is allocated or launched; the first non-neutral setting, at construction or admission, captures
 the steady and post graphs once more, and the kernel then stays in them.
+
+Guided decoding (structured output): each sequence has a guide, a TokenGuide (sequoia_b200.guide) or None.  The guide's
+state after the committed tokens lives in state word SQ_ST_GUIDE_STATE and advances on the device after each walk
+(sq_guide_advance_batch).  In the accept step, after the ban, sq_guide_states_batch walks it down every tree path and
+sq_guide_mask_rows_batch sets every id that a row's state does not allow to -inf, so the greedy walk and the filters
+read the constrained rows.  A guided "spec" sequence gathers its accepted tokens before the walk writes the bonus token,
+so each committed token is the one its row drew, on a branching tree too.  A sequence that still commits an id its
+guide does not allow (a greedy one commits id 0 from a row with no finite entry) ends there with finish_reason "guide".
+While no sequence has a guide nothing is allocated or launched; the first guide, at construction or admission,
+allocates the (B,) table of blob addresses and captures the steady and post graphs once more.  Later admissions, with
+guides of any size, rewrite one table entry.
 """
 from __future__ import annotations
 
@@ -74,11 +85,13 @@ from typing import Dict, List, Mapping, Optional, Sequence, Union
 import torch
 
 from . import _lib, ops
+from .guide import TokenGuide
 from .tree import _Static, check_vocab
 
 F16 = torch.float16
 ST_P, ST_M, ST_FROZEN = 0, 8, 9
 ST_FINISH, ST_END = _lib.SQ_ST_FINISH, _lib.SQ_ST_END
+ST_GUIDED, ST_GUIDE_STATE, ST_GUIDE_POS = _lib.SQ_ST_GUIDED, _lib.SQ_ST_GUIDE_STATE, _lib.SQ_ST_GUIDE_POS
 MAX_STOP = _lib.SQ_MAX_STOP
 PENALTY_MAX_LEN = _lib.SQ_PENALTY_MAX_LEN
 MAX_LOGPROBS = _lib.SQ_MAX_LOGPROBS
@@ -90,7 +103,7 @@ FP16_MAX = 65504.0
 INT32_MAX = (1 << 31) - 1
 POLICIES = ("spec", "greedy")
 _PREVIOUS = object()        # admit(): keep the slot's previous stop set / budget / logprobs / logit bias / allowed set /
-                            # bad words / min_tokens
+                            # bad words / min_tokens / guide
 
 
 def draw_random(prompts: Sequence[torch.Tensor], M: int, S: int, V: int):
@@ -460,6 +473,23 @@ def is_neutral_ban(bad_words: Optional[tuple], min_tokens: int) -> bool:
     return not bad_words and min_tokens == 0
 
 
+def check_guide(guide) -> Optional[TokenGuide]:
+    """A guide: None or a TokenGuide."""
+    if guide is not None and not isinstance(guide, TokenGuide):
+        raise ValueError(f"guide must be None or a TokenGuide, got {guide!r}")
+    return guide
+
+
+def _guides(guide, B: int) -> List[Optional[TokenGuide]]:
+    """One guide (None or a TokenGuide) for all B sequences, or a sequence of B of them."""
+    if isinstance(guide, Sequence) and not isinstance(guide, (str, bytes)):
+        vals = [check_guide(g) for g in guide]
+        if len(vals) != B:
+            raise ValueError(f"guide: {len(vals)} values for {B} sequences")
+        return vals
+    return [check_guide(guide)] * B
+
+
 def check_seed(seed) -> int:
     """A per-sequence seed: an integer in [0, 2^64)."""
     if isinstance(seed, bool) or not isinstance(seed, numbers.Integral):
@@ -511,7 +541,11 @@ class BatchTree:
     output then never contains a word: its last id is banned wherever its other ids end the generated tokens (a one-token
     word everywhere; a word never matches across the prompt).  min_tokens: an integer >= 0 (at most max_new_tokens), for
     all sequences or one per prompt: the sequence's end ids are banned until it has generated that many tokens.  Both
-    policies honour both (module docstring, include/sequoia_b200.h)."""
+    policies honour both (module docstring, include/sequoia_b200.h).
+    guide: None or a TokenGuide (sequoia_b200.guide), for all sequences or one per prompt: every generated token is one
+    the guide allows in its current state.  The guide does not end a sequence; its end ids do.  A guide is refused when
+    one of its states allows no id that the sequence may generate (within its allowed_token_ids and without its
+    one-token bad_words).  Both policies honour it; guide_state(b) gives the slot's state after its committed tokens."""
 
     def __init__(self, draft, target, prompts: Sequence[torch.Tensor], grow_map: dict,
                  policy: Union[str, Sequence[str]] = "spec",
@@ -524,8 +558,9 @@ class BatchTree:
                  presence_penalty: Union[float, Sequence[float]] = 0.0,
                  logprobs: Union[None, int, Sequence[Optional[int]]] = None,
                  logit_bias=None, allowed_token_ids=None, min_p: Union[float, Sequence[float]] = 0.0,
-                 bad_words=None, min_tokens: Union[int, Sequence[int]] = 0):
+                 bad_words=None, min_tokens: Union[int, Sequence[int]] = 0, guide=None):
         B = len(prompts)
+        guides = _guides(guide, B)
         policies = _policies(policy, B)
         min_ps = _min_ps(min_p, B)
         words, min_toks = _bad_words(bad_words, B), _min_tokens(min_tokens, B)
@@ -576,11 +611,19 @@ class BatchTree:
         for b in range(B):
             check_min_tokens(min_toks[b], budgets[b])
             check_bannable(V, words[b], alloweds[b], min_toks[b], end_ids(stops[b], stop_mode))
+            if guides[b] is not None:
+                guides[b].check(V, alloweds[b], words[b])
         M = max_length
         for p in prompts:
             if len(p) + S - 1 > M:
                 raise ValueError(f"max_length={M} must hold the prompt ({len(p)}) + tree ({S}) - 1")
         self.device = dev
+        # guides: each slot's blob address in a (B,) device table (0 = none), read by the three guide kernels inside the
+        # captured graphs, which they join the first time a slot has a guide; the host keeps the blobs alive
+        self.guides = guides
+        self.use_guide = False
+        self.guide_table_dev = self.guide_scratch = None
+        self.guide_blobs: List[Optional[torch.Tensor]] = [None] * B
         # sampling parameters live on the device, so the captured graphs serve any values an admission brings; the top-p
         # filter joins the steady / post graphs only once a sequence has had top_p < 1 (one recapture, see admit)
         # (a greedy sequence's top_p is 1 on the device, so the filter leaves its rows alone)
@@ -683,6 +726,8 @@ class BatchTree:
             self.r, self.rand = r.to(dev), rand.to(dev)
         if any(n is not None for n in lps):
             self._start_logprobs()
+        if any(g is not None for g in guides):
+            self._start_guide()
         for b, p in enumerate(prompts):
             self._load_prompt(b, p)
         with torch.inference_mode():
@@ -770,6 +815,39 @@ class BatchTree:
         starts with a recapture, which takes the new array into the graphs."""
         return self.stop_ids_dev if self.use_stop else self.default_end_dev
 
+    def _start_guide(self):
+        """The guide kernels join op_accept and seq_post, with the blob table and the node-state scratch (rewritten every
+        step before it is read, so not one of the captured buffers)."""
+        self.use_guide = True
+        self.guide_table_dev = torch.zeros(self.B, dtype=torch.int64, device=self.device)
+        self.guide_scratch = torch.zeros(self.B, self.S, dtype=torch.int32, device=self.device)
+        for b in range(self.B):
+            self._write_guide(b)
+
+    def _write_guide(self, b: int):
+        """Slot b's blob and table entry from its host guide: a slot whose guide another slot already holds shares that
+        slot's blob; the old blob is released (the stream orders its reuse after the kernels that read it)."""
+        g = self.guides[b]
+        blob = None
+        if g is not None:
+            blob = next((self.guide_blobs[o] for o in range(self.B) if o != b and self.guides[o] is g
+                         and self.guide_blobs[o] is not None), None)
+            if blob is None:
+                blob = g.pack(self.V).to(self.device, non_blocking=False)
+        self.guide_blobs[b] = blob
+        self.guide_table_dev[b] = 0 if blob is None else blob.data_ptr()
+
+    def guide_state(self, b: int) -> int:
+        """Slot b's guide state after its committed tokens, from the host copy of the state words of its last verify()
+        (the guide's start before its first one); -1 once a token has left the guide.  Refused for a slot without a
+        guide."""
+        if not 0 <= b < self.B:
+            raise IndexError(f"slot {b} out of range for a batch of {self.B}")
+        g = self.guides[b]
+        if g is None:
+            raise ValueError(f"slot {b} has no guide (guide=None)")
+        return g.start if self.last[b] is None else int(self.host_state[b, ST_GUIDE_STATE])
+
     def _load_prompt(self, b: int, prompt: torch.Tensor):
         """Row b of tokens, position ids, state and accept_idx for a new prompt: nothing of an earlier occupant stays."""
         P, S, M = len(prompt), self.S, self.M
@@ -778,6 +856,9 @@ class BatchTree:
         pos[P:P + S - 1] = self.st.depth_cpu[1:] + P - 1
         st0 = torch.zeros(16, dtype=torch.int32)
         st0[ST_P], st0[ST_M] = P, M
+        g = self.guides[b]
+        if g is not None:
+            st0[ST_GUIDED], st0[ST_GUIDE_STATE], st0[ST_GUIDE_POS] = 1, g.start, P
         self.tokens[b].zero_()
         self.tokens[b, :P].copy_(_h2d(prompt), non_blocking=True)
         self.position_ids[b].copy_(_h2d(pos), non_blocking=True)
@@ -802,7 +883,7 @@ class BatchTree:
               stop_tokens=_PREVIOUS, max_new_tokens=_PREVIOUS, repetition_penalty: Optional[float] = None,
               frequency_penalty: Optional[float] = None, presence_penalty: Optional[float] = None,
               logprobs=_PREVIOUS, logit_bias=_PREVIOUS, allowed_token_ids=_PREVIOUS, min_p: Optional[float] = None,
-              bad_words=_PREVIOUS, min_tokens=_PREVIOUS):
+              bad_words=_PREVIOUS, min_tokens=_PREVIOUS, guide=_PREVIOUS):
         """Start `prompt` in the frozen slot b (finished, out of room, or stopped with freeze), at its own policy,
         temperature, top_p and top_k (default: the slot's previous values).  The next verify() runs its first verify next
         to the steady sequences.  The slot draws r and rand as a lone SpecTree on the prompt would, and runs its draft
@@ -827,7 +908,9 @@ class BatchTree:
         none).  The first non-neutral one, in a tree without one, captures the steady and post graphs once more.
         bad_words / min_tokens: the prompt's bad words (None is none) and min_tokens (default: the slot's previous ones);
         min_tokens counts from this prompt.  The first non-neutral one, in a tree without one, captures the steady and post
-        graphs once more."""
+        graphs once more.
+        guide: the prompt's guide (default: the slot's previous one; None is none), which starts at its start state.  The
+        first guide, in a tree without one, captures the steady and post graphs once more."""
         if policy is not None:
             check_policy(policy)
         if top_k is not None:
@@ -851,6 +934,8 @@ class BatchTree:
             bad_words = check_bad_words(bad_words, self.V)
         if min_tokens is not _PREVIOUS:
             min_tokens = check_min_tokens(min_tokens)
+        if guide is not _PREVIOUS:
+            guide = check_guide(guide)
         if not 0 <= b < self.B:
             raise IndexError(f"slot {b} out of range for a batch of {self.B}")
         if not self.frozen[b]:
@@ -879,8 +964,11 @@ class BatchTree:
         words = self.bad_words[b] if bad_words is _PREVIOUS else bad_words
         m = self.min_tokens[b] if min_tokens is _PREVIOUS else min_tokens
         check_min_tokens(m, budget)
-        check_bannable(self.V, words, self.allowed_token_ids[b] if allowed_token_ids is _PREVIOUS else allowed_token_ids,
-                       m, end_ids(stop, self.use_stop or stop is not None or budget is not None))
+        allowed = self.allowed_token_ids[b] if allowed_token_ids is _PREVIOUS else allowed_token_ids
+        check_bannable(self.V, words, allowed, m, end_ids(stop, self.use_stop or stop is not None or budget is not None))
+        gd = self.guides[b] if guide is _PREVIOUS else guide
+        if gd is not None:
+            gd.check(self.V, allowed, words)
         # (every other slot holds the tree's one policy until then, so a different one means both are present; at B = 1
         # it is a switch, which the single-policy graphs do not serve either)
         enter_mixed = not self.mixed and pol != ("greedy" if self.greedy else "spec")
@@ -947,6 +1035,13 @@ class BatchTree:
             self._start_ban()                      # the ban kernel enters op_accept: capture steady and post once more
             for name in ("steady", "post"):
                 self.graphs.pop(name, None)
+        self.guides[b] = gd
+        if self.use_guide:
+            self._write_guide(b)
+        elif gd is not None:
+            self._start_guide()                    # the guide kernels enter the graphs: capture steady and post once more
+            for name in ("steady", "post"):
+                self.graphs.pop(name, None)
         if pol == "spec" and self.r is None:       # the first sampling sequence of a tree built all-greedy
             self.r = torch.zeros(self.B, self.M, dtype=F16, device=self.device)
             self.rand = torch.zeros(self.B, self.S, self.V, dtype=F16, device=self.device)
@@ -1002,6 +1097,9 @@ class BatchTree:
 
     def op_accept(self):
         st = self.st
+        if self.use_guide:                         # the node states first: they read the tree tokens only
+            ops.guide_states_batch(self.guide_table_dev, self.tokens, self.state, st.depth, st.tree_bits, st.tree_words,
+                                   self.S, self.V, self.guide_scratch)
         if self.use_logit_bias:                    # first: a bias is in logit space, the penalties then scale it
             ops.logit_bias_rows_batch_(self.target_logits, self.S, self.state, self.allowed_dev, self.has_mask_dev,
                                        self.bias_ids_dev, self.bias_vals_dev, self.n_bias_dev)
@@ -1009,6 +1107,8 @@ class BatchTree:
             ops.ban_tokens_rows_batch_(self.target_logits, self.tokens, self.state, self.prompt_len_dev, st.depth,
                                        st.tree_bits, st.tree_words, self.S, self.words_dev, self.word_len_dev,
                                        self.n_words_dev, self.min_end_dev, self._ban_end_ids())
+        if self.use_guide:                         # -inf whatever the bias and the ban; the penalties leave -inf alone
+            ops.guide_mask_rows_batch_(self.target_logits, self.S, self.state, self.guide_table_dev, self.guide_scratch)
         if self.use_penalty:                       # first: the greedy walk and the filters rank the penalised rows
             ops.penalize_rows_batch_(self.target_logits, self.tokens, self.state, self.prompt_len_dev, st.tree_bits,
                                      st.tree_words, self.S, self.rep_dev, self.freq_dev, self.pres_dev, self.pen_scratch)
@@ -1081,6 +1181,8 @@ class BatchTree:
 
     def seq_post(self):
         self.op_accept()
+        if self.use_guide:                         # the committed tokens through the guide, before the host-state copy
+            ops.guide_advance_batch(self.guide_table_dev, self.tokens, self.state, self.V)
         if self.use_logprobs:                      # the rows as the walk read them, before anything else writes them
             self.op_logprobs()
         self.op_kv_gather()
@@ -1179,7 +1281,11 @@ class BatchTree:
                 continue
             a, terminal, skipped = int(hs[b, 1]), bool(hs[b, 2]), bool(hs[b, 7])
             finish = int(hs[b, ST_FINISH])          # (always 0 in default mode: only the stop walks write it)
-            if finish:
+            if self.guides[b] is not None and int(hs[b, ST_GUIDE_STATE]) < 0:
+                valid = self.tokens[b, :int(hs[b, ST_GUIDE_POS])]     # the longest prefix the guide accepts
+                terminal = True
+                self.finish_reason[b] = "guide"
+            elif finish:
                 valid = self.tokens[b, :int(hs[b, ST_END])]
                 terminal = True
                 self.finish_reason[b] = "stop" if finish == 1 else "length"

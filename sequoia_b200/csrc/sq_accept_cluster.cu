@@ -294,8 +294,10 @@ __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(CNT) accept_stochas
   }
   if (cx.rank != 0) return;
   __syncthreads();
-  finish_verify(sh_acc, n_new, P, terminal, nan_flag, bonus, true, depth, S, tokens, position_ids, accept_idx, state,
-                max_target_seq);
+  // a guided sequence gathers its accepted slots before it writes the bonus, so its committed tokens stay in its guide
+  const bool bonus_first = !(BATCH && state[ST_GUIDED]);
+  finish_verify(sh_acc, n_new, P, terminal, nan_flag, bonus, bonus_first, depth, S, tokens, position_ids, accept_idx,
+                state, max_target_seq);
   if constexpr (STOP) stop_cut(sh_stop, n_new, P, terminal, tokens, state, max_target_seq);
 }
 

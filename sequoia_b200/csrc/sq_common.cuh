@@ -68,6 +68,9 @@ enum StateWord : int {
   ST_FROZEN = 9,     // batched entry points only: nonzero = finished sequence, its tokens / state / KV rows are not written
   ST_FINISH = 10,    // *_batch_stop walks only: 1 = a stop id ended the sequence, 2 = its length limit, 0 = neither
   ST_END = 11,       // *_batch_stop walks only: the sequence's final length when ST_FINISH != 0, else 0
+  ST_GUIDED = 12,    // batched entry points only, host-written: nonzero = the sequence follows a token guide
+  ST_GUIDE_STATE = 13, // guided sequences: the guide state after the committed tokens (-1 = a token left the guide)
+  ST_GUIDE_POS = 14,   // guided sequences: the tokens before this position have been consumed by the guide
   ST_WORDS = 16
 };
 

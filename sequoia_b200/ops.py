@@ -898,3 +898,78 @@ def ban_tokens_rows_batch_(logits, tokens, state, prompt_len, depth, tree_bits, 
                                                ptr(tree_bits), tree_words, S, ptr(words), ptr(word_len), ptr(n_words),
                                                ptr(min_end), ptr(end_ids), B, stream_ptr()), "sq_ban_tokens_rows_batch")
     return logits
+
+
+# ---- guided decoding: per-sequence token automata (csrc/sq_guide.cu; semantics in include/sequoia_b200.h) ----------------
+def _guide_table(guide_table, B, name):
+    if guide_table is None or guide_table.dtype != torch.int64 or not guide_table.is_cuda or guide_table.dim() != 1 \
+            or guide_table.shape[0] < B or guide_table.stride(0) != 1:
+        raise TypeError(f"{name}: guide_table must be a contiguous ({B},) int64 CUDA tensor of guide blob addresses")
+
+
+def guide_states_batch(guide_table, tokens, state, depth, tree_bits, tree_words: int, S: int, V: int, node_state):
+    """node_state[b, k] = the guide state of node k of every guided sequence b: its committed state (state word
+    SQ_ST_GUIDE_STATE) walked through the tokens of node k's path on the tree (tree_bits), -1 from a disallowed id on.
+    guide_table: (B,) int64 blob addresses (0 = none); tokens (B, ld_seq) int64; depth (S,) int32; node_state (B, S)
+    int32; all on the device.  Unguided and frozen sequences' entries are not written."""
+    name = "guide_states_batch"
+    _need(state, torch.int32, name)
+    _need(tokens, torch.int64, name)
+    _need(tree_bits, torch.int32, name)
+    _need(node_state, torch.int32, name)
+    if not state.is_contiguous() or not tree_bits.is_contiguous():
+        raise ValueError(f"{name}: state and tree_bits must be contiguous")
+    B = state.shape[0]
+    _guide_table(guide_table, B, name)
+    if tokens.shape[0] < B:
+        raise ValueError(f"{name}: {tokens.shape[0]} token rows for {B} sequences")
+    if depth is None or depth.dtype != torch.int32 or not depth.is_cuda or depth.dim() != 1 or depth.shape[0] < S \
+            or depth.stride(0) != 1:
+        raise TypeError(f"{name}: depth must be a contiguous ({S},) int32 CUDA tensor")
+    if tuple(node_state.shape) != (B, S) or not node_state.is_contiguous():
+        raise ValueError(f"{name}: node_state must be a contiguous ({B}, {S}) tensor, got {tuple(node_state.shape)}")
+    check(_lib.load().sq_guide_states_batch(ptr(guide_table), ptr(tokens), _rows(tokens, "tokens"), ptr(state),
+                                            ptr(depth), ptr(tree_bits), tree_words, S, V, ptr(node_state), B,
+                                            stream_ptr()), "sq_guide_states_batch")
+    return node_state
+
+
+def guide_mask_rows_batch_(logits, S: int, state, guide_table, node_state):
+    """Write -inf in place at every id the node's guide state does not allow (every id for a dead node, -1) in the S
+    target rows b*S .. b*S+S-1 of every guided sequence b of the (>= B*S, V) fp16 logits; allowed entries are not
+    touched.  node_state: (B, S) int32 from guide_states_batch."""
+    name = "guide_mask_rows_batch_"
+    _need(logits, F16, name)
+    if logits.dim() != 2 or logits.stride(-1) != 1:
+        raise ValueError(f"{name}: logits must be (rows, V) with contiguous rows, got {tuple(logits.shape)}")
+    _need(state, torch.int32, name)
+    _need(node_state, torch.int32, name)
+    if not state.is_contiguous():
+        raise ValueError(f"{name}: state must be contiguous")
+    B = state.shape[0]
+    _guide_table(guide_table, B, name)
+    if logits.shape[0] < B * S:
+        raise ValueError(f"{name}: {logits.shape[0]} logit rows for {B} sequences of {S}")
+    if tuple(node_state.shape) != (B, S) or not node_state.is_contiguous():
+        raise ValueError(f"{name}: node_state must be a contiguous ({B}, {S}) tensor, got {tuple(node_state.shape)}")
+    check(_lib.load().sq_guide_mask_rows_batch(ptr(logits), logits.stride(0), logits.shape[1], S, ptr(state),
+                                               ptr(guide_table), ptr(node_state), B, stream_ptr()),
+          "sq_guide_mask_rows_batch")
+    return logits
+
+
+def guide_advance_batch(guide_table, tokens, state, V: int):
+    """After the walk: move every guided sequence's committed guide state (state word SQ_ST_GUIDE_STATE) through the
+    tokens the step committed, from position SQ_ST_GUIDE_POS on; a disallowed id kills it (-1) and leaves its position in
+    SQ_ST_GUIDE_POS."""
+    name = "guide_advance_batch"
+    _need(state, torch.int32, name)
+    _need(tokens, torch.int64, name)
+    if not state.is_contiguous():
+        raise ValueError(f"{name}: state must be contiguous")
+    B = state.shape[0]
+    _guide_table(guide_table, B, name)
+    if tokens.shape[0] < B:
+        raise ValueError(f"{name}: {tokens.shape[0]} token rows for {B} sequences")
+    check(_lib.load().sq_guide_advance_batch(ptr(guide_table), ptr(tokens), _rows(tokens, "tokens"), ptr(state), V, B,
+                                             stream_ptr()), "sq_guide_advance_batch")
