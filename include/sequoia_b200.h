@@ -369,7 +369,13 @@ int sq_sample_level_batch(const sq_half* logits, int64_t ld_logits, const int32_
 /* one walk (one 8-CTA cluster) per sequence; target_logits (B*S, V).  Every batched stochastic walk (this one and its
  * _per_seq, _mixed and _stop forms) writes the bonus token at slot a before it gathers the accepted slots, as SpecTree
  * does, except for a sequence whose SQ_ST_GUIDED word is nonzero: that one gathers first and then writes the bonus, as
- * GreedyTree does, so every committed token is the token its own row drew. */
+ * GreedyTree does, so every committed token is the token its own row drew.
+ * SQ_ACCEPT_SKIP_DEAD (policy bit of the _per_seq, _mixed and _stop forms only; refused elsewhere): the walk for draft
+ * rows processed by sq_draft_rows_batch.  A child whose token's entry in its parent's raw draft row (before the
+ * temperature) is -inf (0xFC00) is dead: it is never accepted and leaves p and q exactly as they were, and the walk
+ * moves on to the next sibling.  Without it such a child, once q's support is used up, turns q and then the residual
+ * into NaN and ends the sequence by the NaN flag. */
+#define SQ_ACCEPT_SKIP_DEAD 8
 int sq_accept_stochastic_batch(const sq_half* target_logits, int64_t ld_t, const sq_half* draft_logits, int64_t ld_d,
                                const int32_t* row_base, const int32_t* row_step, const sq_half* r, const sq_half* noise,
                                int64_t ld_noise, const int32_t* succ_off, const int32_t* succ, const int32_t* depth, int S,
@@ -583,6 +589,37 @@ int sq_guide_mask_rows_batch(sq_half* logits, int64_t ld, int V, int S, const in
                              const int64_t* guide_table, const int32_t* node_state, int B, void* stream);
 int sq_guide_advance_batch(const int64_t* guide_table, const int64_t* tokens, int64_t ld_seq, int32_t* state, int V,
                            int B, void* stream);
+/* Constrained drafting (csrc/sq_draft_rows.cu): the processing of sq_logit_bias_rows_batch, sq_ban_tokens_rows_batch and
+ * sq_guide_mask_rows_batch applied, in that order and bit for bit as they define it, to the draft rows of nodes
+ * [k0, k0 + nk) of every sequence, in place (draft row of node k, sequence b: row_base[k] + b * row_step[k], pitch
+ * ld >= V).  A draft row of node k is the distribution of the token after node k, the same context as target row k, so
+ * it gets the same treatment: row k's context is the committed tokens plus node k's tree path, its token lands at
+ * position P + depth[k], and its guide state is node k's.  flags selects the kinds (a nonzero set); the arrays of a kind
+ * that is not selected are not read and may be NULL:
+ *   SQ_DRAFT_BIAS: allowed, allowed_words, has_mask, bias_ids, bias_vals, n_bias as sq_logit_bias_rows_batch takes them;
+ *   SQ_DRAFT_BAN: tokens, ld_seq, tree_bits, tree_words, prompt_len, depth, words, word_len, n_words, min_end, end_ids as
+ *     sq_ban_tokens_rows_batch takes them;
+ *   SQ_DRAFT_GUIDE: tokens, ld_seq, tree_bits, tree_words and guide_table as sq_guide_states_batch takes them, and
+ *     node_state ((B, S) int32): the state of node k is one step() from node_state[b*S + parent(k)] by the token at slot
+ *     P-1+k (the root's is state[b][SQ_ST_GUIDE_STATE]); the call writes it to node_state[b*S + k] and masks the row
+ *     with it.  So the parent of every node in the range must lie below k0 and have been processed by an earlier call
+ *     (a tree level at a time, the root first).
+ * A frozen sequence, and one whose selected kinds are all neutral (no mask, n_bias <= 0, n_words <= 0, min_end <= 0, no
+ * guide), has its rows left byte-identical, as have all rows outside the range.  One PDL-chained launch, grid
+ * (ceil(V/4096), nk, B) of 256 threads.  Refused with SQ_ERR_INVALID_ARG before any launch: flags empty or with unknown
+ * bits, a null array of a selected kind (or of draft_logits, row_base, row_step, state), B outside 1..SQ_MAX_BATCH, V not
+ * a multiple of 8 in 8..131072, ld < V, S outside 1..1024 or tree_words != ceil(S/32), a node range that is neither the
+ * root alone (k0 = 0, nk = 1) nor within [1, S), allowed_words < ceil(V/32), ld_seq < 1. */
+#define SQ_DRAFT_BIAS 1
+#define SQ_DRAFT_BAN 2
+#define SQ_DRAFT_GUIDE 4
+int sq_draft_rows_batch(sq_half* draft_logits, int64_t ld, int V, const int32_t* row_base, const int32_t* row_step,
+                        int k0, int nk, int S, const int32_t* state, int flags, const uint32_t* allowed,
+                        int64_t allowed_words, const int32_t* has_mask, const int32_t* bias_ids, const float* bias_vals,
+                        const int32_t* n_bias, const int64_t* tokens, int64_t ld_seq, const uint32_t* tree_bits,
+                        int tree_words, const int32_t* prompt_len, const int32_t* depth, const int32_t* words,
+                        const int32_t* word_len, const int32_t* n_words, const int32_t* min_end, const int32_t* end_ids,
+                        const int64_t* guide_table, int32_t* node_state, int B, void* stream);
 /* Per-sequence logprobs of the committed tokens (csrc/sq_logprobs.cu), after the walk, from the (B*S, V) target rows as the
  * walk read them (penalised, top-k and top-p filtered; row pitch ld >= V, a multiple of 8).  With P = state[b][SQ_ST_P_OLD],
  * n_new = state[b][SQ_ST_N_NEW], a = P + n_new and M = state[b][SQ_ST_M] (ld_seq when 0), the step committed position

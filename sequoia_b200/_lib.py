@@ -31,6 +31,8 @@ SQ_MAX_BAD_WORDS, SQ_MAX_BAD_WORD_LEN = 128, 16
 SQ_ST_GUIDED, SQ_ST_GUIDE_STATE, SQ_ST_GUIDE_POS = 12, 13, 14
 SQ_MAX_GUIDE_STATES, SQ_MAX_GUIDE_EDGES = 4096, 1 << 20
 SQ_GUIDE_HEADER = 4
+# constrained drafting: the kinds sq_draft_rows_batch applies to draft rows
+SQ_DRAFT_BIAS, SQ_DRAFT_BAN, SQ_DRAFT_GUIDE = 1, 2, 4
 
 i32, i64, f32, vp = C.c_int, C.c_int64, C.c_float, C.c_void_p
 
@@ -132,6 +134,8 @@ _SIGNATURES = {
     "sq_guide_states_batch": (i32, [vp, vp, i64, vp, vp, vp, i32, i32, i32, vp, i32, vp]),
     "sq_guide_mask_rows_batch": (i32, [vp, i64, i32, i32, vp, vp, vp, i32, vp]),
     "sq_guide_advance_batch": (i32, [vp, vp, i64, vp, i32, i32, vp]),
+    "sq_draft_rows_batch": (i32, [vp, i64, i32, vp, vp, i32, i32, i32, vp, i32, vp, i64, vp, vp, vp, vp, vp, i64, vp, i32,
+                                  vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, vp]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

@@ -74,6 +74,16 @@ guide does not allow (a greedy one commits id 0 from a row with no finite entry)
 While no sequence has a guide nothing is allocated or launched; the first guide, at construction or admission,
 allocates the (B,) table of blob addresses and captures the steady and post graphs once more.  Later admissions, with
 guides of any size, rewrite one table entry.
+
+Constrained drafting: with constrain_draft=True (tree-wide, default False) every draft row a sampler reads gets what its
+target row gets above, up to and including the guide mask: the allowed set and logit bias, the bad words and min_tokens
+of the node's context, and the guide mask of the node's state (sq_draft_rows_batch, in the draft graph: the root rows
+first, then each level whose nodes have children, one launch each).  The draft then proposes only tokens the target rows
+keep.  A child whose token is -inf in its parent's processed draft row is dead (a row with fewer finite entries than
+children, an all -inf row, or a NaN sampling key); the stochastic walks never accept one and leave the residual as it was
+(SQ_ACCEPT_SKIP_DEAD), so speculative sampling stays exact.  A seeded sequence commits a different, equally distributed
+output than without it; greedy sequences commit the same.  While every slot is neutral nothing is launched; when a
+constraint kind starts, the draft graph is captured once more along with the steady and post graphs.
 """
 from __future__ import annotations
 
@@ -545,7 +555,11 @@ class BatchTree:
     guide: None or a TokenGuide (sequoia_b200.guide), for all sequences or one per prompt: every generated token is one
     the guide allows in its current state.  The guide does not end a sequence; its end ids do.  A guide is refused when
     one of its states allows no id that the sequence may generate (within its allowed_token_ids and without its
-    one-token bad_words).  Both policies honour it; guide_state(b) gives the slot's state after its committed tokens."""
+    one-token bad_words).  Both policies honour it; guide_state(b) gives the slot's state after its committed tokens.
+    constrain_draft: a bool (default False), for the whole tree: the draft rows get each sequence's allowed set, logit
+    bias, bad words, min_tokens and guide as its target rows do, so the draft proposes only tokens the target rows keep,
+    and the walks skip the children those rows set to -inf (module docstring).  A seeded "spec" sequence then commits a
+    different, equally distributed output; admit() does not change it."""
 
     def __init__(self, draft, target, prompts: Sequence[torch.Tensor], grow_map: dict,
                  policy: Union[str, Sequence[str]] = "spec",
@@ -558,7 +572,9 @@ class BatchTree:
                  presence_penalty: Union[float, Sequence[float]] = 0.0,
                  logprobs: Union[None, int, Sequence[Optional[int]]] = None,
                  logit_bias=None, allowed_token_ids=None, min_p: Union[float, Sequence[float]] = 0.0,
-                 bad_words=None, min_tokens: Union[int, Sequence[int]] = 0, guide=None):
+                 bad_words=None, min_tokens: Union[int, Sequence[int]] = 0, guide=None, constrain_draft: bool = False):
+        if not isinstance(constrain_draft, bool):
+            raise ValueError(f"constrain_draft must be a bool, got {constrain_draft!r}")
         B = len(prompts)
         guides = _guides(guide, B)
         policies = _policies(policy, B)
@@ -618,6 +634,9 @@ class BatchTree:
             if len(p) + S - 1 > M:
                 raise ValueError(f"max_length={M} must hold the prompt ({len(p)}) + tree ({S}) - 1")
         self.device = dev
+        # constrained drafting: every draft row a sampler reads gets its sequence's allowed set, logit bias, bad words and
+        # guide, as its target row does, inside the draft graph; the walks then skip dead children (SQ_ACCEPT_SKIP_DEAD)
+        self.constrain_draft = constrain_draft
         # guides: each slot's blob address in a (B,) device table (0 = none), read by the three guide kernels inside the
         # captured graphs, which they join the first time a slot has a guide; the host keeps the blobs alive
         self.guides = guides
@@ -848,6 +867,16 @@ class BatchTree:
             raise ValueError(f"slot {b} has no guide (guide=None)")
         return g.start if self.last[b] is None else int(self.host_state[b, ST_GUIDE_STATE])
 
+    def _draft_processed(self) -> bool:
+        """Whether the draft graph processes draft rows: a constrained tree with at least one constraint kind started."""
+        return self.constrain_draft and (self.use_logit_bias or self.use_ban or self.use_guide)
+
+    def _start_kind(self):
+        """A constraint kind starts (its kernel joins op_accept): capture steady and post once more, and the draft graph
+        too in a constrained tree (its processing and the walks' dead-child rule enter)."""
+        for name in ("draft", "steady", "post") if self.constrain_draft else ("steady", "post"):
+            self.graphs.pop(name, None)
+
     def _load_prompt(self, b: int, prompt: torch.Tensor):
         """Row b of tokens, position ids, state and accept_idx for a new prompt: nothing of an earlier occupant stays."""
         P, S, M = len(prompt), self.S, self.M
@@ -1001,7 +1030,8 @@ class BatchTree:
         self.end_limit_dev[b] = _end_limit(P, budget)
         if (stop is not None or budget is not None) and not self.use_stop:
             self.use_stop = True                   # the stop walks replace the walks: capture steady and post once more
-            for name in ("steady", "post"):
+            # (and the draft graph when it bans end ids: they become the stop ids, as in the target rows)
+            for name in ("draft", "steady", "post") if self.constrain_draft and self.use_ban else ("steady", "post"):
                 self.graphs.pop(name, None)
         self.repetition_penalty[b], self.frequency_penalty[b], self.presence_penalty[b] = rep, freq, pres
         self.rep_dev[b], self.freq_dev[b], self.pres_dev[b] = rep, freq, pres
@@ -1026,22 +1056,19 @@ class BatchTree:
             self._write_logit_bias(b)
         elif not is_neutral_bias(self.logit_bias[b], self.allowed_token_ids[b]):
             self._start_logit_bias()               # the bias kernel enters op_accept: capture steady and post once more
-            for name in ("steady", "post"):
-                self.graphs.pop(name, None)
+            self._start_kind()
         self.bad_words[b], self.min_tokens[b] = words, m
         if self.use_ban:
             self._write_ban(b)
         elif not is_neutral_ban(words, m):
             self._start_ban()                      # the ban kernel enters op_accept: capture steady and post once more
-            for name in ("steady", "post"):
-                self.graphs.pop(name, None)
+            self._start_kind()
         self.guides[b] = gd
         if self.use_guide:
             self._write_guide(b)
         elif gd is not None:
             self._start_guide()                    # the guide kernels enter the graphs: capture steady and post once more
-            for name in ("steady", "post"):
-                self.graphs.pop(name, None)
+            self._start_kind()
         if pol == "spec" and self.r is None:       # the first sampling sequence of a tree built all-greedy
             self.r = torch.zeros(self.B, self.M, dtype=F16, device=self.device)
             self.rand = torch.zeros(self.B, self.S, self.V, dtype=F16, device=self.device)
@@ -1097,6 +1124,7 @@ class BatchTree:
 
     def op_accept(self):
         st = self.st
+        policy = ops.ACCEPT_SKIP_DEAD if self._draft_processed() else 0
         if self.use_guide:                         # the node states first: they read the tree tokens only
             ops.guide_states_batch(self.guide_table_dev, self.tokens, self.state, st.depth, st.tree_bits, st.tree_words,
                                    self.S, self.V, self.guide_scratch)
@@ -1148,17 +1176,17 @@ class BatchTree:
                                              self.noise, st.succ_off, st.succ, st.depth, self.S, self.T_dev,
                                              self.greedy_dev if self.mixed else None, self.stop_ids_dev,
                                              self.end_limit_dev, self.tokens, self.position_ids, self.accept_idx,
-                                             self.state, self.max_target_seq)
+                                             self.state, self.max_target_seq, policy)
             return
         if self.mixed:
             ops.accept_stochastic_batch_mixed(self.target_logits, self.draft_logits, self.row_base, self.row_step, self.r,
                                               self.noise, st.succ_off, st.succ, st.depth, self.S, self.T_dev,
                                               self.greedy_dev, self.tokens, self.position_ids, self.accept_idx, self.state,
-                                              self.max_target_seq)
+                                              self.max_target_seq, policy)
             return
         ops.accept_stochastic_batch_per_seq(self.target_logits, self.draft_logits, self.row_base, self.row_step, self.r,
                                             self.noise, st.succ_off, st.succ, st.depth, self.S, self.T_dev, self.tokens,
-                                            self.position_ids, self.accept_idx, self.state, self.max_target_seq)
+                                            self.position_ids, self.accept_idx, self.state, self.max_target_seq, policy)
 
     def op_kv_gather(self):
         md = max(self.st.max_depth, 1)
@@ -1170,10 +1198,29 @@ class BatchTree:
         self.draft.engine.runner.forward(1, self.tokens, self.position_ids, self.storage_ids, state=self.state, n0=0,
                                          kv_end=1, batch=True, logits_out=self.draft_logits[0:self.B], **self._mask_kw())
 
+    def op_draft_rows(self, k0: int, nk: int):
+        """The draft rows of nodes [k0, k0 + nk) of every sequence get the processing their target rows get in op_accept,
+        up to and including the guide mask (one launch)."""
+        st = self.st
+        ops.draft_rows_batch_(
+            self.draft_logits, self.row_base, self.row_step, k0, nk, self.S, self.state,
+            bias=(self.allowed_dev, self.has_mask_dev, self.bias_ids_dev, self.bias_vals_dev, self.n_bias_dev)
+            if self.use_logit_bias else None,
+            ban=(self.prompt_len_dev, st.depth, self.words_dev, self.word_len_dev, self.n_words_dev, self.min_end_dev,
+                 self._ban_end_ids()) if self.use_ban else None,
+            guide=(self.guide_table_dev, self.guide_scratch) if self.use_guide else None,
+            tokens=self.tokens, tree_bits=st.tree_bits, tree_words=st.tree_words)
+
     def seq_draft(self):
+        levels = self.st.levels
+        processed = self._draft_processed()
+        if processed:                              # the root row, from the bonus forward or an admission's draft prefill
+            self.op_draft_rows(0, 1)
         for i in range(self.st.draft_step - 1):
             self.op_sample(i)
             self.op_draft_level(i)
+            if processed and i + 1 < len(levels):  # a level whose nodes have children: before op_sample(i + 1) reads it
+                self.op_draft_rows(levels[i]["n0"], levels[i]["tb"])
 
     def op_logprobs(self):
         ops.token_logprobs_batch_(self.target_logits, self.S, self.st.max_depth, self.tokens, self.state, self.accept_idx,

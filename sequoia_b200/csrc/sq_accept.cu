@@ -350,7 +350,7 @@ static int accept_stochastic_batch(const char* name, const sq_half* target_logit
                                    const int32_t* stop_ids = nullptr, const int32_t* end_limit = nullptr) {
   SQ_CHECK_ARG(S >= 1 && S <= 1024, "%s: S=%d unsupported", name, S);
   SQ_CHECK_ARG(B >= 1 && B <= SQ_MAX_BATCH, "%s: B=%d (1..%d)", name, B, SQ_MAX_BATCH);
-  SQ_CHECK_ARG((policy & ~3) == 0, "%s: unknown policy bits %d", name, policy);
+  SQ_CHECK_ARG((policy & ~(T_seq ? 3 | SQ_ACCEPT_SKIP_DEAD : 3)) == 0, "%s: unknown policy bits %d", name, policy);
   SQ_CHECK_ARG(row_base && row_step, "%s: null draft-row table", name);
   SQ_CHECK_ARG(ld_acc >= S && ld_noise >= V, "%s: accept_idx / noise rows too short", name);
   BatchArgs ba{B, ld_seq, ld_noise, ld_acc, row_base, row_step, greedy, stop_ids, end_limit};

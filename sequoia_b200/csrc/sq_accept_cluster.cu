@@ -81,7 +81,9 @@ struct ClusterCtx {
 // nothing (its walk is the greedy kernel's).
 // STOP (PER_SEQ only): stop mode.  The fixed 0 / 2 end rule is compiled out; rank 0 then cuts the committed tokens at the
 // sequence's stop ids and length limit (ba.stop_ids / ba.end_limit, stop_cut) and writes ST_FINISH / ST_END.
-template <bool BATCH, int NCH, bool PER_SEQ = false, bool MIXED = false, bool STOP = false>
+// SKIP_DEAD (PER_SEQ only; policy bit SQ_ACCEPT_SKIP_DEAD): a child whose token is -inf in its parent's raw draft row is
+// dead and skipped: no test, no residual, q unchanged.  Every CTA reads the same fp16 word, so the skip is uniform.
+template <bool BATCH, int NCH, bool PER_SEQ = false, bool MIXED = false, bool STOP = false, bool SKIP_DEAD = false>
 __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(CNT) accept_stochastic_cluster_kernel(
     const __half* __restrict__ target_logits, int64_t ld_t, const __half* __restrict__ draft_logits, int64_t ld_d,
     const __half* __restrict__ r, const __half* __restrict__ noise, const int32_t* __restrict__ succ_off,
@@ -91,6 +93,7 @@ __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(CNT) accept_stochas
   static_assert(BATCH || !PER_SEQ, "per-sequence parameters need the batched kernel");
   static_assert(PER_SEQ || !MIXED, "a per-sequence policy needs the per-sequence temperature");
   static_assert(PER_SEQ || !STOP, "stop mode needs the per-sequence walk");
+  static_assert(PER_SEQ || !SKIP_DEAD, "dead children come from processed draft rows of a per-sequence batch");
   __shared__ Xch xch;
   __shared__ float red[CNW];
   __shared__ int32_t sh_acc[1024];
@@ -175,6 +178,10 @@ __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(CNT) accept_stochas
       const int child = succ[ci];
       const int slot = P - 1 + child;
       const int tok = (int)tokens[slot];
+      if constexpr (SKIP_DEAD) {
+        const __half raw = draft_logits[ba.row<BATCH>(cur, b) * ld_d + tok];
+        if (__half_as_ushort(raw) == 0xFC00u) continue;      // dead: p and q stay as they are
+      }
       const int tc = tok >> 3, te = tok & 7;
       // owner of the tested token: chunk own_i of this thread (-1: not this thread)
       int own_i;
@@ -305,37 +312,58 @@ __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(CNT) accept_stochas
 
 using namespace sq;
 
+template <int NCH, bool SKIP_DEAD>
+static int launch_accept_batch(const sq_half* target_logits, int64_t ld_t, const sq_half* draft_logits, int64_t ld_d,
+                               const sq_half* r, const sq_half* noise, const int32_t* succ_off, const int32_t* succ,
+                               const int32_t* depth, int S, int V, int64_t* tokens, int64_t* position_ids,
+                               int32_t* accept_idx, int32_t* state, int max_target_seq, int policy, void* stream,
+                               const BatchArgs* batch, const float* T_seq) {
+  if (batch->stop_ids) {
+    if (batch->greedy)
+      accept_stochastic_cluster_kernel<true, NCH, true, true, true, SKIP_DEAD>
+          <<<dim3(CL, batch->B), CNT, 0, (cudaStream_t)stream>>>(
+              (const __half*)target_logits, ld_t, (const __half*)draft_logits, ld_d, (const __half*)r,
+              (const __half*)noise, succ_off, succ, depth, S, V, T_seq, tokens, position_ids, accept_idx, state,
+              max_target_seq, policy, *batch);
+    else
+      accept_stochastic_cluster_kernel<true, NCH, true, false, true, SKIP_DEAD>
+          <<<dim3(CL, batch->B), CNT, 0, (cudaStream_t)stream>>>(
+              (const __half*)target_logits, ld_t, (const __half*)draft_logits, ld_d, (const __half*)r,
+              (const __half*)noise, succ_off, succ, depth, S, V, T_seq, tokens, position_ids, accept_idx, state,
+              max_target_seq, policy, *batch);
+    SQ_CHECK_LAUNCH("sq_accept_stochastic_batch_stop");
+    return SQ_OK;
+  }
+  if (batch->greedy) {
+    accept_stochastic_cluster_kernel<true, NCH, true, true, false, SKIP_DEAD>
+        <<<dim3(CL, batch->B), CNT, 0, (cudaStream_t)stream>>>(
+            (const __half*)target_logits, ld_t, (const __half*)draft_logits, ld_d, (const __half*)r, (const __half*)noise,
+            succ_off, succ, depth, S, V, T_seq, tokens, position_ids, accept_idx, state, max_target_seq, policy, *batch);
+    SQ_CHECK_LAUNCH("sq_accept_stochastic_batch_mixed");
+    return SQ_OK;
+  }
+  accept_stochastic_cluster_kernel<true, NCH, true, false, false, SKIP_DEAD>
+      <<<dim3(CL, batch->B), CNT, 0, (cudaStream_t)stream>>>(
+          (const __half*)target_logits, ld_t, (const __half*)draft_logits, ld_d, (const __half*)r, (const __half*)noise,
+          succ_off, succ, depth, S, V, T_seq, tokens, position_ids, accept_idx, state, max_target_seq, policy, *batch);
+  SQ_CHECK_LAUNCH("sq_accept_stochastic_batch_per_seq");
+  return SQ_OK;
+}
+
 template <int NCH>
 static int launch_accept_nch(const sq_half* target_logits, int64_t ld_t, const sq_half* draft_logits, int64_t ld_d,
                              const sq_half* r, const sq_half* noise, const int32_t* succ_off, const int32_t* succ,
                              const int32_t* depth, int S, int V, float T, int64_t* tokens, int64_t* position_ids,
                              int32_t* accept_idx, int32_t* state, int max_target_seq, int policy, void* stream,
                              const BatchArgs* batch, const float* T_seq) {
-  if (batch && T_seq && batch->stop_ids) {
-    if (batch->greedy)
-      accept_stochastic_cluster_kernel<true, NCH, true, true, true><<<dim3(CL, batch->B), CNT, 0, (cudaStream_t)stream>>>(
-          (const __half*)target_logits, ld_t, (const __half*)draft_logits, ld_d, (const __half*)r, (const __half*)noise,
-          succ_off, succ, depth, S, V, T_seq, tokens, position_ids, accept_idx, state, max_target_seq, policy, *batch);
-    else
-      accept_stochastic_cluster_kernel<true, NCH, true, false, true><<<dim3(CL, batch->B), CNT, 0, (cudaStream_t)stream>>>(
-          (const __half*)target_logits, ld_t, (const __half*)draft_logits, ld_d, (const __half*)r, (const __half*)noise,
-          succ_off, succ, depth, S, V, T_seq, tokens, position_ids, accept_idx, state, max_target_seq, policy, *batch);
-    SQ_CHECK_LAUNCH("sq_accept_stochastic_batch_stop");
-    return SQ_OK;
-  }
-  if (batch && T_seq && batch->greedy) {
-    accept_stochastic_cluster_kernel<true, NCH, true, true><<<dim3(CL, batch->B), CNT, 0, (cudaStream_t)stream>>>(
-        (const __half*)target_logits, ld_t, (const __half*)draft_logits, ld_d, (const __half*)r, (const __half*)noise,
-        succ_off, succ, depth, S, V, T_seq, tokens, position_ids, accept_idx, state, max_target_seq, policy, *batch);
-    SQ_CHECK_LAUNCH("sq_accept_stochastic_batch_mixed");
-    return SQ_OK;
-  }
   if (batch && T_seq) {
-    accept_stochastic_cluster_kernel<true, NCH, true><<<dim3(CL, batch->B), CNT, 0, (cudaStream_t)stream>>>(
-        (const __half*)target_logits, ld_t, (const __half*)draft_logits, ld_d, (const __half*)r, (const __half*)noise,
-        succ_off, succ, depth, S, V, T_seq, tokens, position_ids, accept_idx, state, max_target_seq, policy, *batch);
-    SQ_CHECK_LAUNCH("sq_accept_stochastic_batch_per_seq");
-    return SQ_OK;
+    if (policy & SQ_ACCEPT_SKIP_DEAD)
+      return launch_accept_batch<NCH, true>(target_logits, ld_t, draft_logits, ld_d, r, noise, succ_off, succ, depth, S,
+                                            V, tokens, position_ids, accept_idx, state, max_target_seq, policy, stream,
+                                            batch, T_seq);
+    return launch_accept_batch<NCH, false>(target_logits, ld_t, draft_logits, ld_d, r, noise, succ_off, succ, depth, S, V,
+                                           tokens, position_ids, accept_idx, state, max_target_seq, policy, stream, batch,
+                                           T_seq);
   }
   if (batch) {
     accept_stochastic_cluster_kernel<true, NCH><<<dim3(CL, batch->B), CNT, 0, (cudaStream_t)stream>>>(

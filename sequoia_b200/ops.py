@@ -178,6 +178,7 @@ def argmax_rows(logits, out=None):
 
 
 ACCEPT_GE, ACCEPT_KEEP_Q = 1, 2          # sq_accept_stochastic policy bits (include/sequoia_b200.h)
+ACCEPT_SKIP_DEAD = 8                     # the per-sequence, mixed and stop batch walks only: skip dead children
 
 
 def accept_stochastic(target_logits, draft_logits, r, noise, succ_off, succ, depth, S, T, tokens, position_ids,
@@ -973,3 +974,80 @@ def guide_advance_batch(guide_table, tokens, state, V: int):
         raise ValueError(f"{name}: {tokens.shape[0]} token rows for {B} sequences")
     check(_lib.load().sq_guide_advance_batch(ptr(guide_table), ptr(tokens), _rows(tokens, "tokens"), ptr(state), V, B,
                                              stream_ptr()), "sq_guide_advance_batch")
+
+
+# ---- constrained drafting: the target-row processing on draft rows (csrc/sq_draft_rows.cu; include/sequoia_b200.h) ----
+def draft_rows_batch_(draft_logits, row_base, row_step, k0: int, nk: int, S: int, state, *, bias=None, ban=None,
+                      guide=None, tokens=None, tree_bits=None, tree_words: int = 0):
+    """Apply, in place, sequence b's allowed set and logit bias, bad words and min_tokens, and guide mask to the draft rows
+    of nodes [k0, k0 + nk) (row row_base[k] + b * row_step[k] of the fp16 draft logits), exactly as logit_bias_rows_batch_,
+    ban_tokens_rows_batch_ and guide_mask_rows_batch_ process target row k.  Each kind is None (not applied) or a tuple:
+      bias  = (allowed, has_mask, bias_ids, bias_vals, n_bias)                    as logit_bias_rows_batch_ takes them;
+      ban   = (prompt_len, depth, words, word_len, n_words, min_end, end_ids)    as ban_tokens_rows_batch_ takes them;
+      guide = (guide_table, node_state): node_state (B, S) int32 holds the parents' states from earlier calls and
+              receives the states of nodes [k0, k0 + nk).
+    tokens (B, ld_seq) int64 and tree_bits / tree_words are needed by ban and guide.  The node range is the root alone
+    (0, 1) or a range in [1, S) whose nodes' parents lie below k0."""
+    name = "draft_rows_batch_"
+    _need(draft_logits, F16, name)
+    if draft_logits.dim() != 2 or draft_logits.stride(-1) != 1:
+        raise ValueError(f"{name}: draft_logits must be (rows, V) with contiguous rows, got {tuple(draft_logits.shape)}")
+    _need(state, torch.int32, name)
+    if not state.is_contiguous():
+        raise ValueError(f"{name}: state must be contiguous")
+    B, V = state.shape[0], draft_logits.shape[1]
+    for k, t in (("row_base", row_base), ("row_step", row_step)):
+        if t is None or t.dtype != torch.int32 or not t.is_cuda or t.dim() != 1 or t.shape[0] < S or t.stride(0) != 1:
+            raise TypeError(f"{name}: {k} must be a contiguous ({S},) int32 CUDA tensor")
+    flags = 0
+    args_bias = [None, 0, None, None, None, None]
+    if bias is not None:
+        flags |= _lib.SQ_DRAFT_BIAS
+        allowed, has_mask, bias_ids, bias_vals, n_bias = bias
+        _need(allowed, torch.int32, name)
+        if allowed.dim() != 2 or allowed.shape[0] < B or allowed.shape[1] < mask_words(V) or not allowed.is_contiguous():
+            raise ValueError(f"{name}: allowed must be a contiguous ({B}, >= {mask_words(V)}) tensor")
+        for k, t, dt in (("has_mask", has_mask, torch.int32), ("n_bias", n_bias, torch.int32)):
+            if t is None or t.dtype != dt or not t.is_cuda or t.dim() != 1 or t.shape[0] < B or t.stride(0) != 1:
+                raise TypeError(f"{name}: {k} must be a contiguous ({B},) int32 CUDA tensor")
+        nmax = _lib.SQ_MAX_LOGIT_BIAS
+        for k, t, dt in (("bias_ids", bias_ids, torch.int32), ("bias_vals", bias_vals, torch.float32)):
+            _need(t, dt, name)
+            if t.dim() != 2 or t.shape[0] < B or t.shape[1] != nmax or not t.is_contiguous():
+                raise ValueError(f"{name}: {k} must be a contiguous ({B}, {nmax}) tensor")
+        args_bias = [ptr(allowed), allowed.shape[1], ptr(has_mask), ptr(bias_ids), ptr(bias_vals), ptr(n_bias)]
+    args_ban = [None] * 7
+    if ban is not None:
+        flags |= _lib.SQ_DRAFT_BAN
+        prompt_len, depth, words, word_len, n_words, min_end, end_ids = ban
+        for k, t, n in (("prompt_len", prompt_len, B), ("n_words", n_words, B), ("min_end", min_end, B),
+                        ("depth", depth, S)):
+            if t is None or t.dtype != torch.int32 or not t.is_cuda or t.dim() != 1 or t.shape[0] < n or t.stride(0) != 1:
+                raise TypeError(f"{name}: {k} must be a contiguous ({n},) int32 CUDA tensor")
+        nw, wl, ns = _lib.SQ_MAX_BAD_WORDS, _lib.SQ_MAX_BAD_WORD_LEN, _lib.SQ_MAX_STOP
+        for k, t, shape in (("words", words, (nw, wl)), ("word_len", word_len, (nw,)), ("end_ids", end_ids, (ns,))):
+            _need(t, torch.int32, name)
+            if tuple(t.shape[1:]) != shape or t.shape[0] < B or not t.is_contiguous():
+                raise ValueError(f"{name}: {k} must be a contiguous ({B}, {', '.join(map(str, shape))}) tensor")
+        args_ban = [ptr(prompt_len), ptr(depth), ptr(words), ptr(word_len), ptr(n_words), ptr(min_end), ptr(end_ids)]
+    args_guide = [None, None]
+    if guide is not None:
+        flags |= _lib.SQ_DRAFT_GUIDE
+        guide_table, node_state = guide
+        _guide_table(guide_table, B, name)
+        _need(node_state, torch.int32, name)
+        if tuple(node_state.shape) != (B, S) or not node_state.is_contiguous():
+            raise ValueError(f"{name}: node_state must be a contiguous ({B}, {S}) tensor")
+        args_guide = [ptr(guide_table), ptr(node_state)]
+    ld_seq = 0
+    if ban is not None or guide is not None:
+        _need(tokens, torch.int64, name)
+        _need(tree_bits, torch.int32, name)
+        if tokens.shape[0] < B or not tree_bits.is_contiguous():
+            raise ValueError(f"{name}: tokens must hold {B} rows and tree_bits must be contiguous")
+        ld_seq = _rows(tokens, "tokens")
+    check(_lib.load().sq_draft_rows_batch(
+        ptr(draft_logits), draft_logits.stride(0), V, ptr(row_base), ptr(row_step), k0, nk, S, ptr(state), flags,
+        *args_bias, ptr(tokens) if ld_seq else None, ld_seq, ptr(tree_bits) if ld_seq else None, tree_words, *args_ban,
+        *args_guide, B, stream_ptr()), "sq_draft_rows_batch")
+    return draft_logits

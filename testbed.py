@@ -285,7 +285,8 @@ def decode_chunk(tree, chunk, limits, stop=DEFAULT_STOP, logprob_means=None, i0:
 @torch.inference_mode()
 def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: int, stop=DEFAULT_STOP,
                      refill: bool = False, seeds=None, policies=None, top_k: int = 0, device_stop: bool = False,
-                     penalties=None, logprobs=None, logit_bias=None, min_p: float = 0.0, bad_words=None):
+                     penalties=None, logprobs=None, logit_bias=None, min_p: float = 0.0, bad_words=None,
+                     constrain_draft: bool = False):
     """--batch B: the same metric loop with B prompts decoded together (sequoia_b200.batch.BatchTree).  Chunked: B
     prompts at a time, each chunk until its last sequence stops.  refill: one batch whose finished slots take the next
     prompt (BatchTree.admit).  seeds: one per prompt (--device-rng): each sequence draws its random numbers on the device
@@ -297,7 +298,8 @@ def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: i
     prompt's generated tokens is printed and returned.  logit_bias: every prompt's logit_bias / allowed_token_ids keywords
     (--logit-bias / --allowed-token-ids, batch_logit_bias); refill admissions keep them.  min_p: every sampled prompt's
     min-p filter (--min-p, 0 = off); refill admissions keep it.  bad_words: every prompt's bad_words / min_tokens
-    keywords (--bad-words / --min-tokens, batch_bad_words); refill admissions keep them."""
+    keywords (--bad-words / --min-tokens, batch_bad_words); refill admissions keep them.  constrain_draft: BatchTree's
+    constrain_draft (--constrain-draft): the draft rows get the allowed set, bias, bad words and guide too."""
     from sequoia_b200.batch import BatchTree
     steps = decoded = 0                          # steps: target steps summed over sequences (per-sequence tokens / step)
     total_time = 0.0
@@ -318,7 +320,7 @@ def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: i
             kw.update(stop_tokens=dstop[0][i0:i0 + len(chunk)], max_new_tokens=dstop[1][i0:i0 + len(chunk)])
         tree = BatchTree(draft, target, chunk, grow_map, policy=pol, temperature=T, top_p=top_p, max_length=M,
                          max_target_seq=M, seeds=None if seeds is None else seeds[i0:i0 + len(chunk)], top_k=top_k, min_p=min_p,
-                         **kw)
+                         constrain_draft=constrain_draft, **kw)
         torch.cuda.synchronize()
         t1 = time.time()
         if refill:
@@ -378,6 +380,9 @@ def build_parser():
                     help="with --batch: ID,ID,...;ID;... token sequences no prompt's output may contain")
     ap.add_argument("--min-tokens", type=int, default=None,
                     help="with --batch: the tokens every prompt generates before a stop id (or 0 / 2) may end it")
+    ap.add_argument("--constrain-draft", action="store_true",
+                    help="with --batch: apply the allowed ids, logit bias and bad words to the draft rows too, so the "
+                         "draft proposes only tokens the target rows keep")
     ap.add_argument("--min-p", type=float, default=0.0,
                     help="with --batch: keep the target tokens whose probability is at least P times the row's largest, "
                          "before top_k and top_p (0 = off)")
@@ -543,6 +548,13 @@ def batch_logit_bias(args) -> dict:
     return kw
 
 
+def batch_constrain_draft(args) -> bool:
+    """--constrain-draft: BatchTree's constrain_draft.  Refused without --batch: the lone trees process no draft rows."""
+    if args.constrain_draft and args.batch == 1 and not args.refill:
+        raise SystemExit("--constrain-draft runs with --batch (the batched tree); the lone trees process no draft rows")
+    return bool(args.constrain_draft)
+
+
 def batch_bad_words(args) -> dict:
     """--bad-words ID,ID,...;ID;... / --min-tokens N: BatchTree's bad_words / min_tokens for every prompt ({} when
     neither is given).  Refused when malformed or outside what BatchTree takes (ids are checked against the vocabulary
@@ -587,6 +599,7 @@ def main(argv=None):
     logprobs = batch_logprobs(args)
     logit_bias = batch_logit_bias(args)
     bad_words = batch_bad_words(args)
+    constrain_draft = batch_constrain_draft(args)
     if args.batch != 1 or args.refill:
         B = check_batch_args(args, len(prompts))
         target = GraphInferenceEngineTG(max_length=args.M, model_name_or_path=args.target, dtype=torch.float16,
@@ -599,7 +612,8 @@ def main(argv=None):
         res = simulation_batch(target, draft, prompts, grow_map, args.tree, args.T, args.P, args.M, B, stop=stop,
                                refill=args.refill, seeds=seeds, policies=policies, top_k=top_k,
                                device_stop=device_stop, penalties=penalties, logprobs=logprobs,
-                               logit_bias=logit_bias, min_p=min_p, bad_words=bad_words)
+                               logit_bias=logit_bias, min_p=min_p, bad_words=bad_words,
+                               constrain_draft=constrain_draft)
         print(json.dumps({k: (round(v, 5) if isinstance(v, float) else v) for k, v in res.items()}))
         return res
     target = (tcls(max_length=args.M, model_name_or_path=args.target, dtype=torch.float16, device=DEV)
