@@ -647,6 +647,28 @@ int sq_token_logprobs_batch(const sq_half* logits, int64_t ld, int V, int S, int
                             int64_t ld_seq, const int32_t* state, const int32_t* accept_idx, int64_t ld_acc,
                             const float* T, const int32_t* greedy, const int32_t* n_top, float* lp_token,
                             int32_t* lp_ids, float* lp_top, int B, void* stream);
+/* Prompt logprobs (csrc/sq_logprobs.cu): the log-probability of each prompt token under the model's raw distribution, from
+ * the fp16 logits of the prompt rows of a first verify (row pitch ld >= V, a multiple of 8, n_logit_rows rows).  parts is
+ * a HOST array of n_parts entries, copied into the kernel arguments; part j scores sequence seq:
+ *   Row r < n_rows of part j is logits row logits_row0 + r, the model's prediction after prompt tokens 0 .. r.  It scores
+ *   tokens[seq][r + 1] and writes position r + 1 of the outputs.  Position 0 is never written.
+ *   Value: the rule of sq_token_logprobs_batch at T = 1 (s_i = the fp16 logit itself), the fp32 log-softmax
+ *   s_t - (m + log sum_i exp(s_i - m)); a row holding +inf or NaN, or only -inf, gives NaN for every value; a token
+ *   outside [0, V) gets NaN.  Top entries: n = min(n_top, V) ids ranked as sq_top_k_filter ranks them, with their logprobs.
+ *   No temperature, filter, penalty, bias, ban or guide applies: no prompt token was drawn from a processed row.
+ * Output at absolute positions: plp_token (B, ld_seq) fp32 [seq][r + 1]; plp_ids (B, ld_seq, SQ_MAX_LOGPROBS) int32 and
+ * plp_top (same shape, fp32) entries [seq][r + 1][0 .. n).  Nothing else is written: not an unlisted sequence, not
+ * position 0 or positions from n_rows + 1 on, not entries from n on.  One PDL-chained launch, grid (max n_rows, n_parts)
+ * of one 1024-thread CTA per row; no state between calls.  Refused with SQ_ERR_INVALID_ARG before any launch: a null
+ * array, B outside 1..SQ_MAX_BATCH, V not a multiple of 8 in 8..131072, ld < V or not a multiple of 8, logits not
+ * 16-byte aligned, n_parts outside 1..B, a seq outside [0, B) or listed twice, n_rows < 1 or n_rows + 1 > ld_seq, rows
+ * outside [0, n_logit_rows), n_top outside 0..SQ_MAX_LOGPROBS. */
+typedef struct {
+  int32_t seq, logits_row0, n_rows, n_top;
+} sq_prompt_lp_part;
+int sq_prompt_logprobs_ragged(const sq_half* logits, int64_t ld, int V, int64_t n_logit_rows,
+                              const sq_prompt_lp_part* parts, int n_parts, const int64_t* tokens, int64_t ld_seq,
+                              float* plp_token, int32_t* plp_ids, float* plp_top, int B, void* stream);
 
 /* ---- ragged batches: a forward over a chosen set of the B sequences, each with its own row count ----
  * A part list names the sequences to run.  Part j is n rows of sequence seq in that sequence's tree-relative addressing:

@@ -129,6 +129,7 @@ _SIGNATURES = {
     "sq_accept_greedy_batch_stop": (i32, [vp, vp, vp, vp, i32, vp, vp, i64, vp, i64, vp, vp, vp, vp, i32, i32, vp]),
     "sq_penalize_rows_batch": (i32, [vp, i64, i32, vp, i64, vp, vp, vp, i32, i32, vp, vp, vp, vp, i64, i32, vp]),
     "sq_token_logprobs_batch": (i32, [vp, i64, i32, i32, i32, vp, i64, vp, vp, i64, vp, vp, vp, vp, vp, vp, i32, vp]),
+    "sq_prompt_logprobs_ragged": (i32, [vp, i64, i32, i64, vp, i32, vp, i64, vp, vp, vp, i32, vp]),
     "sq_logit_bias_rows_batch": (i32, [vp, i64, i32, i32, vp, vp, i64, vp, vp, vp, vp, i32, vp]),
     "sq_ban_tokens_rows_batch": (i32, [vp, i64, i32, vp, i64, vp, vp, vp, vp, i32, i32, vp, vp, vp, vp, vp, i32, vp]),
     "sq_guide_states_batch": (i32, [vp, vp, i64, vp, vp, vp, i32, i32, i32, vp, i32, vp]),

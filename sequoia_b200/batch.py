@@ -43,6 +43,17 @@ generated part to the host.  With T = 1 and no filter, penalty, logit bias or al
 log-probabilities.  While every sequence is off nothing is allocated or launched; the first sequence with logprobs on, at
 construction or admission, captures the steady and post graphs once more.
 
+Prompt logprobs: each sequence has prompt_logprobs None (off) or n in 0..20, vLLM's parameter, for scoring a text.  The
+first verify of a prompt of length P already runs its rows [0, P + S - 1) through every target layer in one ragged
+forward; with the setting on, one lm_head GEMM per sequence turns its final-normed prompt rows 0 .. P-2 into logits (the
+target runner's own logits buffer), and one sq_prompt_logprobs_ragged launch for all of them writes the log-probability of
+each prompt token 1 .. P-1 given the tokens before it, and the n best ids of its row with theirs, into (B, M) /
+(B, M, 20) device buffers; prompt_logprobs(b) copies slot b's to the host.  The values are the model's raw distribution:
+the fp32 log-softmax of the fp16 logits at T = 1.  No temperature, filter, penalty, logit bias, allowed set, bad word or
+guide applies, because no prompt token was drawn from a processed row (token_logprobs, in contrast, reads the processed
+rows).  This is eager work in the first verify, outside every captured graph: graphs, captures and replayed launches are
+the same with the setting on or off, and while every sequence is off nothing is allocated or launched.
+
 Logit bias and allowed tokens: each sequence has a logit_bias {id: bias} and an allowed_token_ids set, vLLM's parameters.
 Every target row of the sequence is processed alike, first of all in the accept step (sq_logit_bias_rows_batch): ids
 outside the allowed set become -inf, then each bias is added to its finite logit; the penalties, the greedy walk and the
@@ -112,8 +123,8 @@ DEFAULT_END_IDS = (0, 2)    # the ids the walks end a sequence on in default mod
 FP16_MAX = 65504.0
 INT32_MAX = (1 << 31) - 1
 POLICIES = ("spec", "greedy")
-_PREVIOUS = object()        # admit(): keep the slot's previous stop set / budget / logprobs / logit bias / allowed set /
-                            # bad words / min_tokens / guide
+_PREVIOUS = object()        # admit(): keep the slot's previous stop set / budget / logprobs / prompt logprobs / logit
+                            # bias / allowed set / bad words / min_tokens / guide
 
 
 def draw_random(prompts: Sequence[torch.Tensor], M: int, S: int, V: int):
@@ -321,6 +332,26 @@ def _logprobs(logprobs, B: int) -> List[Optional[int]]:
             raise ValueError(f"logprobs: {len(vals)} values for {B} sequences")
         return vals
     return [check_logprobs(logprobs)] * B
+
+
+def check_prompt_logprobs(prompt_logprobs) -> Optional[int]:
+    """A prompt_logprobs setting: None (off) or an integer in 0..20, the number of top alternatives per prompt token."""
+    if prompt_logprobs is None:
+        return None
+    if isinstance(prompt_logprobs, bool) or not isinstance(prompt_logprobs, numbers.Integral) \
+            or not 0 <= prompt_logprobs <= MAX_LOGPROBS:
+        raise ValueError(f"prompt_logprobs must be None or an integer in 0..{MAX_LOGPROBS}, got {prompt_logprobs!r}")
+    return int(prompt_logprobs)
+
+
+def _prompt_logprobs(prompt_logprobs, B: int) -> List[Optional[int]]:
+    """One prompt_logprobs setting for all B sequences, or a sequence of B of them."""
+    if _is_collection(prompt_logprobs):
+        vals = [check_prompt_logprobs(n) for n in prompt_logprobs]
+        if len(vals) != B:
+            raise ValueError(f"prompt_logprobs: {len(vals)} values for {B} sequences")
+        return vals
+    return [check_prompt_logprobs(prompt_logprobs)] * B
 
 
 def check_logit_bias(logit_bias, V: Optional[int] = None) -> Optional[tuple]:
@@ -542,6 +573,10 @@ class BatchTree:
     logprobs: None (off) or an integer in 0..20, for all sequences or one per prompt: token_logprobs(b) then gives the
     log-probability of each generated token and of the n best alternatives of its row (module docstring,
     include/sequoia_b200.h).  Both policies honour it; verify() returns what it returns without it.
+    prompt_logprobs: None (off) or an integer in 0..20, for all sequences or one per prompt: prompt_logprobs(b) then gives
+    the log-probability of each prompt token after the first, given the tokens before it, and the n best alternatives of
+    its row, under the target's raw distribution (T = 1, no processing; module docstring).  It is computed in the first
+    verify, outside the captured graphs; verify() returns what it returns without it.
     logit_bias: None or a mapping {id: bias} of at most 1024 ids in [0, V) with biases in [-100, 100] (-100 bans an id in
     practice), for all sequences or one per prompt.  allowed_token_ids: None or a non-empty collection of distinct ids in
     [0, V), for all sequences or one per prompt: every other id is -inf in the sequence's target rows.  Both policies
@@ -571,7 +606,7 @@ class BatchTree:
                  frequency_penalty: Union[float, Sequence[float]] = 0.0,
                  presence_penalty: Union[float, Sequence[float]] = 0.0,
                  logprobs: Union[None, int, Sequence[Optional[int]]] = None,
-                 logit_bias=None, allowed_token_ids=None, min_p: Union[float, Sequence[float]] = 0.0,
+                 prompt_logprobs: Union[None, int, Sequence[Optional[int]]] = None, logit_bias=None, allowed_token_ids=None, min_p: Union[float, Sequence[float]] = 0.0,
                  bad_words=None, min_tokens: Union[int, Sequence[int]] = 0, guide=None, constrain_draft: bool = False):
         if not isinstance(constrain_draft, bool):
             raise ValueError(f"constrain_draft must be a bool, got {constrain_draft!r}")
@@ -582,6 +617,7 @@ class BatchTree:
         words, min_toks = _bad_words(bad_words, B), _min_tokens(min_tokens, B)
         biases, alloweds = _logit_biases(logit_bias, B), _allowed_sets(allowed_token_ids, B)
         lps = _logprobs(logprobs, B)
+        plps = _prompt_logprobs(prompt_logprobs, B)
         reps = _penalties("repetition_penalty", repetition_penalty, B)
         freqs = _penalties("frequency_penalty", frequency_penalty, B)
         press = _penalties("presence_penalty", presence_penalty, B)
@@ -685,6 +721,12 @@ class BatchTree:
         self.n_top_dev = torch.tensor([-1 if n is None else n for n in lps], dtype=torch.int32, device=dev)
         self.use_logprobs = False
         self.lp_token = self.lp_ids = self.lp_top = None
+        # prompt logprobs: each slot's n (None = off) and whether its current prompt has had its first verify (the
+        # buffers hold its values from then until the next admission); the (B, M) / (B, M, 20) buffers are allocated for
+        # the first slot that turns it on
+        self.prompt_logprobs_n = plps
+        self.plp_ready = [False] * B
+        self.plp_token = self.plp_ids = self.plp_top = None
         # bad words and min_tokens: each slot's word table and absolute limit L + min_tokens on the device, read by
         # sq_ban_tokens_rows_batch inside the captured graphs, which it joins the first time a slot is non-neutral
         self.bad_words, self.min_tokens = words, min_toks
@@ -745,6 +787,8 @@ class BatchTree:
             self.r, self.rand = r.to(dev), rand.to(dev)
         if any(n is not None for n in lps):
             self._start_logprobs()
+        if any(n is not None for n in plps):
+            self._start_prompt_logprobs()
         if any(g is not None for g in guides):
             self._start_guide()
         for b, p in enumerate(prompts):
@@ -770,6 +814,14 @@ class BatchTree:
         self.lp_token = torch.full((B, M), float("nan"), dtype=torch.float32, device=dev)
         self.lp_ids = torch.full((B, M, MAX_LOGPROBS), -1, dtype=torch.int32, device=dev)
         self.lp_top = torch.full((B, M, MAX_LOGPROBS), float("nan"), dtype=torch.float32, device=dev)
+
+    def _start_prompt_logprobs(self):
+        """The (B, M) / (B, M, 20) prompt-logprobs buffers, NaN / -1 filled (written eagerly by the first verify of each
+        prompt with the setting on, outside the captured graphs)."""
+        B, M, dev = self.B, self.M, self.device
+        self.plp_token = torch.full((B, M), float("nan"), dtype=torch.float32, device=dev)
+        self.plp_ids = torch.full((B, M, MAX_LOGPROBS), -1, dtype=torch.int32, device=dev)
+        self.plp_top = torch.full((B, M, MAX_LOGPROBS), float("nan"), dtype=torch.float32, device=dev)
 
     def _start_logit_bias(self):
         """The mask-and-bias kernel joins op_accept, with every slot's device rows; it writes no scratch, so nothing joins
@@ -912,7 +964,7 @@ class BatchTree:
               stop_tokens=_PREVIOUS, max_new_tokens=_PREVIOUS, repetition_penalty: Optional[float] = None,
               frequency_penalty: Optional[float] = None, presence_penalty: Optional[float] = None,
               logprobs=_PREVIOUS, logit_bias=_PREVIOUS, allowed_token_ids=_PREVIOUS, min_p: Optional[float] = None,
-              bad_words=_PREVIOUS, min_tokens=_PREVIOUS, guide=_PREVIOUS):
+              bad_words=_PREVIOUS, min_tokens=_PREVIOUS, guide=_PREVIOUS, prompt_logprobs=_PREVIOUS):
         """Start `prompt` in the frozen slot b (finished, out of room, or stopped with freeze), at its own policy,
         temperature, top_p and top_k (default: the slot's previous values).  The next verify() runs its first verify next
         to the steady sequences.  The slot draws r and rand as a lone SpecTree on the prompt would, and runs its draft
@@ -933,6 +985,8 @@ class BatchTree:
         the steady and post graphs once more.
         logprobs: the prompt's logprobs setting (default: the slot's previous one; None is off).  The first one that is
         on, in a tree without one, captures the steady and post graphs once more.
+        prompt_logprobs: the prompt's prompt_logprobs setting (default: the slot's previous one; None is off).  Its values
+        come from the next verify(), the prompt's first; until then prompt_logprobs(b) is refused.  No recapture.
         logit_bias / allowed_token_ids: the prompt's logit bias and allowed set (default: the slot's previous ones; None is
         none).  The first non-neutral one, in a tree without one, captures the steady and post graphs once more.
         bad_words / min_tokens: the prompt's bad words (None is none) and min_tokens (default: the slot's previous ones);
@@ -955,6 +1009,8 @@ class BatchTree:
                  ("presence_penalty", presence_penalty))]
         if logprobs is not _PREVIOUS:
             logprobs = check_logprobs(logprobs)
+        if prompt_logprobs is not _PREVIOUS:
+            prompt_logprobs = check_prompt_logprobs(prompt_logprobs)
         if logit_bias is not _PREVIOUS:
             logit_bias = check_logit_bias(logit_bias, self.V)
         if allowed_token_ids is not _PREVIOUS:
@@ -1048,6 +1104,11 @@ class BatchTree:
             self._start_logprobs()                 # the logprobs kernel enters seq_post: capture steady and post once more
             for name in ("steady", "post"):
                 self.graphs.pop(name, None)
+        if prompt_logprobs is not _PREVIOUS:
+            self.prompt_logprobs_n[b] = prompt_logprobs
+        self.plp_ready[b] = False                  # the earlier occupant's values are not this prompt's
+        if self.prompt_logprobs_n[b] is not None and self.plp_token is None:
+            self._start_prompt_logprobs()
         if logit_bias is not _PREVIOUS:
             self.logit_bias[b] = logit_bias
         if allowed_token_ids is not _PREVIOUS:
@@ -1116,11 +1177,27 @@ class BatchTree:
 
     def op_target_first(self, seqs):
         """First verify of the sequences `seqs` (SpecTree.py:164-176) as one ragged forward: each one's rows [0, P+S-1),
-        the logits of its S tree rows."""
+        the logits of its S tree rows.  Then the prompt logprobs of those with the setting on (op_prompt_logprobs)."""
         S = self.S
-        self.target.engine.runner.forward_ragged(
+        runner = self.target.engine.runner
+        row0 = runner.forward_ragged(
             [(b, self.ground_truth_len[b] + S - 1, 1 - self.ground_truth_len[b], S, S,
               self.target_logits[b * S:(b + 1) * S]) for b in seqs], self.tokens, self.position_ids, self.storage_ids, state=self.state, **self._mask_kw())
+        self.op_prompt_logprobs(seqs, row0)
+
+    def op_prompt_logprobs(self, seqs, row0):
+        """Prompt logprobs of the first-verify sequences `seqs` with the setting on and P >= 2, whose ragged forward left
+        the final-normed rows of sequence seqs[j] at the target runner's rows [row0[j], ...): one lm_head GEMM per
+        sequence over its prompt rows [row0[j], row0[j] + P - 1), into the runner's logits at the same rows, then one
+        sq_prompt_logprobs_ragged launch for all of them.  Eager (outside every graph); nothing when no sequence is on."""
+        runner = self.target.engine.runner
+        parts = [(b, r0, self.ground_truth_len[b] - 1, self.prompt_logprobs_n[b]) for b, r0 in zip(seqs, row0)
+                 if self.prompt_logprobs_n[b] is not None and self.ground_truth_len[b] >= 2]
+        if not parts:
+            return
+        for _, r0, n_rows, _ in parts:
+            runner.lm_head_rows(r0, r0 + n_rows)
+        ops.prompt_logprobs_ragged_(runner.logits, parts, self.tokens, self.plp_token, self.plp_ids, self.plp_top)
 
     def op_accept(self):
         st = self.st
@@ -1304,6 +1381,8 @@ class BatchTree:
         if self.external_noise is not None and not self.greedy:
             self.noise.copy_(self.external_noise[self.iter])
         first = [b for b in range(self.B) if not self.frozen[b] and self.target_kv_len[b] != self.ground_truth_len[b] - 1]
+        for b in range(self.B):                         # this step is every decoding prompt's first verify or a later one
+            self.plp_ready[b] = self.plp_ready[b] or not self.frozen[b]
         if first:
             if len(first) + sum(self.frozen) < self.B:
                 # steady sequences share the step with admitted ones: their tree rows first, the admitted slots frozen
@@ -1367,3 +1446,21 @@ class BatchTree:
         k = min(n_lp, self.V)
         return (self.lp_token[b, L:end].cpu(), self.lp_ids[b, L:end, :k].cpu().to(torch.int64),
                 self.lp_top[b, L:end, :k].cpu())
+
+    def prompt_logprobs(self, b: int):
+        """Slot b's prompt scores, on the host: -> (token_lp (P-1,) float32, top_ids (P-1, k) int64, top_lp (P-1, k)
+        float32), P = len(prompt), k = the slot's prompt_logprobs setting (at most V).  Row i is prompt position i + 1:
+        token_lp[i] is the log-probability of prompt token i + 1 given tokens 0 .. i, top_ids[i] / top_lp[i] the k best ids
+        of that row, best first, and theirs, all under the target's raw distribution (T = 1, no processing).  Position 0
+        has no value; a prompt of length 1 gives empty arrays.  Refused for a slot whose setting is off and for a slot
+        whose current prompt has not had its first verify() yet."""
+        if not 0 <= b < self.B:
+            raise IndexError(f"slot {b} out of range for a batch of {self.B}")
+        n = self.prompt_logprobs_n[b]
+        if n is None:
+            raise ValueError(f"slot {b} has prompt logprobs off (prompt_logprobs=None)")
+        if not self.plp_ready[b]:
+            raise ValueError(f"slot {b}: its prompt has not had its first verify() yet")
+        P, k = self.prompt_lens[b], min(n, self.V)
+        return (self.plp_token[b, 1:P].cpu(), self.plp_ids[b, 1:P, :k].cpu().to(torch.int64),
+                self.plp_top[b, 1:P, :k].cpu())

@@ -8,6 +8,8 @@
 //      index order (a block scan per tile of 8192 entries).
 // The select is top_k_filter_kernel's two-level 256-bin histogram select (sq_sampling.cu) with the same key (topk_key),
 // so the ids are exactly those the top-k filter would keep, ranked.  Counts are integers: no result depends on timing.
+// sq_prompt_logprobs_ragged runs the same per-row body (lp_row) at T = 1 on the prompt rows of a first verify, one CTA per
+// row of every listed sequence in one launch.
 #include "sq_common.cuh"
 
 namespace sq {
@@ -51,12 +53,14 @@ __device__ __forceinline__ void lp_reduce_select(uint32_t (*whist)[256], uint32_
   __syncthreads();
 }
 
-__global__ void __launch_bounds__(LP_NT)
-    token_logprobs_kernel(const __half* __restrict__ logits, int64_t ld, int V, int S, const int64_t* __restrict__ tokens,
-                          int64_t ld_seq, const int32_t* __restrict__ state, const int32_t* __restrict__ accept_idx,
-                          int64_t ld_acc, const float* __restrict__ T, const int32_t* __restrict__ greedy,
-                          const int32_t* __restrict__ n_top, float* __restrict__ lp_token, int32_t* __restrict__ lp_ids,
-                          float* __restrict__ lp_top) {
+// One row's logprobs, by every thread (tid = threadIdx.x) of a 1024-thread CTA after the dependency wait: the
+// log-softmax of s_i = fp16(x_i * inv_T) at token tokens[pos] into lp_token[pos], and the n best ids (topk_key order,
+// ties by index) with their logprobs into lp_ids / lp_top[pos][0 .. n).  token_logprobs_kernel and prompt_logprobs_kernel
+// share it, so one rule serves generated and prompt tokens.  (The caller reads tid before its early exits: that keeps
+// token_logprobs_kernel's SASS what it was before the body moved here.)
+__device__ __forceinline__ void lp_row(const __half* row, int V, float inv_T, int n,
+                                       const int64_t* __restrict__ tokens, int64_t pos, float* __restrict__ lp_token,
+                                       int32_t* __restrict__ lp_ids, float* __restrict__ lp_top, int tid) {
   __shared__ uint32_t whist[LP_NW][256];
   __shared__ uint32_t hist[256];
   __shared__ float red[LP_NW];
@@ -65,24 +69,9 @@ __global__ void __launch_bounds__(LP_NT)
   __shared__ int n_above;
   __shared__ uint32_t c_key[SQ_MAX_LOGPROBS];
   __shared__ int c_idx[SQ_MAX_LOGPROBS];
-  pdl_wait();
-  pdl_trigger();
-  const int j = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
   const int lane = tid & 31, warp = tid >> 5;
-  const int32_t* st = state + b * ST_WORDS;
-  if (st[ST_FROZEN] || n_top[b] < 0) return;
-  const int P = st[ST_P_OLD], n_new = st[ST_N_NEW], a = P + n_new;
-  const int M = st[ST_M] > 0 ? st[ST_M] : (int)min(ld_seq, (int64_t)INT32_MAX);
-  const int committed = n_new + ((!st[ST_TERMINAL] && a < M) ? 1 : 0);      // finish_verify's bonus_ok
-  if (j >= committed || P < 1 || (int64_t)P + j >= ld_seq) return;
-  const int node = j == 0 ? 0 : accept_idx[b * ld_acc + j - 1] - (P - 1);
-  if (node < 0 || node >= S) return;                                          // (not a walk's output)
-  const int n = min(min(n_top[b], SQ_MAX_LOGPROBS), V);
-  const float inv_T = greedy[b] ? 1.0f : 1.0f / T[b];                         // the walk's inv_temp
-  const __half* row = logits + ((int64_t)b * S + node) * ld;
   const uint4* row4 = reinterpret_cast<const uint4*>(row);
   const int nvec = V / 8;
-  const int64_t pos = (int64_t)b * ld_seq + P + j;
 
   // pass 1: max of s, a +inf / NaN flag, level-0 histogram
   if (n > 0) {
@@ -206,6 +195,48 @@ __global__ void __launch_bounds__(LP_NT)
   }
 }
 
+__global__ void __launch_bounds__(LP_NT)
+    token_logprobs_kernel(const __half* __restrict__ logits, int64_t ld, int V, int S, const int64_t* __restrict__ tokens,
+                          int64_t ld_seq, const int32_t* __restrict__ state, const int32_t* __restrict__ accept_idx,
+                          int64_t ld_acc, const float* __restrict__ T, const int32_t* __restrict__ greedy,
+                          const int32_t* __restrict__ n_top, float* __restrict__ lp_token, int32_t* __restrict__ lp_ids,
+                          float* __restrict__ lp_top) {
+  pdl_wait();
+  pdl_trigger();
+  const int j = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
+  const int32_t* st = state + b * ST_WORDS;
+  if (st[ST_FROZEN] || n_top[b] < 0) return;
+  const int P = st[ST_P_OLD], n_new = st[ST_N_NEW], a = P + n_new;
+  const int M = st[ST_M] > 0 ? st[ST_M] : (int)min(ld_seq, (int64_t)INT32_MAX);
+  const int committed = n_new + ((!st[ST_TERMINAL] && a < M) ? 1 : 0);      // finish_verify's bonus_ok
+  if (j >= committed || P < 1 || (int64_t)P + j >= ld_seq) return;
+  const int node = j == 0 ? 0 : accept_idx[b * ld_acc + j - 1] - (P - 1);
+  if (node < 0 || node >= S) return;                                          // (not a walk's output)
+  const int n = min(min(n_top[b], SQ_MAX_LOGPROBS), V);
+  const float inv_T = greedy[b] ? 1.0f : 1.0f / T[b];                         // the walk's inv_temp
+  const int64_t pos = (int64_t)b * ld_seq + P + j;
+  lp_row(logits + ((int64_t)b * S + node) * ld, V, inv_T, n, tokens, pos, lp_token, lp_ids, lp_top, tid);
+}
+
+// Prompt logprobs (sq_prompt_logprobs_ragged): CTA (r, j) scores tokens[seq_j][r + 1] on logits row logits_row0_j + r at
+// T = 1, position r + 1 of the outputs.
+struct PromptLpParts {
+  int seq[SQ_MAX_BATCH], row0[SQ_MAX_BATCH], n_rows[SQ_MAX_BATCH], n_top[SQ_MAX_BATCH];
+};
+
+__global__ void __launch_bounds__(LP_NT)
+    prompt_logprobs_kernel(const __half* __restrict__ logits, int64_t ld, int V, PromptLpParts parts,
+                           const int64_t* __restrict__ tokens, int64_t ld_seq, float* __restrict__ plp_token,
+                           int32_t* __restrict__ plp_ids, float* __restrict__ plp_top) {
+  pdl_wait();
+  pdl_trigger();
+  const int r = blockIdx.x, j = blockIdx.y;
+  if (r >= parts.n_rows[j]) return;
+  const int n = min(parts.n_top[j], V);
+  const int64_t pos = (int64_t)parts.seq[j] * ld_seq + r + 1;
+  lp_row(logits + ((int64_t)parts.row0[j] + r) * ld, V, 1.0f, n, tokens, pos, plp_token, plp_ids, plp_top, threadIdx.x);
+}
+
 }  // namespace sq
 
 using namespace sq;
@@ -229,5 +260,42 @@ extern "C" int sq_token_logprobs_batch(const sq_half* logits, int64_t ld, int V,
   launch_k(token_logprobs_kernel, dim3(max_depth + 1, B), dim3(LP_NT), 0, (cudaStream_t)stream, (const __half*)logits, ld,
            V, S, tokens, ld_seq, state, accept_idx, ld_acc, T, greedy, n_top, lp_token, lp_ids, lp_top);
   SQ_CHECK_LAUNCH("sq_token_logprobs_batch");
+  return SQ_OK;
+}
+
+extern "C" int sq_prompt_logprobs_ragged(const sq_half* logits, int64_t ld, int V, int64_t n_logit_rows,
+                                         const sq_prompt_lp_part* parts, int n_parts, const int64_t* tokens,
+                                         int64_t ld_seq, float* plp_token, int32_t* plp_ids, float* plp_top, int B,
+                                         void* stream) {
+  SQ_CHECK_ARG(logits && parts && tokens && plp_token && plp_ids && plp_top, "sq_prompt_logprobs_ragged: null array");
+  SQ_CHECK_ARG(B >= 1 && B <= SQ_MAX_BATCH, "sq_prompt_logprobs_ragged: B=%d (1..%d)", B, SQ_MAX_BATCH);
+  SQ_CHECK_ARG(V % 8 == 0 && V > 0 && V <= 131072, "sq_prompt_logprobs_ragged: V=%d must be a multiple of 8, <= 131072",
+               V);
+  SQ_CHECK_ARG(ld >= V && ld % 8 == 0, "sq_prompt_logprobs_ragged: ld=%lld must be >= V=%d and a multiple of 8",
+               (long long)ld, V);
+  SQ_CHECK_ARG(((uintptr_t)logits & 15) == 0, "sq_prompt_logprobs_ragged: logits must be 16-byte aligned");
+  SQ_CHECK_ARG(n_parts >= 1 && n_parts <= B, "sq_prompt_logprobs_ragged: %d parts for %d sequences", n_parts, B);
+  PromptLpParts pp{};
+  unsigned seen = 0;
+  int max_rows = 0;
+  for (int j = 0; j < n_parts; ++j) {
+    const sq_prompt_lp_part& p = parts[j];
+    SQ_CHECK_ARG(p.seq >= 0 && p.seq < B, "sq_prompt_logprobs_ragged: part %d names sequence %d of %d", j, p.seq, B);
+    SQ_CHECK_ARG(!(seen >> p.seq & 1u), "sq_prompt_logprobs_ragged: sequence %d listed twice", p.seq);
+    SQ_CHECK_ARG(p.n_rows >= 1 && (int64_t)p.n_rows + 1 <= ld_seq,
+                 "sq_prompt_logprobs_ragged: part %d has n_rows=%d (1..ld_seq-1, ld_seq=%lld)", j, p.n_rows,
+                 (long long)ld_seq);
+    SQ_CHECK_ARG(p.logits_row0 >= 0 && (int64_t)p.logits_row0 + p.n_rows <= n_logit_rows,
+                 "sq_prompt_logprobs_ragged: part %d reads logits rows [%d, %lld) of %lld", j, p.logits_row0,
+                 (long long)p.logits_row0 + p.n_rows, (long long)n_logit_rows);
+    SQ_CHECK_ARG(p.n_top >= 0 && p.n_top <= SQ_MAX_LOGPROBS, "sq_prompt_logprobs_ragged: part %d has n_top=%d (0..%d)", j,
+                 p.n_top, SQ_MAX_LOGPROBS);
+    seen |= 1u << p.seq;
+    pp.seq[j] = p.seq; pp.row0[j] = p.logits_row0; pp.n_rows[j] = p.n_rows; pp.n_top[j] = p.n_top;
+    max_rows = max(max_rows, p.n_rows);
+  }
+  launch_k(prompt_logprobs_kernel, dim3(max_rows, n_parts), dim3(LP_NT), 0, (cudaStream_t)stream,
+           (const __half*)logits, ld, V, pp, tokens, ld_seq, plp_token, plp_ids, plp_top);
+  SQ_CHECK_LAUNCH("sq_prompt_logprobs_ragged");
   return SQ_OK;
 }

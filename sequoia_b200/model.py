@@ -18,7 +18,7 @@ import json
 import math
 import os
 from dataclasses import dataclass
-from typing import Dict, Optional
+from typing import Dict, List, Optional
 
 import torch
 
@@ -442,12 +442,14 @@ class LlamaRunner:
 
     @torch.no_grad()
     def forward_ragged(self, parts, tokens: torch.Tensor, position_ids: torch.Tensor, storage_ids: torch.Tensor, *,
-                       state: torch.Tensor, tree_bits=None, tree_words: int = 0, tree_size: int = 0) -> None:
+                       state: torch.Tensor, tree_bits=None, tree_words: int = 0, tree_size: int = 0) -> List[int]:
         """Forward a chosen set of the engine's B sequences, each with its own row count, at the cost of those rows.
         parts: (seq, n, n0, kv_end, n_logits, logits_out) per sequence -- n rows of sequence seq in the tree-relative
         addressing of its state row (as forward(batch=True) with that n0 / kv_end), packed in list order for the row-wise
         ops and the GEMMs; the logits of its last n_logits rows go to logits_out (n_logits, V).  Sequences not listed are
-        neither read nor written (their SQ_ST_FROZEN word is not consulted)."""
+        neither read nor written (their SQ_ST_FROZEN word is not consulted).
+        -> row0: part j's rows are activation rows [row0[j], row0[j + 1]) (len(parts) + 1 entries); their final-normed
+        hidden states stay in self.normed until the next forward (lm_head_rows reads them)."""
         if self.tp.size > 1:
             raise NotImplementedError("forward_ragged runs on one GPU: tensor-parallel engines use forward(batch=True)")
         geo = [tuple(int(x) for x in p[:4]) for p in parts]
@@ -468,6 +470,14 @@ class LlamaRunner:
         self._layers(row0[-1], attend)
         for (_, n, _, _), (*_, m, out), r0 in zip(geo, parts, row0):
             self._lm_head(r0 + n - m, r0 + n, out)
+        return row0
+
+    def lm_head_rows(self, start: int, end: int) -> torch.Tensor:
+        """The logits of the final-normed rows [start, end) of the last forward into self.logits[start:end] (sq_gemm at
+        <= 128 rows where the engine has its plan, cuBLASLt above), returned."""
+        if not 0 <= start < end <= self.n_max:
+            raise ValueError(f"lm_head_rows: rows [{start}, {end}) outside [0, {self.n_max})")
+        return self._lm_head(start, end, self.logits[start:end])
 
     def _layers(self, n: int, attend):
         """The decoder layers over activation rows [0, n); attend(l) is layer l's RoPE + KV append and attention."""

@@ -814,6 +814,38 @@ def token_logprobs_batch_(target_logits, S: int, max_depth: int, tokens, state, 
           "sq_token_logprobs_batch")
 
 
+class PromptLpPart(C.Structure):
+    """sq_prompt_lp_part: rows [0, n_rows) of sequence seq's prompt scores, on logits rows logits_row0 + r, n_top best"""
+    _fields_ = [("seq", C.c_int32), ("logits_row0", C.c_int32), ("n_rows", C.c_int32), ("n_top", C.c_int32)]
+
+
+def prompt_logprobs_ragged_(logits, parts, tokens, plp_token, plp_ids, plp_top):
+    """Prompt logprobs at T = 1 for the listed sequences, one launch: parts is (seq, logits_row0, n_rows, n_top) per
+    sequence; row r of a part (logits row logits_row0 + r, the prediction after prompt tokens 0 .. r) scores tokens[seq,
+    r + 1] into plp_token[seq, r + 1], and its min(n_top, V) best ids with their logprobs into plp_ids / plp_top[seq, r + 1,
+    :n].  logits: (rows, V) fp16 with contiguous rows; tokens: (B, M) int64; plp_token: (B, M) float32; plp_ids: (B, M, 20)
+    int32; plp_top: (B, M, 20) float32.  Nothing else of the outputs is written."""
+    name = "prompt_logprobs_ragged_"
+    _need(logits, F16, name)
+    if logits.dim() != 2 or logits.stride(-1) != 1:
+        raise ValueError(f"{name}: logits must be (rows, V) with contiguous rows, got {tuple(logits.shape)}")
+    _need(tokens, torch.int64, name)
+    if tokens.dim() != 2:
+        raise ValueError(f"{name}: tokens must be (B, M), got {tuple(tokens.shape)}")
+    B, M = tokens.shape
+    for k, t, dt, shape in (("plp_token", plp_token, torch.float32, (B, M)),
+                            ("plp_ids", plp_ids, torch.int32, (B, M, _lib.SQ_MAX_LOGPROBS)),
+                            ("plp_top", plp_top, torch.float32, (B, M, _lib.SQ_MAX_LOGPROBS))):
+        _need(t, dt, name)
+        if tuple(t.shape) != shape or not t.is_contiguous():
+            raise ValueError(f"{name}: {k} must be a contiguous {shape} tensor, got {tuple(t.shape)}")
+    arr = (PromptLpPart * len(parts))(*[tuple(int(x) for x in p) for p in parts])
+    check(_lib.load().sq_prompt_logprobs_ragged(ptr(logits), logits.stride(0), logits.shape[1], logits.shape[0],
+                                                C.addressof(arr), len(arr), ptr(tokens), _rows(tokens, "tokens"),
+                                                ptr(plp_token), ptr(plp_ids), ptr(plp_top), B, stream_ptr()),
+          "sq_prompt_logprobs_ragged")
+
+
 # ---- per-sequence allowed-token mask and logit bias (csrc/sq_logit_bias.cu; semantics in include/sequoia_b200.h) ----------
 def mask_words(V: int) -> int:
     """int32 words of one allowed-token bitmask row: ceil(V / 32)."""

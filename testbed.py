@@ -16,6 +16,7 @@ from __future__ import annotations
 
 import argparse
 import json
+import math
 import os
 import random
 import sys
@@ -202,8 +203,16 @@ def _record_logprobs(tree, b: int, i: int, means):
         means[i] = float(lp.double().mean()) if len(lp) else float("nan")
 
 
+def _record_prompt_logprobs(tree, b: int, i: int, means):
+    """means[i] = the mean logprob of prompt i's tokens after the first, scored in slot b (a tree with prompt logprobs;
+    means None: off; NaN for a one-token prompt)."""
+    if means is not None:
+        lp = tree.prompt_logprobs(b)[0]
+        means[i] = float(lp.double().mean()) if len(lp) else float("nan")
+
+
 def decode_refill(tree, prompts, limits, stop=DEFAULT_STOP, step_times=None, seeds=None, policies=None,
-                  device_stop=None, logprob_means=None):
+                  device_stop=None, logprob_means=None, prompt_logprob_means=None):
     """Decode every prompt of a queue on a BatchTree whose B slots start with prompts[:B]: each slot that finishes (a stop
     token, its length limit `limits[i]`, or out of room) takes the next prompt, until the queue is empty.
     -> (outputs, decoded tokens, per-sequence target steps, admission order); outputs[i] = prompt i's committed tokens.
@@ -211,7 +220,8 @@ def decode_refill(tree, prompts, limits, stop=DEFAULT_STOP, step_times=None, see
     first admit() of the step to the end of its verify.  seeds: for a seeded tree, prompt i's seed is seeds[i].
     policies: prompt i decodes with policies[i] ("spec" / "greedy"); None keeps each slot's policy.
     device_stop: (stop_tokens, max_new_tokens) per prompt (device_stop_settings), passed to each admission; None keeps
-    each slot's.  logprob_means: a list that receives prompt i's mean token logprob at index i (--logprobs)."""
+    each slot's.  logprob_means: a list that receives prompt i's mean token logprob at index i (--logprobs).
+    prompt_logprob_means: the same for the mean logprob of prompt i's own tokens (--prompt-logprobs)."""
     B = len(tree.frozen)
     slot = list(range(B))                        # prompt index decoding in each slot (None: the queue ran out)
     length = [len(p) for p in prompts[:B]]
@@ -247,6 +257,7 @@ def decode_refill(tree, prompts, limits, stop=DEFAULT_STOP, step_times=None, see
             if terminate or tree.frozen[b] or last in stop or length[b] >= limits[i]:
                 outputs[i] = valid.clone()           # the slot's token row is reused by the next prompt
                 _record_logprobs(tree, b, i, logprob_means)
+                _record_prompt_logprobs(tree, b, i, prompt_logprob_means)
                 if not tree.frozen[b]:
                     tree.freeze(b)
                 if nxt < len(prompts):
@@ -259,9 +270,10 @@ def decode_refill(tree, prompts, limits, stop=DEFAULT_STOP, step_times=None, see
     return outputs, decoded, steps, order
 
 
-def decode_chunk(tree, chunk, limits, stop=DEFAULT_STOP, logprob_means=None, i0: int = 0):
+def decode_chunk(tree, chunk, limits, stop=DEFAULT_STOP, logprob_means=None, i0: int = 0, prompt_logprob_means=None):
     """Decode a BatchTree built on `chunk` until every sequence has finished.  -> (decoded tokens, per-sequence steps)
-    logprob_means: a list that receives the mean token logprob of chunk[b] at index i0 + b (--logprobs)."""
+    logprob_means: a list that receives the mean token logprob of chunk[b] at index i0 + b (--logprobs);
+    prompt_logprob_means the same for the mean logprob of chunk[b]'s own tokens (--prompt-logprobs)."""
     length = [len(p) for p in chunk]
     done = set()
     decoded = steps = 0
@@ -277,6 +289,7 @@ def decode_chunk(tree, chunk, limits, stop=DEFAULT_STOP, logprob_means=None, i0:
             if terminate or tree.frozen[b] or last in stop or length[b] >= limits[b]:
                 done.add(b)
                 _record_logprobs(tree, b, i0 + b, logprob_means)
+                _record_prompt_logprobs(tree, b, i0 + b, prompt_logprob_means)
                 if not tree.frozen[b]:
                     tree.freeze(b)
     return decoded, steps
@@ -286,7 +299,7 @@ def decode_chunk(tree, chunk, limits, stop=DEFAULT_STOP, logprob_means=None, i0:
 def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: int, stop=DEFAULT_STOP,
                      refill: bool = False, seeds=None, policies=None, top_k: int = 0, device_stop: bool = False,
                      penalties=None, logprobs=None, logit_bias=None, min_p: float = 0.0, bad_words=None,
-                     constrain_draft: bool = False):
+                     constrain_draft: bool = False, prompt_logprobs=None):
     """--batch B: the same metric loop with B prompts decoded together (sequoia_b200.batch.BatchTree).  Chunked: B
     prompts at a time, each chunk until its last sequence stops.  refill: one batch whose finished slots take the next
     prompt (BatchTree.admit).  seeds: one per prompt (--device-rng): each sequence draws its random numbers on the device
@@ -299,7 +312,10 @@ def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: i
     (--logit-bias / --allowed-token-ids, batch_logit_bias); refill admissions keep them.  min_p: every sampled prompt's
     min-p filter (--min-p, 0 = off); refill admissions keep it.  bad_words: every prompt's bad_words / min_tokens
     keywords (--bad-words / --min-tokens, batch_bad_words); refill admissions keep them.  constrain_draft: BatchTree's
-    constrain_draft (--constrain-draft): the draft rows get the allowed set, bias, bad words and guide too."""
+    constrain_draft (--constrain-draft): the draft rows get the allowed set, bias, bad words and guide too.
+    prompt_logprobs: every prompt's prompt_logprobs setting (--prompt-logprobs, None = off); the mean logprob of each
+    prompt's own tokens after the first and its perplexity exp(-mean) are printed and returned; refill admissions keep
+    it."""
     from sequoia_b200.batch import BatchTree
     steps = decoded = 0                          # steps: target steps summed over sequences (per-sequence tokens / step)
     total_time = 0.0
@@ -308,6 +324,7 @@ def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: i
     chunks = [prompts[:B]] if refill else [prompts[i:i + B] for i in range(0, len(prompts), B)]
     dstop = device_stop_settings(prompts, stop) if device_stop else None
     means = None if logprobs is None else [float("nan")] * len(prompts)
+    pmeans = None if prompt_logprobs is None else [float("nan")] * len(prompts)
     for c, chunk in enumerate(chunks):
         i0 = c * B
         pol = policy if policies is None else policies[i0:i0 + len(chunk)]
@@ -316,6 +333,8 @@ def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: i
         kw.update(bad_words or {})
         if logprobs is not None:
             kw["logprobs"] = logprobs
+        if prompt_logprobs is not None:
+            kw["prompt_logprobs"] = prompt_logprobs
         if dstop is not None:
             kw.update(stop_tokens=dstop[0][i0:i0 + len(chunk)], max_new_tokens=dstop[1][i0:i0 + len(chunk)])
         tree = BatchTree(draft, target, chunk, grow_map, policy=pol, temperature=T, top_p=top_p, max_length=M,
@@ -325,9 +344,10 @@ def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: i
         t1 = time.time()
         if refill:
             _, d, s, _ = decode_refill(tree, prompts, limits, stop, seeds=seeds, policies=policies, device_stop=dstop,
-                                       logprob_means=means)
+                                       logprob_means=means, prompt_logprob_means=pmeans)
         else:
-            d, s = decode_chunk(tree, chunk, limits[:len(chunk)], stop, logprob_means=means, i0=i0)
+            d, s = decode_chunk(tree, chunk, limits[:len(chunk)], stop, logprob_means=means, i0=i0,
+                                prompt_logprob_means=pmeans)
         decoded += d
         steps += s
         torch.cuda.synchronize()
@@ -345,6 +365,11 @@ def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: i
         for i, m in enumerate(means):
             print(f"prompt {i}: mean token logprob {m:.4f}")
         res["mean_token_logprob"] = means
+    if pmeans is not None:
+        ppl = [math.exp(-m) for m in pmeans]
+        for i, (m, p) in enumerate(zip(pmeans, ppl)):
+            print(f"prompt {i}: mean prompt-token logprob {m:.4f}, perplexity {p:.3f}")
+        res["mean_prompt_logprob"], res["prompt_perplexity"] = pmeans, ppl
     return res
 
 
@@ -397,6 +422,9 @@ def build_parser():
                     help="with --batch: vLLM's presence penalty of every prompt (0 = off), on the target rows")
     ap.add_argument("--logprobs", type=int, default=None,
                     help="with --batch: the top alternatives per token (0..20); prints each prompt's mean token logprob")
+    ap.add_argument("--prompt-logprobs", type=int, default=None,
+                    help="with --batch: the top alternatives per prompt token (0..20); prints each prompt's mean "
+                         "prompt-token logprob and perplexity under the target")
     ap.add_argument("--logit-bias", type=str, default=None,
                     help="with --batch: ID:BIAS[,ID:BIAS...], added to every prompt's target logits (bias in [-100, 100])")
     ap.add_argument("--allowed-token-ids", type=str, default=None,
@@ -490,6 +518,21 @@ def batch_penalties(args) -> dict:
         raise SystemExit("--repetition-penalty / --frequency-penalty / --presence-penalty run with --batch (the batched "
                          "tree); the lone trees keep the reference's sampling")
     return vals
+
+
+def batch_prompt_logprobs(args):
+    """--prompt-logprobs N: every prompt's prompt_logprobs setting (None = off).  Refused outside 0..20, and without
+    --batch: the lone trees score no prompt."""
+    if args.prompt_logprobs is None:
+        return None
+    from sequoia_b200.batch import check_prompt_logprobs
+    try:
+        n = check_prompt_logprobs(args.prompt_logprobs)
+    except ValueError as e:
+        raise SystemExit(f"--prompt-logprobs: {e}")
+    if args.batch == 1 and not args.refill:
+        raise SystemExit("--prompt-logprobs runs with --batch (the batched tree); the lone trees score no prompt")
+    return n
 
 
 def batch_logprobs(args):
@@ -597,6 +640,7 @@ def main(argv=None):
     device_stop = batch_device_stop(args)
     penalties = batch_penalties(args)
     logprobs = batch_logprobs(args)
+    prompt_logprobs = batch_prompt_logprobs(args)
     logit_bias = batch_logit_bias(args)
     bad_words = batch_bad_words(args)
     constrain_draft = batch_constrain_draft(args)
@@ -613,7 +657,7 @@ def main(argv=None):
                                refill=args.refill, seeds=seeds, policies=policies, top_k=top_k,
                                device_stop=device_stop, penalties=penalties, logprobs=logprobs,
                                logit_bias=logit_bias, min_p=min_p, bad_words=bad_words,
-                               constrain_draft=constrain_draft)
+                               constrain_draft=constrain_draft, prompt_logprobs=prompt_logprobs)
         print(json.dumps({k: (round(v, 5) if isinstance(v, float) else v) for k, v in res.items()}))
         return res
     target = (tcls(max_length=args.M, model_name_or_path=args.target, dtype=torch.float16, device=DEV)
