@@ -352,6 +352,13 @@ int sq_rope_kv_append_batch(sq_half* qkv, int ld, int H, int Hkv, int D, const s
  * accept_idx row); tail rows are left stale as in sq_kv_gather with state */
 int sq_kv_gather_batch(sq_half* k_cache, sq_half* v_cache, int L, int B, int Hkv, int M, int D, const int32_t* accept_idx,
                        int ld_idx, const int32_t* state, int max_n, void* stream);
+/* prefix reuse: copy rows [0, n) of sequence src to the same rows of sequence dst, K and V of every layer and kv head, in
+ * one launch (grid (L*Hkv, 2, chunks), 16-byte loads and stores, no shared memory).  Every other byte of both caches,
+ * dst's rows >= n included, is left as it was.  Refused with SQ_ERR_INVALID_ARG before any launch: a null or not 16-byte
+ * aligned cache, L or Hkv < 1, D % 8 != 0, B outside 1..SQ_MAX_BATCH, src or dst outside [0, B), src == dst, n outside
+ * 1..M. */
+int sq_kv_copy_prefix(sq_half* k_cache, sq_half* v_cache, int L, int B, int Hkv, int M, int D, int src, int dst, int n,
+                      void* stream);
 /* attention plan over a (L, B, Hkv, M, D) cache; q / out hold B*n rows (n_max counts all of them) */
 int sq_attn_plan_create_batch(sq_attn_plan** plan, const sq_half* q, int ld, int n_max, int H, int Hkv, int D,
                               const sq_half* k_cache, const sq_half* v_cache, int L, int B, int M, sq_half* out,

@@ -97,6 +97,7 @@ _SIGNATURES = {
     "sq_embed_rows_batch": (i32, [vp, vp, i64, vp, i32, i32, i32, i32, vp, vp]),
     "sq_rope_kv_append_batch": (i32, [vp, i32, i32, i32, i32, vp, vp, vp, vp, i64, vp, i32, i32, i32, vp, vp, i32, vp]),
     "sq_kv_gather_batch": (i32, [vp, vp, i32, i32, i32, i32, i32, vp, i32, vp, i32, vp]),
+    "sq_kv_copy_prefix": (i32, [vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, vp]),
     "sq_attn_plan_create_batch": (i32, [C.POINTER(vp), vp, i32, i32, i32, i32, i32, vp, vp, i32, i32, i32, vp, vp, i64]),
     "sq_tree_attn_batch": (i32, [vp, i32, i32, i32, vp, i32, i32, vp, i32, i32, vp]),
     "sq_sample_level_batch": (i32, [vp, i64, vp, vp, vp, i64, i64, vp, vp, vp, i32, i32, i32, f32, i32, vp, i64, vp, i32,

@@ -95,6 +95,13 @@ children, an all -inf row, or a NaN sampling key); the stochastic walks never ac
 (SQ_ACCEPT_SKIP_DEAD), so speculative sampling stays exact.  A seeded sequence commits a different, equally distributed
 output than without it; greedy sequences commit the same.  While every slot is neutral nothing is launched; when a
 constraint kind starts, the draft graph is captured once more along with the steady and post graphs.
+
+Prefix reuse: admit(..., reuse_prefix=True) looks for the longest prefix of the new prompt (at most P - 1 tokens) that a
+slot's ready prefix holds, the first target_kv_len[d] tokens of slot d, whose K/V both caches hold and no later step
+rewrites.  Rows [0, L) are copied from the donor into the slot's rows of both caches (sq_kv_copy_prefix, one launch per
+cache; none when the donor is the slot itself), and the draft prefill and first verify run rows [L, ...) only.  This is
+eager admission work: the captured graphs are the same with or without it.  The copied rows are the donor's bytes, which
+a forward of another shape computed, so the result matches a full prefill up to fp16 rounding, not bit for bit.
 """
 from __future__ import annotations
 
@@ -531,6 +538,35 @@ def _guides(guide, B: int) -> List[Optional[TokenGuide]]:
     return [check_guide(guide)] * B
 
 
+def check_reuse_prefix(reuse_prefix) -> bool:
+    """admit()'s reuse_prefix: a bool."""
+    if not isinstance(reuse_prefix, bool):
+        raise ValueError(f"reuse_prefix must be a bool, got {reuse_prefix!r}")
+    return reuse_prefix
+
+
+def prefix_donor(prompt: torch.Tensor, rows: torch.Tensor, ready: Sequence[int], b: int,
+                 prompt_logprobs: Optional[int] = None):
+    """The prefix an admission into slot b reuses (host tensors): slot d offers its first ready[d] tokens rows[d] (whose
+    K/V both caches hold); L is the longest common prefix of the prompt with any of them, capped at len(prompt) - 1 (the
+    last prompt row always runs: it gives node 0's draft logits and the first verify's root).  The largest L wins; on a
+    tie slot b itself (no copy), then the lowest index.  A slot with prompt_logprobs on reuses nothing (its rows below L
+    would get no values).  -> (donor, L), or (None, 0)."""
+    P = len(prompt)
+    if prompt_logprobs is not None or P < 2:
+        return None, 0
+    best, best_len = None, 0
+    for d in [b] + [d for d in range(len(ready)) if d != b]:
+        m = min(int(ready[d]), P - 1)
+        if m <= best_len:
+            continue
+        diff = (rows[d, :m] != prompt[:m]).nonzero()
+        n = m if len(diff) == 0 else int(diff[0])
+        if n > best_len:
+            best, best_len = d, n
+    return best, best_len
+
+
 def check_seed(seed) -> int:
     """A per-sequence seed: an integer in [0, 2^64)."""
     if isinstance(seed, bool) or not isinstance(seed, numbers.Integral):
@@ -670,6 +706,9 @@ class BatchTree:
             if len(p) + S - 1 > M:
                 raise ValueError(f"max_length={M} must hold the prompt ({len(p)}) + tree ({S}) - 1")
         self.device = dev
+        # prefix reuse: (donor slot, L) of each slot's current prompt when its admission took rows [0, L) of K/V from a
+        # slot's ready prefix (admit(reuse_prefix=True)), else None; the draft prefill and first verify start at row L
+        self.reused_prefix: List[Optional[tuple]] = [None] * B
         # constrained drafting: every draft row a sampler reads gets its sequence's allowed set, logit bias, bad words and
         # guide, as its target row does, inside the draft graph; the walks then skip dead children (SQ_ACCEPT_SKIP_DEAD)
         self.constrain_draft = constrain_draft
@@ -946,12 +985,43 @@ class BatchTree:
         self.state[b].copy_(_h2d(st0), non_blocking=True)
         self.accept_idx[b].zero_()
 
+    def _prefill_start(self, b: int) -> int:
+        """The first prompt row slot b's draft prefill and first verify run: L of a reused prefix, else 0."""
+        reused = self.reused_prefix[b]
+        return 0 if reused is None else reused[1]
+
     def op_draft_prefill(self, seqs):
-        """Draft prefill of the sequences `seqs` (SpecTree.py:67-80) as one ragged forward: each one's rows [0, P) causal,
-        its last row's logits -> its node 0."""
-        self.draft.engine.runner.forward_ragged(
-            [(b, self.ground_truth_len[b], 1 - self.ground_truth_len[b], 1, 1, self.draft_logits[b:b + 1]) for b in seqs],
-            self.tokens, self.position_ids, self.storage_ids, state=self.state, **self._mask_kw())
+        """Draft prefill of the sequences `seqs` (SpecTree.py:67-80) as one ragged forward: each one's rows [L, P) causal
+        (L = 0 unless its admission reused a prefix), its last row's logits -> its node 0."""
+        parts = []
+        for b in seqs:
+            P, L = self.ground_truth_len[b], self._prefill_start(b)
+            parts.append((b, P - L, 1 - P + L, 1, 1, self.draft_logits[b:b + 1]))
+        self.draft.engine.runner.forward_ragged(parts, self.tokens, self.position_ids, self.storage_ids, state=self.state,
+                                                **self._mask_kw())
+
+    def _reuse_prefix(self, b: int, prompt: torch.Tensor):
+        """Find the prefix an admission of `prompt` into slot b reuses (prefix_donor over every slot's ready prefix
+        tokens[d, :target_kv_len[d]], read back in one device-to-host copy) and copy its K/V rows from another slot into
+        b's, in both caches.  Runs before slot b's token row is reloaded.  -> (donor, L) or None."""
+        P = len(prompt)
+        m = min(P - 1, max(self.target_kv_len))
+        if m < 1 or self.prompt_logprobs_n[b] is not None:
+            return None
+        # (L <= m, so the prompt's first m + 1 tokens give the same donor and L as the whole prompt; on the device they
+        # travel with the rows, in the same copy)
+        if prompt.is_cuda:
+            both = torch.cat([self.tokens[:, :m + 1], prompt[None, :m + 1].to(torch.int64)]).cpu()
+            rows, head = both[:self.B], both[self.B]
+        else:
+            rows, head = self.tokens[:, :m].cpu(), prompt[:m + 1]
+        donor, L = prefix_donor(head, rows, self.target_kv_len, b, self.prompt_logprobs_n[b])
+        if L == 0:
+            return None
+        if donor != b:
+            for eng in (self.draft, self.target):
+                ops.kv_copy_prefix(eng.engine.kv_cache, donor, b, L)
+        return donor, L
 
     def freeze(self, b: int):
         """Stop sequence b (the caller's length limit); it stays frozen until admit() gives the slot a new prompt."""
@@ -964,7 +1034,8 @@ class BatchTree:
               stop_tokens=_PREVIOUS, max_new_tokens=_PREVIOUS, repetition_penalty: Optional[float] = None,
               frequency_penalty: Optional[float] = None, presence_penalty: Optional[float] = None,
               logprobs=_PREVIOUS, logit_bias=_PREVIOUS, allowed_token_ids=_PREVIOUS, min_p: Optional[float] = None,
-              bad_words=_PREVIOUS, min_tokens=_PREVIOUS, guide=_PREVIOUS, prompt_logprobs=_PREVIOUS):
+              bad_words=_PREVIOUS, min_tokens=_PREVIOUS, guide=_PREVIOUS, prompt_logprobs=_PREVIOUS,
+              reuse_prefix: bool = False):
         """Start `prompt` in the frozen slot b (finished, out of room, or stopped with freeze), at its own policy,
         temperature, top_p and top_k (default: the slot's previous values).  The next verify() runs its first verify next
         to the steady sequences.  The slot draws r and rand as a lone SpecTree on the prompt would, and runs its draft
@@ -993,7 +1064,21 @@ class BatchTree:
         min_tokens counts from this prompt.  The first non-neutral one, in a tree without one, captures the steady and post
         graphs once more.
         guide: the prompt's guide (default: the slot's previous one; None is none), which starts at its start state.  The
-        first guide, in a tree without one, captures the steady and post graphs once more."""
+        first guide, in a tree without one, captures the steady and post graphs once more.
+        reuse_prefix: a bool (default False).  With True the prompt reuses the longest prefix whose K/V a slot already
+        holds (prefix_donor): slot d offers its first target_kv_len[d] tokens, its ready prefix, which is 0 until its
+        current prompt's first verify, then the committed length minus the bonus token after each verify that leaves it
+        decoding, and unchanged by the verify that ends it (the rows below that step's start are never rewritten).  Slot
+        b itself is a candidate: its previous occupant's rows are still there (multi-turn chat: the finished output plus
+        a new turn).  With L >= 1 reused rows from another slot, sq_kv_copy_prefix copies them into b's rows of the draft
+        and the target cache; the draft prefill then runs rows [L, P) and the first verify rows [L, P + S - 1).  L is at
+        most P - 1, and 0 for a slot with prompt_logprobs on.  reused_prefix[b] reports (donor, L), or None.  A slot
+        admitted since the last verify() is no donor (its ready length is 0): to fan one prompt out to several slots
+        (parallel sampling), admit it once, run one verify(), then admit the copies with reuse_prefix=True.  The reused
+        rows hold the donor's bytes, computed by a forward of another shape, so the admission matches a full prefill up
+        to fp16 rounding, not bit for bit; a seeded "spec" slot may commit a different, equally distributed output.
+        No graph is captured again."""
+        check_reuse_prefix(reuse_prefix)
         if policy is not None:
             check_policy(policy)
         if top_k is not None:
@@ -1133,6 +1218,7 @@ class BatchTree:
         if pol == "spec" and self.r is None:       # the first sampling sequence of a tree built all-greedy
             self.r = torch.zeros(self.B, self.M, dtype=F16, device=self.device)
             self.rand = torch.zeros(self.B, self.S, self.V, dtype=F16, device=self.device)
+        self.reused_prefix[b] = self._reuse_prefix(b, prompt) if reuse_prefix else None   # (the copies first)
         self._load_prompt(b, prompt)
         self.frozen[b] = False
         self.finish_reason[b] = None
@@ -1176,13 +1262,17 @@ class BatchTree:
                                           **self._mask_kw())
 
     def op_target_first(self, seqs):
-        """First verify of the sequences `seqs` (SpecTree.py:164-176) as one ragged forward: each one's rows [0, P+S-1),
-        the logits of its S tree rows.  Then the prompt logprobs of those with the setting on (op_prompt_logprobs)."""
+        """First verify of the sequences `seqs` (SpecTree.py:164-176) as one ragged forward: each one's rows [L, P+S-1)
+        (L = 0 unless its admission reused a prefix), the logits of its S tree rows.  Then the prompt logprobs of those
+        with the setting on (op_prompt_logprobs; their L is 0)."""
         S = self.S
         runner = self.target.engine.runner
-        row0 = runner.forward_ragged(
-            [(b, self.ground_truth_len[b] + S - 1, 1 - self.ground_truth_len[b], S, S,
-              self.target_logits[b * S:(b + 1) * S]) for b in seqs], self.tokens, self.position_ids, self.storage_ids, state=self.state, **self._mask_kw())
+        parts = []
+        for b in seqs:
+            P, L = self.ground_truth_len[b], self._prefill_start(b)
+            parts.append((b, P - L + S - 1, 1 - P + L, S, S, self.target_logits[b * S:(b + 1) * S]))
+        row0 = runner.forward_ragged(parts, self.tokens, self.position_ids, self.storage_ids, state=self.state,
+                                     **self._mask_kw())
         self.op_prompt_logprobs(seqs, row0)
 
     def op_prompt_logprobs(self, seqs, row0):

@@ -70,6 +70,36 @@ __global__ void kv_gather_scratch_kernel(__half* __restrict__ k_cache, __half* _
   }
 }
 
+// Prefix copy between two sequences of a (L, B, Hkv, M, D) cache: rows [0, n) of each (layer, kv-head) plane of sequence
+// src to the same rows of sequence dst.  Those rows are one contiguous run of n*D/8 16-byte words per plane, so a plane
+// is a flat copy.  grid (L*Hkv, K|V, chunks); a CTA moves COPY_ITEMS words per thread per pass, all loads before the
+// stores, and strides over its plane by gridDim.z chunks.
+constexpr int COPY_ITEMS = 4;
+
+__global__ void kv_copy_prefix_kernel(__half* __restrict__ k_cache, __half* __restrict__ v_cache, int B, int Hkv, int M,
+                                      int D, int src, int dst, int n) {
+  const int l = blockIdx.x / Hkv, h = blockIdx.x % Hkv;
+  __half* cache = blockIdx.y == 0 ? k_cache : v_cache;
+  const int64_t plane = (int64_t)M * D;
+  const uint4* s = reinterpret_cast<const uint4*>(cache + ((int64_t)(l * B + src) * Hkv + h) * plane);
+  uint4* d = reinterpret_cast<uint4*>(cache + ((int64_t)(l * B + dst) * Hkv + h) * plane);
+  const int64_t words = (int64_t)n * D / 8;
+  const int64_t chunk = (int64_t)blockDim.x * COPY_ITEMS;
+  for (int64_t base = blockIdx.z * chunk + threadIdx.x; base < words; base += gridDim.z * chunk) {
+    uint4 v[COPY_ITEMS];
+#pragma unroll
+    for (int i = 0; i < COPY_ITEMS; ++i) {
+      const int64_t j = base + (int64_t)i * blockDim.x;
+      if (j < words) v[i] = s[j];
+    }
+#pragma unroll
+    for (int i = 0; i < COPY_ITEMS; ++i) {
+      const int64_t j = base + (int64_t)i * blockDim.x;
+      if (j < words) d[j] = v[i];
+    }
+  }
+}
+
 }  // namespace sq
 
 using namespace sq;
@@ -126,6 +156,27 @@ extern "C" int sq_kv_gather_batch(sq_half* k_cache, sq_half* v_cache, int L, int
                                      (cudaStream_t)stream);
   if (rc) return rc;
   SQ_CHECK_LAUNCH("sq_kv_gather_batch");
+  return SQ_OK;
+}
+
+extern "C" int sq_kv_copy_prefix(sq_half* k_cache, sq_half* v_cache, int L, int B, int Hkv, int M, int D, int src,
+                                 int dst, int n, void* stream) {
+  SQ_CHECK_ARG(k_cache != nullptr && v_cache != nullptr, "sq_kv_copy_prefix: null cache");
+  SQ_CHECK_ARG(((uintptr_t)k_cache | (uintptr_t)v_cache) % 16 == 0, "sq_kv_copy_prefix: caches not 16-byte aligned");
+  SQ_CHECK_ARG(L >= 1 && Hkv >= 1 && D >= 8 && D % 8 == 0, "sq_kv_copy_prefix: bad shape L=%d Hkv=%d D=%d (D %% 8 == 0)",
+               L, Hkv, D);
+  SQ_CHECK_ARG(B >= 1 && B <= SQ_MAX_BATCH, "sq_kv_copy_prefix: B=%d outside 1..%d", B, SQ_MAX_BATCH);
+  SQ_CHECK_ARG(src >= 0 && src < B && dst >= 0 && dst < B && src != dst,
+               "sq_kv_copy_prefix: src=%d / dst=%d must be distinct sequences in [0, %d)", src, dst, B);
+  SQ_CHECK_ARG(n >= 1 && n <= M, "sq_kv_copy_prefix: n=%d rows outside 1..M=%d", n, M);
+  // one 16-byte word per thread and pass: a short copy gets warp-sized CTAs, one per plane; a long one 256 threads and
+  // as many chunks of 256 * COPY_ITEMS words as its planes hold
+  const int64_t words = (int64_t)n * D / 8;
+  const int threads = (int)(words >= 256 ? 256 : (words + 31) / 32 * 32);
+  const int64_t chunks = (words + (int64_t)threads * COPY_ITEMS - 1) / ((int64_t)threads * COPY_ITEMS);
+  kv_copy_prefix_kernel<<<dim3(L * Hkv, 2, (unsigned)(chunks < 65535 ? chunks : 65535)), threads, 0,
+                          (cudaStream_t)stream>>>((__half*)k_cache, (__half*)v_cache, B, Hkv, M, D, src, dst, n);
+  SQ_CHECK_LAUNCH("sq_kv_copy_prefix");
   return SQ_OK;
 }
 

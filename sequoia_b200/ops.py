@@ -432,6 +432,16 @@ def kv_gather_batch(k_cache, v_cache, accept_idx, state, max_n):
           "sq_kv_gather_batch")
 
 
+def kv_copy_prefix(kv_cache, src: int, dst: int, n: int):
+    """Rows [0, n) of sequence src's K and V, every layer, into sequence dst's of the same (L, B, Hkv, M, D) cache
+    (an object with k_cache / v_cache, as KV_Cache); one launch."""
+    k, v = kv_cache.k_cache, kv_cache.v_cache
+    assert k.shape == v.shape and k.dtype == v.dtype == torch.float16 and k.is_contiguous() and v.is_contiguous()
+    L, B, Hkv, M, D = k.shape
+    check(_lib.load().sq_kv_copy_prefix(ptr(k), ptr(v), L, B, Hkv, M, D, int(src), int(dst), int(n), stream_ptr()),
+          "sq_kv_copy_prefix")
+
+
 def tree_attn_batch(plan: AttnPlan, layer, n, *, state, n0=0, kv_end=0, tree_bits=None, tree_words=0, tree_size=0):
     check(_lib.load().sq_tree_attn_batch(plan.handle, layer, n, state.shape[0], ptr(state), n0, kv_end, ptr(tree_bits),
                                          tree_words, tree_size, stream_ptr()), "sq_tree_attn_batch")

@@ -212,7 +212,7 @@ def _record_prompt_logprobs(tree, b: int, i: int, means):
 
 
 def decode_refill(tree, prompts, limits, stop=DEFAULT_STOP, step_times=None, seeds=None, policies=None,
-                  device_stop=None, logprob_means=None, prompt_logprob_means=None):
+                  device_stop=None, logprob_means=None, prompt_logprob_means=None, reused=None):
     """Decode every prompt of a queue on a BatchTree whose B slots start with prompts[:B]: each slot that finishes (a stop
     token, its length limit `limits[i]`, or out of room) takes the next prompt, until the queue is empty.
     -> (outputs, decoded tokens, per-sequence target steps, admission order); outputs[i] = prompt i's committed tokens.
@@ -221,7 +221,9 @@ def decode_refill(tree, prompts, limits, stop=DEFAULT_STOP, step_times=None, see
     policies: prompt i decodes with policies[i] ("spec" / "greedy"); None keeps each slot's policy.
     device_stop: (stop_tokens, max_new_tokens) per prompt (device_stop_settings), passed to each admission; None keeps
     each slot's.  logprob_means: a list that receives prompt i's mean token logprob at index i (--logprobs).
-    prompt_logprob_means: the same for the mean logprob of prompt i's own tokens (--prompt-logprobs)."""
+    prompt_logprob_means: the same for the mean logprob of prompt i's own tokens (--prompt-logprobs).
+    reused: a list that receives the prompt tokens each admission reused from a slot's cached prefix; admissions then
+    pass reuse_prefix=True (--reuse-prefix).  None: admit without it."""
     B = len(tree.frozen)
     slot = list(range(B))                        # prompt index decoding in each slot (None: the queue ran out)
     length = [len(p) for p in prompts[:B]]
@@ -238,7 +240,11 @@ def decode_refill(tree, prompts, limits, stop=DEFAULT_STOP, step_times=None, see
                 kw["policy"] = policies[slot[b]]
             if device_stop is not None:
                 kw["stop_tokens"], kw["max_new_tokens"] = device_stop[0][slot[b]], device_stop[1][slot[b]]
+            if reused is not None:
+                kw["reuse_prefix"] = True
             tree.admit(b, prompts[slot[b]], **kw)
+            if reused is not None:
+                reused.append(0 if tree.reused_prefix[b] is None else tree.reused_prefix[b][1])
         kind = "admission" if pending else "steady"
         pending = []
         tree.construct_grow_map()
@@ -299,7 +305,7 @@ def decode_chunk(tree, chunk, limits, stop=DEFAULT_STOP, logprob_means=None, i0:
 def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: int, stop=DEFAULT_STOP,
                      refill: bool = False, seeds=None, policies=None, top_k: int = 0, device_stop: bool = False,
                      penalties=None, logprobs=None, logit_bias=None, min_p: float = 0.0, bad_words=None,
-                     constrain_draft: bool = False, prompt_logprobs=None):
+                     constrain_draft: bool = False, prompt_logprobs=None, reuse_prefix: bool = False):
     """--batch B: the same metric loop with B prompts decoded together (sequoia_b200.batch.BatchTree).  Chunked: B
     prompts at a time, each chunk until its last sequence stops.  refill: one batch whose finished slots take the next
     prompt (BatchTree.admit).  seeds: one per prompt (--device-rng): each sequence draws its random numbers on the device
@@ -315,7 +321,8 @@ def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: i
     constrain_draft (--constrain-draft): the draft rows get the allowed set, bias, bad words and guide too.
     prompt_logprobs: every prompt's prompt_logprobs setting (--prompt-logprobs, None = off); the mean logprob of each
     prompt's own tokens after the first and its perplexity exp(-mean) are printed and returned; refill admissions keep
-    it."""
+    it.  reuse_prefix: every refill admission reuses the longest cached prefix of its prompt (--reuse-prefix); the total
+    of reused prompt tokens is printed and returned."""
     from sequoia_b200.batch import BatchTree
     steps = decoded = 0                          # steps: target steps summed over sequences (per-sequence tokens / step)
     total_time = 0.0
@@ -325,6 +332,7 @@ def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: i
     dstop = device_stop_settings(prompts, stop) if device_stop else None
     means = None if logprobs is None else [float("nan")] * len(prompts)
     pmeans = None if prompt_logprobs is None else [float("nan")] * len(prompts)
+    reused = [] if reuse_prefix else None
     for c, chunk in enumerate(chunks):
         i0 = c * B
         pol = policy if policies is None else policies[i0:i0 + len(chunk)]
@@ -344,7 +352,7 @@ def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: i
         t1 = time.time()
         if refill:
             _, d, s, _ = decode_refill(tree, prompts, limits, stop, seeds=seeds, policies=policies, device_stop=dstop,
-                                       logprob_means=means, prompt_logprob_means=pmeans)
+                                       logprob_means=means, prompt_logprob_means=pmeans, reused=reused)
         else:
             d, s = decode_chunk(tree, chunk, limits[:len(chunk)], stop, logprob_means=means, i0=i0,
                                 prompt_logprob_means=pmeans)
@@ -370,6 +378,9 @@ def simulation_batch(target, draft, prompts, grow_map, policy, T, top_p, M, B: i
         for i, (m, p) in enumerate(zip(pmeans, ppl)):
             print(f"prompt {i}: mean prompt-token logprob {m:.4f}, perplexity {p:.3f}")
         res["mean_prompt_logprob"], res["prompt_perplexity"] = pmeans, ppl
+    if reused is not None:
+        print(f"reused prompt tokens: {sum(reused)} in {len(reused)} admissions")
+        res["reused_prompt_tokens"] = sum(reused)
     return res
 
 
@@ -425,6 +436,9 @@ def build_parser():
     ap.add_argument("--prompt-logprobs", type=int, default=None,
                     help="with --batch: the top alternatives per prompt token (0..20); prints each prompt's mean "
                          "prompt-token logprob and perplexity under the target")
+    ap.add_argument("--reuse-prefix", action="store_true",
+                    help="with --batch --refill: each admission copies the longest prefix of its prompt whose K/V a "
+                         "slot already holds and prefills only the rest; prints the reused prompt tokens")
     ap.add_argument("--logit-bias", type=str, default=None,
                     help="with --batch: ID:BIAS[,ID:BIAS...], added to every prompt's target logits (bias in [-100, 100])")
     ap.add_argument("--allowed-token-ids", type=str, default=None,
@@ -598,6 +612,14 @@ def batch_constrain_draft(args) -> bool:
     return bool(args.constrain_draft)
 
 
+def batch_reuse_prefix(args) -> bool:
+    """--reuse-prefix: admit(reuse_prefix=True) for every refill admission.  Refused without --refill: only admissions
+    reuse a prefix (a tree's first prompts have none cached)."""
+    if args.reuse_prefix and not args.refill:
+        raise SystemExit("--reuse-prefix runs with --refill (admissions reuse cached prefixes; a new tree has none)")
+    return bool(args.reuse_prefix)
+
+
 def batch_bad_words(args) -> dict:
     """--bad-words ID,ID,...;ID;... / --min-tokens N: BatchTree's bad_words / min_tokens for every prompt ({} when
     neither is given).  Refused when malformed or outside what BatchTree takes (ids are checked against the vocabulary
@@ -644,6 +666,7 @@ def main(argv=None):
     logit_bias = batch_logit_bias(args)
     bad_words = batch_bad_words(args)
     constrain_draft = batch_constrain_draft(args)
+    reuse_prefix = batch_reuse_prefix(args)
     if args.batch != 1 or args.refill:
         B = check_batch_args(args, len(prompts))
         target = GraphInferenceEngineTG(max_length=args.M, model_name_or_path=args.target, dtype=torch.float16,
@@ -657,7 +680,8 @@ def main(argv=None):
                                refill=args.refill, seeds=seeds, policies=policies, top_k=top_k,
                                device_stop=device_stop, penalties=penalties, logprobs=logprobs,
                                logit_bias=logit_bias, min_p=min_p, bad_words=bad_words,
-                               constrain_draft=constrain_draft, prompt_logprobs=prompt_logprobs)
+                               constrain_draft=constrain_draft, prompt_logprobs=prompt_logprobs,
+                               reuse_prefix=reuse_prefix)
         print(json.dumps({k: (round(v, 5) if isinstance(v, float) else v) for k, v in res.items()}))
         return res
     target = (tcls(max_length=args.M, model_name_or_path=args.target, dtype=torch.float16, device=DEV)
